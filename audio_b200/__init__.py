@@ -1,4 +1,4 @@
-"""audio_b200 -- B200-native (sm_100a) implementation of torchaudio's DSP front-end hot path.
+"""audio_b200 -- H100-native (sm_90a) implementation of torchaudio's DSP front-end hot path.
 
     import audio_b200.transforms as T          # Spectrogram, MelSpectrogram, MFCC, LFCC, Resample, InverseSpectrogram,
                                                # GriffinLim, TimeStretch, PitchShift, Speed, ...

@@ -5,7 +5,7 @@ Every function here has a C twin exported from ``libb200audio.so``
 ``b200a_resample_width``, ``b200a_pad_index``); ``tests/test_bookkeeping.py``
 checks both against the reference's shapes bit-exactly (tests/golden/ref_integers.npz).
 
-Reference call sites (relative to /root/reference):
+Reference call sites (relative to pytorch/audio):
   * frame count      -- torch.stft as called at src/torchaudio/functional/functional.py:123-134
   * resample lengths -- src/torchaudio/functional/functional.py:1359, 1424-1428
 """

@@ -1,8 +1,8 @@
-"""In-tree build of libb200audio.so with nvcc for sm_100a (no torch headers, no JIT cache).
+"""In-tree build of libb200audio.so with nvcc for sm_90a (H100; no torch headers, no JIT cache).
 
 ``python -m audio_b200._build`` (or ``__graft_entry__.build()``) compiles every ``csrc/*.cu``
 into ``audio_b200/lib/libb200audio.so``.  The shared object is git-ignored but travels with
-the working tree, so a GPU box only ever loads the prebuilt file.
+the working tree, so a GPU machine only ever loads the prebuilt file.
 """
 from __future__ import annotations
 
@@ -21,8 +21,9 @@ OBJ_DIR = os.path.join(PKG_DIR, "build")
 LIB_PATH = os.path.join(LIB_DIR, "libb200audio.so")
 STAMP = os.path.join(LIB_DIR, "libb200audio.stamp")
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
@@ -83,10 +84,10 @@ def build(force: bool = False, verbose: bool = True) -> str:
     os.makedirs(OBJ_DIR, exist_ok=True)
     srcs = _sources()
     if verbose:
-        print(f"[audio_b200] nvcc sm_100a build of {len(srcs)} files -> {LIB_PATH}", file=sys.stderr)
+        print(f"[audio_b200] nvcc sm_90a build of {len(srcs)} files -> {LIB_PATH}", file=sys.stderr)
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(srcs))) as pool:
         objs = list(pool.map(lambda s: _compile_one(nvcc, s, OBJ_DIR), srcs))
-    link = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH, *objs]
+    link = [nvcc, *GENCODE, "-shared", "-o", LIB_PATH, *objs]
     proc = subprocess.run(link, capture_output=True, text=True)
     if proc.returncode != 0:
         raise RuntimeError(f"link failed:\n{proc.stdout}\n{proc.stderr}")

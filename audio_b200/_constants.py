@@ -6,7 +6,7 @@ CPU op sequence and dtypes as the reference so the resulting buffers are bit-ide
 and ``state_dict``s interchange with torchaudio's (tests/test_constants.py checks this
 against tests/golden/ref_cases.npz).
 
-Reference (relative to /root/reference/src/torchaudio/functional/functional.py):
+Reference (relative to pytorch/audio/src/torchaudio/functional/functional.py):
   melscale_fbanks 518-587 (+ _hz_to_mel 425-455, _mel_to_hz 458-489, triangles 492-515),
   create_dct 636-667, _get_sinc_resample_kernel 1305-1402.
 """

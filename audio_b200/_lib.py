@@ -74,8 +74,6 @@ _SIGNATURES = {
     "b200a_resample_width": (c_int32, [c_int32, c_int32, c_int32, c_double]),
     "b200a_resample_len": (c_int64, [c_int64, c_int32, c_int32]),
     "b200a_resample_support": (ctypes.c_int, [c_int32, c_int32, c_int32, c_double, c_int32, POINTER(c_int32), POINTER(c_int32)]),
-    "b200a_resample_plan_info": (ctypes.c_int, [c_int32, c_int32, c_int32, POINTER(c_int32)]),
-    "b200a_resample_tc_band": (ctypes.c_int, [c_int32, c_int32, c_int32, c_int32, POINTER(c_int32), POINTER(c_int32)]),
     "b200a_frontend_workspace_bytes": (c_size_t, [POINTER(FrontendDesc)]),
     "b200a_frontend_prepare": (
         ctypes.c_int,
@@ -146,7 +144,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing. Build it with `python -m audio_b200._build` "
-                "(nvcc, sm_100a). audio_b200 has no CPU or ATen fallback."
+                "(nvcc, sm_90a). audio_b200 has no CPU or ATen fallback."
             )
         handle = ctypes.CDLL(LIB_PATH)
         for name, (restype, argtypes) in _SIGNATURES.items():

@@ -2,8 +2,7 @@
 
 Pinned host buffers that feed a GPU over PCIe should live on the socket the GPU hangs off: with one
 process per GPU and no binding, ``pin_memory()`` lands wherever the rank happened to be scheduled and
-half the ranks of an 8-GPU box pull their waveforms across the inter-socket link (the 0.48 end-to-end
-scaling efficiency of round 1).  No dependency beyond sysfs; a no-op when the topology cannot be read.
+half the ranks of a two-socket, 8-GPU machine pull their waveforms across the inter-socket link.  No dependency beyond sysfs; a no-op when the topology cannot be read.
 """
 from __future__ import annotations
 

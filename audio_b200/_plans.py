@@ -19,7 +19,7 @@ def _require_cuda_f32(t: torch.Tensor, what: str) -> None:
         raise TypeError(f"{what} must be a torch.Tensor")
     if not t.is_cuda:
         raise RuntimeError(
-            f"audio_b200: {what} is on '{t.device}'. This package runs only hand-written sm_100a CUDA "
+            f"audio_b200: {what} is on '{t.device}'. This package runs only hand-written sm_90a CUDA "
             "kernels; there is no CPU or ATen fallback -- move the tensor (and the module) to a CUDA device."
         )
     if t.dtype != torch.float32:

@@ -1,7 +1,7 @@
 """Drop-in ``torchaudio.compliance.kaldi`` (spectrogram / fbank / mfcc), backed by libb200audio.so.
 
 Same names, argument order, defaults, assertions and output shapes as the reference
-(/root/reference/src/torchaudio/compliance/kaldi.py: ``spectrogram`` 229-316, ``fbank`` 514-645, ``mfcc`` 669-813,
+(pytorch/audio/src/torchaudio/compliance/kaldi.py: ``spectrogram`` 229-316, ``fbank`` 514-645, ``mfcc`` 669-813,
 ``get_mel_banks`` 436-511 and the mel / VTLN helpers 318-433).  The constant tables (window, mel banks, DCT, lifter)
 are built on the host with the reference's own op sequence in float32, so they are the reference's tables; the
 per-frame work -- framing (snip_edges or mirrored edges), DC removal, log energy, pre-emphasis, window, zero padding,

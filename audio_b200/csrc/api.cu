@@ -28,8 +28,6 @@ int apply_fbank_impl(const float*, int64_t, int64_t, int64_t, int64_t, int64_t, 
                      cudaStream_t);
 int amplitude_to_db_impl(const float*, int64_t, int64_t, float, float, float, float, float*, float*, cudaStream_t);
 size_t resample_workspace_bytes_impl(int, int);
-int resample_plan_info_impl(int, int, int, int32_t*);
-int resample_tc_band_impl(int, int, int, int, int32_t*, int32_t*);
 int resample_prepare_impl(const float*, int, int, int, void*, size_t, cudaStream_t);
 int resample_run_impl(const void*, const float*, int, int, int, const float*, int64_t, int64_t, int64_t, float*, int64_t,
                       int64_t, cudaStream_t);
@@ -270,14 +268,6 @@ int b200a_ratio_f32(const float* pairs, int64_t n, float* out, b200a_stream stre
 int b200a_fill_f32(float* dst, int64_t n, float value, b200a_stream stream) {
   if (dst == nullptr || n < 0) return B200A_EINVAL;
   return fill_impl(dst, n, value, static_cast<cudaStream_t>(stream));
-}
-
-int b200a_resample_plan_info(int32_t orig_r, int32_t new_r, int32_t width, int32_t* info) {
-  return resample_plan_info_impl(orig_r, new_r, width, info);
-}
-
-int b200a_resample_tc_band(int32_t orig_r, int32_t new_r, int32_t width, int32_t phase, int32_t* first, int32_t* last) {
-  return resample_tc_band_impl(orig_r, new_r, width, phase, first, last);
 }
 
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps) {

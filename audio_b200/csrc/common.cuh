@@ -1,4 +1,4 @@
-// Shared declarations for libb200audio (sm_100a).  No torch headers anywhere in csrc/.
+// Shared declarations for libb200audio (sm_90a).  No torch headers anywhere in csrc/.
 #pragma once
 #include <cuda_runtime.h>
 #include <math_constants.h>
@@ -49,6 +49,15 @@ inline WsLayout ws_layout(const b200a_frontend_desc& d) {
   off = align_up(off + sizeof(float) * (size_t)(d.n_mels > 0 ? d.n_mels : 0) * (d.n_mfcc > 0 ? d.n_mfcc : 0), 256);
   l.total = off;
   return l;
+}
+
+// SMs of the current device (persistent grids are sized to one wave of it); -1 if the query fails
+inline int device_sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      n <= 0)
+    return -1;
+  return n;
 }
 
 inline int launch_status() { return cudaGetLastError() == cudaSuccess ? B200A_OK : B200A_ECUDA; }

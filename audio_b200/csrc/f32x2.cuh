@@ -1,12 +1,11 @@
-// Packed FP32 arithmetic (sm_100 `add/mul/fma.rn.f32x2`, SASS FADD2 / FMUL2 / FFMA2) on complex values kept in
-// aligned register pairs.
+// Pair-wise FP32 arithmetic on complex values and on frame pairs kept in register pairs.
 //
-// The PTX instructions only take 64-bit register pairs, but the SASS instructions have per-operand modes --
-// `.F32x2.LO_HI` (halves swapped), `.F32` (one scalar register broadcast to both halves) and per-half sign
-// patterns (`.NP`, `.PN`) -- and ptxas folds `mov.b64 {y, x}`, `{t, t}`, `{-t, t}` operand constructions into
-// them (checked with cuobjdump: no MOV / FNEG survives).  So a complex multiply-accumulate
+// sm_90 has no packed FP32 instructions, so every pair operation is two scalar FADD / FMUL / FFMA.  The
+// interface keeps the (lo, hi) pair in one 64-bit value so that callers can build operands such as
+// `{y, x}`, `{t, t}` or `{-t, t}` without caring how they are evaluated; ptxas removes the moves.
+// A complex multiply-accumulate
 //     (ar + wr br - wi bi,  ai + wr bi + wi br)
-// is TWO issue slots:  t = fma2(splat(wr), b, a);  p = fma2({-wi, wi}, {bi, br}, t)  instead of four.
+// is  t = fma2(splat(wr), b, a);  p = fma2({-wi, wi}, {bi, br}, t)  -- four FFMA.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -25,19 +24,16 @@ __device__ __forceinline__ float2 upk2(uint64_t v) {
   return r;
 }
 __device__ __forceinline__ uint64_t add2_raw(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  const float2 x = upk2(a), y = upk2(b);
+  return pk2(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y));
 }
 __device__ __forceinline__ uint64_t mul2_raw(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  const float2 x = upk2(a), y = upk2(b);
+  return pk2(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
 }
 __device__ __forceinline__ uint64_t fma2_raw(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  const float2 x = upk2(a), y = upk2(b), z = upk2(c);
+  return pk2(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
 }
 
 // element-wise on (x, y) pairs

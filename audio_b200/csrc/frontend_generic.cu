@@ -519,8 +519,7 @@ mfcc_finish_tiled_kernel(const float* __restrict__ feat, int64_t total_rows, int
 // Tensor-pipe variant: out[128 rows x n_mfcc] = clamp(feat[128 x n_mels]) * dct on mma.sync m16n8k8 TF32 with
 // error-compensated operands (A_hi B_hi + A_lo B_hi + A_hi B_lo, ~2^-21 relative to sum |a b|).  One warp per 16 rows,
 // all column tiles; the DCT matrix is kept in shared memory pre-split in B-fragment order.  ~7x fewer issued
-// instructions than the FP32 register-tiled kernel above, which is issue bound (54 % issue utilisation at 59 us):
-// 59 -> 29 us at config 4.  Used for the dB path of MFCC / LFCC (top_db clamp requested; parity bar 1e-4 relative);
+// instructions than the FP32 register-tiled kernel above, which is issue bound.  Used for the dB path of MFCC / LFCC (top_db clamp requested; parity bar 1e-4 relative);
 // un-clamped callers -- log-mel MFCC, and the Kaldi MFCC whose goldens hold cepstra (differences of ~20-valued log
 // energies) to 1e-5 absolute -- keep the FP32 kernel: a six-product TF32 scheme that reaches fp32 accuracy was measured
 // and is no faster than FP32 FMAs here.
@@ -886,7 +885,9 @@ int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* 
         return B200A_ECUDA;
       const int64_t tiles = (total + kMmaFinRows - 1) / kMmaFinRows;
       const int per_sm = msmem <= 72 * 1024 ? 3 : (msmem <= 110 * 1024 ? 2 : 1);
-      const int64_t grid = tiles < 148 * per_sm ? tiles : 148 * per_sm;
+      const int sms = device_sm_count();
+      if (sms < 0) return B200A_ECUDA;
+      const int64_t grid = tiles < (int64_t)sms * per_sm ? tiles : (int64_t)sms * per_sm;
       mfcc_finish_mma_kernel<<<(unsigned)grid, 256, msmem, stream>>>(feat, total, frames, d->n_mels, d->n_mfcc, dct, group_max,
                                                                    rows_per_group > 0 ? rows_per_group : 1, top_db, out);
       return launch_status();
@@ -900,7 +901,9 @@ int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* 
       if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
         return B200A_ECUDA;
       const int64_t tiles = (total + kFinRows - 1) / kFinRows;
-      const int64_t grid = tiles < 148 * 4 ? tiles : 148 * 4;
+      const int sms = device_sm_count();
+      if (sms < 0) return B200A_ECUDA;
+      const int64_t grid = tiles < (int64_t)sms * 4 ? tiles : (int64_t)sms * 4;
       kern<<<(unsigned)grid, 256, tsmem, stream>>>(feat, total, frames, d->n_mels, d->n_mfcc, dct, group_max,
                                                    rows_per_group > 0 ? rows_per_group : 1, top_db, out);
       return launch_status();

@@ -13,30 +13,15 @@
 //                                                                    B = (Z[k] - conj Z[N-k]) / 2i
 //   every lane ends with bins k = l + G m (m < 16) of its two frames; |.|^p -> global (Spectrogram: 16
 //   independent warps per CTA), or -> shared memory for the mel contraction.
-//   mel     warp specialised, two bodies behind one kernel (picked by the plan prepare_tc_kernel built):
-//           tcgen05 (n_fft <= 1024, banded filterbank fits shared memory: every real mel / linear bank):
-//             12 (n_fft = 256: 8) transform warps publish fp32 power values in UMMA core-matrix order,
-//             4 operand warps convert them in place to bf16 hi / lo planes, one thread issues
-//             tcgen05.mma kind::f16 (M = 64, accumulator in TMEM, banded k-steps), the operand warps read
-//             the previous tile's accumulator with tcgen05.ld; error-compensated bf16, ~2^-16 relative.
-//           mma.sync (any other filterbank up to 512 filters, n_fft = 2048, or B200A_TC=0):
-//             8 transform warps publish power rows, 4 contraction warps multiply each finished tile with
-//             the filterbank: m16n8k8 TF32 with error-compensated operands (P_hi*F_hi + P_lo*F_hi +
-//             P_hi*F_lo, ~2^-21 relative), visiting only the k-steps where a group of 8 filters is non-zero.
+//   mel     warp specialised (any filterbank up to 512 filters): 8 transform warps publish power rows,
+//           4 contraction warps multiply each finished tile with the filterbank on the tensor cores:
+//           mma.sync m16n8k8 TF32 with error-compensated operands (P_hi*F_hi + P_lo*F_hi + P_hi*F_lo,
+//           ~2^-21 relative), visiting only the k-steps where a group of 8 filters is non-zero.
 //           (-> dB / log) -> global.
 // Nothing but the waveform is read from HBM and nothing but the final features is written.
 //
-// tcgen05 at n_fft = 1024: an M = 64 tile of 513 bins does not fit next to the transform working set, so
-// the tile has 24 real rows (what 12 warps finish per iteration) and the other 40 operand rows alias
-// whatever follows in shared memory -- each accumulator row depends on its own operand row only, and the
-// TMEM lanes of those rows are never read.  See DESIGN.md ("mel projection").
-//
 // Reference semantics: src/torchaudio/functional/functional.py:54-145 and
 // transforms/_transforms.py:403-415, :701-705 (see frontend_generic.cu for the any-size path).
-#include <cuda_bf16.h>
-
-#include <cstdlib>
-
 #include <type_traits>
 #include <utility>
 
@@ -90,7 +75,7 @@ struct MelPlan {  // built on the device by prepare_mma_kernel
 };
 
 struct Pow2Extra {  // tables appended to the generic workspace
-  size_t tw2d, tw_eo, plan, frags, tc_plan, tc_b, total;
+  size_t tw2d, tw_eo, plan, frags, total;
 };
 
 inline int mel_tiles(int n_mels) { return (n_mels + 7) / 8; }
@@ -108,11 +93,6 @@ inline Pow2Extra pow2_layout(const b200a_frontend_desc& d, size_t base) {
   off = align_up(off + sizeof(MelPlan), 256);
   e.frags = off;  // worst case: every tile spans every bin
   off = align_up(off + sizeof(float4) * 32 * nt * ((n_bins + 7) / 8 + 1), 256);
-  const bool tc = d.n_mels > 0 && d.n_fft <= 1024;  // tcgen05 contraction: step table + banded bf16 B blocks
-  e.tc_plan = off;
-  off = align_up(off + (tc ? 1024 : 0), 256);
-  e.tc_b = off;
-  off = align_up(off + (tc ? 96 * 1024 : 0), 256);
   e.total = off;
   return e;
 }
@@ -152,7 +132,7 @@ __device__ constexpr float kSin32[17] = {0.f, 0.19509032201612825f, 0.3826834323
                                          0.38268343236508989f, 0.19509032201612861f, 0.f};
 
 // DIT butterfly (a, b) -> (a + W b, a - W b), W = exp(-2 pi i E / 32), E in [0, 16), on packed FP32 pairs
-// (f32x2.cuh): 2 issue slots for the trivial twiddles, 3 for the others (was 4 / 6 with scalar FADD / FFMA).
+// (f32x2.cuh).
 template <int E>
 __device__ __forceinline__ void bfly(float2& a, float2& b) {
   if constexpr (E == 0) {
@@ -209,8 +189,6 @@ struct Pow2Params {
   const MelPlan* plan;
   const float4* frags;   // [steps][32] (b0_hi, b1_hi, b0_lo, b1_lo) in mma B-fragment order
   const WsHeader* hdr;
-  const struct TcPlan* tc;     // tcgen05 contraction plan (nullptr: not available for this size)
-  const unsigned char* tc_b;   // its banded bf16 B blocks
   int hop, pad, center, pad_mode, n_mels;
   int stage, log_mels, bulk_ok, stage_ok;
   // output row geometry: value m of frame t goes to out[(row * frames + t) * out_width + out_col0 + m]
@@ -829,8 +807,6 @@ __device__ __forceinline__ void mel_body_mma(const Pow2Params& p, unsigned char*
       __syncwarp();
       if (lane == 0) mbar_arrive(s_full + b);
     }
-  } else if (warp >= kWarps + kMelWarps) {
-    reg_dealloc<24>();  // launched for the tcgen05 body's 12 transform warps: hand the registers back and leave
   } else {
     // =============================== contraction warps =========================================
     reg_dealloc<kMelRegs>();
@@ -1135,707 +1111,12 @@ __global__ void prepare_tw_eo_kernel(float2* tw_eo) {  // [17][32]: W_2048^(l + 
   }
 }
 
-// ================================================================================================
-// Mel contraction on tcgen05 (5th-generation tensor cores, accumulator in tensor memory).
-//
-// Moving the contraction to the tensor core frees the registers and issue slots of four mma.sync warps, so
-// this body runs NW = 12 transform warps (n_fft >= 512; the transform is latency bound and scales with
-// resident warps) next to four light "operand" warps.  One CTA iteration finishes R = 2 NW (32 / G) frames.
-//   transform warps     publish fp32 power values into the OPERAND BUFFER, already in the tensor core's
-//                       K-major core-matrix order: chunk = 8 bins; per chunk, per group of 8 frames, a
-//                       256-byte block [8 rows x 8 floats]; arrive on `full`
-//   operand warps       convert each block IN PLACE to [8 rows x 8 bf16 hi | 8 rows x 8 bf16 lo] (read 32 B,
-//                       __syncwarp, write 16 + 16 B), fence to the async proxy, arrive on `ready`
-//   warp NW + 3         issues, per k-step of 16 bins,
-//                           D[:, 2 n0 : 2 n0 + 2 N] += P_hi [F_hi | F_lo] + P_lo [F_hi | F_lo]   (tcgen05.mma kind::f16,
-//                       M = 64, two instructions) and commits to the buffer's `mma` barrier, which is also what
-//                       the transform warps wait on before they publish into that buffer again.  The filterbank
-//                       sits in shared memory as BANDED UMMA B blocks: for each k-step only the filters that
-//                       are non-zero there (groups of 8: 8 rows F_hi, 8 rows F_lo), so filter f owns accumulator
-//                       columns 16 (f / 8) + f % 8 and + 8.  Tile rows >= R of the M = 64 instruction alias
-//                       whatever follows in shared memory and land in TMEM lanes nobody reads (an accumulator
-//                       row depends on its own operand row only).
-//   epilogue            ceil(R / 16) of the operand warps (one TMEM lane quadrant each) tcgen05.ld the PREVIOUS
-//                       tile's accumulator (two accumulators alternate) while the tensor core works on the
-//                       current one: hi + lo columns, dB / log, top_db maximum, store.
-// Error-compensated bf16 carries ~2^-16 relative error per product (the 1e-4 bar; the TF32x3 mma.sync body
-// ~2^-21).
-// ================================================================================================
-constexpr int kTcMaxSteps = 34;       // k-steps of 16 bins (n_fft = 1024: 33)
-constexpr int kTcMaxN = 128;          // filters: 2 accumulator columns each, two accumulators in 512 TMEM columns
-constexpr int kTcWsBBytes = 96 * 1024;  // workspace reserved for the banded B blocks
-
-struct TcStep {
-  uint32_t b_off;  // byte offset of the step's block in the B region (64 n bytes: 2 k-chunks x 2 n operand rows)
-  uint32_t n;      // filters covered (multiple of 8)
-  uint32_t col;    // first filter
-  uint32_t kstep;  // which 16 bins: [16 kstep, 16 kstep + 16)
-};
-struct TcPlan {  // built on the device by prepare_tc_kernel
-  int ok, steps, n_pad, b_bytes;
-  TcStep step[kTcMaxSteps];
-};
-struct __align__(16) TcIssue {  // ready-to-issue descriptors of one k-step (operand buffer 0), built per CTA
-  uint64_t a_hi, a_lo, b;
-  uint32_t idesc, col;
-};
-
-template <int G>
-struct TcGeo {
-  using Ge = Geo<G>;
-  static constexpr int NW = G == 8 ? 8 : 12;               // transform warps
-  static constexpr int NB = G == 8 ? 2 : 1;                // operand buffers
-  static constexpr int kThreads = (NW + kMelWarps) * 32;
-  static constexpr int kFftRegs = NW == 12 ? 144 : 216;    // 384*144 + 128*80 = 65536 = 512*128; 256*216 + 128*72 = 64512
-  static constexpr int kOpRegs = NW == 12 ? 80 : 72;
-  static constexpr int kRows = NW * Ge::kFrames;           // frames per tile: 24 / 48 / 64
-  static constexpr int kChunks = 2 * G + 2;                // ceil((16 G + 1) / 8) rounded up to even
-  static constexpr int kSteps = kChunks / 2;
-  static constexpr int kChunkStride = kRows * 32 + 32;     // bytes; == 32 (mod 128): conflict-free publishing
-  static constexpr int kOperand = kChunks * kChunkStride;  // bytes of one operand buffer
-  static constexpr int kEpi = (kRows + 15) / 16;           // epilogue warps == TMEM lane quadrants in use
-  static constexpr int kFixed = NB * kOperand + 8 * (NW * Ge::kTileF2 + 32 * G) + 16 * NB * kRows +
-                                (int)sizeof(TcIssue) * kTcMaxSteps + 8 * (NW + 4 * NB + 4) + 16;
-  static constexpr int kBBudget = ((227 * 1024 - kFixed) / 128) * 128;
-  static_assert(kSteps <= kTcMaxSteps && kRows <= 64 && kRows % 8 == 0, "one M = 64 tile per iteration");
-};
-struct Tc2;
-int tc_b_budget(int n_fft);  // defined after Tc2
-
-// (x, y) -> packed bf16 pair (x in the low half) and the packed pair of the residuals
-__device__ __forceinline__ void split_bf16x2(float x, float y, uint32_t& hi, uint32_t& lo) {
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(y), "f"(x));
-  const float rx = x - __uint_as_float(hi << 16), ry = y - __uint_as_float(hi & 0xffff0000u);
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(ry), "f"(rx));
-}
-
+// The mel / MFCC-feature kernel: 8 transform warps and 4 mma.sync contraction warps (three warpgroups, so each
+// setmaxnreg covers whole warpgroups).
 template <int POWER_MODE, int G, int HG, bool KALDI>
-__device__ __forceinline__ void mel_body_tc(const Pow2Params& p, unsigned char* smem_raw) {
-  using Ge = Geo<G>;
-  using Tc = TcGeo<G>;
-  constexpr int NW = Tc::NW, NB = Tc::NB, kRows = Tc::kRows, kEpi = Tc::kEpi, kStride = Tc::kChunkStride;
-  unsigned char* s_a = smem_raw;                                                   // [NB] operand buffers
-  unsigned char* s_b = s_a + NB * Tc::kOperand;                                    // banded B blocks
-  float2* s_tile_all = reinterpret_cast<float2*>(s_b + Tc::kBBudget);              // [NW][kTileF2]
-  float2* s_tw = s_tile_all + NW * Ge::kTileF2;                                    // [32][G]
-  int64_t* s_slot = reinterpret_cast<int64_t*>(s_tw + 32 * G);                     // [NB][kRows]
-  int64_t* s_grp = s_slot + NB * kRows;                                            // [NB][kRows]
-  TcIssue* s_issue = reinterpret_cast<TcIssue*>(s_grp + NB * kRows);               // [kTcMaxSteps]
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_issue + kTcMaxSteps);            // [NW] staging
-  uint64_t* s_full = s_bar + NW;                                                   // [NB] fp32 values published
-  uint64_t* s_ready = s_full + NB;                                                 // [NB] converted to bf16 planes
-  uint64_t* s_mma = s_ready + NB;                                                  // [NB] MMAs of the buffer complete
-  uint64_t* s_tfree = s_mma + NB;                                                  // [2] accumulator read out
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_tfree + 2);
-
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform
-  const int n_steps = p.tc->steps, n_pad = p.tc->n_pad;
-  for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
-  {  // the pad chunk of every operand buffer stays zero; B blocks come prepared
-    uint4* a4 = reinterpret_cast<uint4*>(s_a);
-    for (int i = tid; i < NB * Tc::kOperand / 16; i += blockDim.x) a4[i] = make_uint4(0, 0, 0, 0);
-    const uint4* src = reinterpret_cast<const uint4*>(p.tc_b);
-    uint4* b4 = reinterpret_cast<uint4*>(s_b);
-    const int n16 = p.tc->b_bytes / 16;
-    for (int i = tid; i < n16; i += blockDim.x) b4[i] = src[i];
-  }
-  if (tid < n_steps) {
-    const TcStep st = p.tc->step[tid];
-    const uint32_t a_addr = smem_u32(s_a) + st.kstep * 2 * kStride;
-    TcIssue o;
-    o.a_hi = umma_smem_desc(a_addr, kStride, 256);        // 8-row groups 256 B apart: [hi 128 B | lo 128 B]
-    o.a_lo = umma_smem_desc(a_addr + 128, kStride, 256);
-    o.b = umma_smem_desc(smem_u32(s_b) + st.b_off, st.n * 32, 128);  // 2 n rows: per 8 filters, 8 hi rows then 8 lo rows
-    o.idesc = umma_idesc_bf16(64, 2 * (int)st.n);
-    o.col = 2 * st.col;
-    s_issue[tid] = o;
-  }
-  if (tid < NW) mbar_init(s_bar + tid, 1);
-  if (tid == 0) {
-    for (int i = 0; i < NB; ++i) {
-      mbar_init(s_full + i, NW);
-      mbar_init(s_ready + i, kMelWarps);
-      mbar_init(s_mma + i, 1);
-    }
-    mbar_init(s_tfree + 0, kEpi);
-    mbar_init(s_tfree + 1, kEpi);
-  }
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // B blocks, zeroed buffers -> the tensor core
-  __syncthreads();
-
-  const int64_t stride = (int64_t)gridDim.x * NW;
-  const int64_t u0 = (int64_t)blockIdx.x * NW;
-  const int width = p.out_width;
-
-  if (warp < NW) {
-    // =============================== transform warps ===========================================
-    reg_alloc<Tc::kFftRegs>();
-    float2* tile = s_tile_all + warp * Ge::kTileF2;
-    float* stage = reinterpret_cast<float*>(tile);
-    uint64_t* bar = s_bar + warp;
-    float wreg[32];
-    load_window<G>(p, lane, wreg);
-    const int half = frame_lead(p, Ge::kNfft);
-    const int gi = lane / G, l = lane % G;
-    uint32_t parity = 0;
-    bool staged = false;
-    UnitCursor cur;
-    cur.init(u0 + warp, stride, p.units_per_row);
-    if (bulk_eligible<G>(p, half, cur.u, cur.ub)) {
-      if (lane == 0) issue_bulk<G>(p, half, cur.row, cur.ub, stage, bar);
-      staged = true;
-    }
-    // value (row, bin k) lives at chunk (k / 8), 8-row group (row / 8): [row % 8][k % 8] floats
-    const int row_a = Ge::kFrames * warp + 2 * gi;  // even: rows a and a + 1 share the 8-row group
-    const int lane_off = (l >> 3) * kStride + (row_a >> 3) * 256 + (row_a & 7) * 32 + (l & 7) * 4;
-    constexpr int kStepM = (G / 8) * kStride;
-    int it = 0;
-    for (int64_t base = u0; base < p.total_units; base += stride, ++it, cur.advance()) {
-      const bool valid = cur.u < p.total_units;
-      float pa[17], pb[17];
-      if (valid)
-        transform_unit<POWER_MODE, G, HG, true, KALDI>(p, wreg, s_tw, tile, stage, bar, parity, staged, cur, half, lane, pa,
-                                                pb);
-      const int b = it % NB;
-      if (it >= NB) mbar_wait(s_mma + b, ((it / NB) & 1) ^ 1);  // the tensor core has consumed this buffer
-      unsigned char* dst = s_a + (size_t)b * Tc::kOperand + lane_off;
-      if (valid) {
-#pragma unroll
-        for (int m = 0; m < 16; ++m) {
-          *reinterpret_cast<float*>(dst + m * kStepM) = pa[m];
-          *reinterpret_cast<float*>(dst + m * kStepM + 32) = pb[m];
-        }
-        if (l == 0) {  // bin n_fft/2 opens chunk 2 G: write the whole 8-float row, the other 7 are zeros
-          float4* ra = reinterpret_cast<float4*>(dst + 16 * kStepM);
-          ra[0] = make_float4(pa[16], 0.f, 0.f, 0.f);
-          ra[1] = make_float4(0.f, 0.f, 0.f, 0.f);
-          ra[2] = make_float4(pb[16], 0.f, 0.f, 0.f);
-          ra[3] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-      if (l == 0) {
-        const int64_t ta = cur.ub * Ge::kFrames + 2 * gi;
-        const int64_t oa = (cur.row * p.frames + ta) * (int64_t)width + p.out_col0;
-        s_slot[b * kRows + row_a] = (valid && ta < p.frames) ? oa : -1;
-        s_slot[b * kRows + row_a + 1] = (valid && ta + 1 < p.frames) ? oa + width : -1;
-        const int64_t g = cur.row / p.rows_per_group;
-        s_grp[b * kRows + row_a] = g;
-        s_grp[b * kRows + row_a + 1] = g;
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_full + b);
-    }
-  } else {
-    // ============ operand warps (all four), MMA issue (the last), epilogue (the first kEpi of them) ============
-    reg_dealloc<Tc::kOpRegs>();  // one setmaxnreg for the whole warpgroup
-    const int cw = warp - NW;    // == TMEM lane quadrant (NW % 4 == 0)
-    static_assert(NW % 4 == 0, "operand warp i must own TMEM lane quadrant i");
-    const uint32_t acc_cols = 2 * n_pad;  // one accumulator; two of them alternate
-    const uint32_t tmem_cols =
-        acc_cols <= 16 ? 32u : (acc_cols <= 32 ? 64u : (acc_cols <= 64 ? 128u : (acc_cols <= 128 ? 256u : 512u)));
-    if (cw == 0) tmem_alloc(s_tmem, tmem_cols);
-    tc_fence_before();
-    asm volatile("bar.sync 1, %0;" ::"n"(kMelWarps * 32) : "memory");
-    tc_fence_after();
-    const uint32_t tmem_d = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-    GroupMax gmax{p.stage == B200A_STAGE_FEAT ? p.group_max : nullptr, -1, -CUDART_INF_F};
-    // conversion items: (chunk, row) with the row fastest (8 consecutive lanes = one 256-byte block)
-    constexpr int kItems = (Tc::kChunks - 1) * kRows, kRounds = (kItems + 127) / 128;
-    const int erow = 16 * cw + (lane & 15);  // epilogue: thread i < 16 owns tile row 16 cw + i == TMEM lane 32 cw + i
-
-    // accumulator of tile `t` -> dB / log -> global; o / g: output offset and top_db group of this thread's row
-    auto epilogue = [&](int t, int64_t o, int64_t g) {
-      const uint32_t acc = tmem_d + ((uint32_t)(32 * cw) << 16) + (uint32_t)(t & 1) * acc_cols;
-      const bool row_ok = lane < 16 && o >= 0;
-#pragma unroll 1
-      for (int f0 = 0; f0 < n_pad; f0 += 16) {
-        float u[16], w[16], v[16];
-        tmem_ld16(acc + 2 * f0, u);
-        tmem_ld16(acc + 2 * f0 + 16, w);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          v[q] = u[q] + u[q + 8];
-          v[q + 8] = w[q] + w[q + 8];
-        }
-        if (p.k_log) {  // Kaldi fbank: log(max(mel, FLT_EPSILON)), kaldi.py:629-631
-#pragma unroll
-          for (int q = 0; q < 16; ++q) v[q] = 0.69314718055994531f * __log2f(fmaxf(v[q], kKaldiEps));
-        }
-        if (p.stage == B200A_STAGE_FEAT) {
-          // one thread owns a whole row here, so the logarithms are the epilogue's critical path: MUFU.LG2
-          // (2^-22 absolute on the log2, i.e. < 1e-5 dB) instead of the ~30-instruction log10f
-          float mx = -CUDART_INF_F;
-          const float scale = p.log_mels ? 0.69314718055994531f : p.db_mult * 0.30102999566398120f;
-          const float offs = p.log_mels ? 0.f : p.db_offset;
-#pragma unroll
-          for (int q = 0; q < 16; ++q) {
-            const float arg = p.log_mels ? v[q] + 1e-6f : fmaxf(v[q], p.db_amin);
-            v[q] = fmaf(scale, __log2f(arg), -offs);
-            if (f0 + q < p.n_mels) mx = fmaxf(mx, v[q]);
-          }
-          gmax.add(g, mx, row_ok);
-        }
-        if (row_ok) {
-          float* dst = p.out + o + f0;
-          if (p.out_vec >= 4 && f0 + 16 <= p.n_mels) {
-#pragma unroll
-            for (int q = 0; q < 16; q += 4)
-              *reinterpret_cast<float4*>(dst + q) = make_float4(v[q], v[q + 1], v[q + 2], v[q + 3]);
-          } else {
-#pragma unroll
-            for (int q = 0; q < 16; ++q)
-              if (f0 + q < p.n_mels) dst[q] = v[q];
-          }
-        }
-      }
-      tc_fence_before();  // my tcgen05.ld are done before this accumulator is handed back
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_tfree + (t & 1));
-    };
-
-    int it = 0;
-    int64_t o_prev = -1, g_prev = -1;
-    for (int64_t base = u0; base < p.total_units; base += stride, ++it) {
-      const int b = it % NB;
-      const uint32_t use = (uint32_t)(it / NB) & 1;  // parity of this use of buffer b
-      mbar_wait(s_full + b, use);
-      int64_t o_cur = -1, g_cur = -1;
-      if (cw < kEpi && erow < kRows) {
-        o_cur = s_slot[b * kRows + erow];
-        g_cur = s_grp[b * kRows + erow];
-      }
-      {
-        unsigned char* buf = s_a + (size_t)b * Tc::kOperand;
-#pragma unroll 2
-        for (int rd = 0; rd < kRounds; ++rd) {
-          const int item = rd * 128 + cw * 32 + lane;
-          const bool live = item < kItems;
-          const int chunk = item / kRows, row = item % kRows;
-          unsigned char* blk = buf + chunk * kStride + (row >> 3) * 256;
-          float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-          if (live) {
-            v0 = *reinterpret_cast<const float4*>(blk + (row & 7) * 32);
-            v1 = *reinterpret_cast<const float4*>(blk + (row & 7) * 32 + 16);
-          }
-          uint4 hi, lo;
-          split_bf16x2(v0.x, v0.y, hi.x, lo.x);
-          split_bf16x2(v0.z, v0.w, hi.y, lo.y);
-          split_bf16x2(v1.x, v1.y, hi.z, lo.z);
-          split_bf16x2(v1.z, v1.w, hi.w, lo.w);
-          __syncwarp();  // the 8 rows of a block are 8 lanes of this warp: all reads before any write
-          if (live) {
-            *reinterpret_cast<uint4*>(blk + (row & 7) * 16) = hi;
-            *reinterpret_cast<uint4*>(blk + 128 + (row & 7) * 16) = lo;
-          }
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // my plane writes -> async proxy
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_ready + b);
-      if (cw == kMelWarps - 1) {
-        // ---- issue: D[it & 1][:, 2 n0 : 2 n0 + 2 N] += P_hi [F_hi | F_lo] + P_lo [F_hi | F_lo] per k-step ----
-        mbar_wait(s_ready + b, use);
-        if (it >= 2) mbar_wait(s_tfree + (it & 1), ((it >> 1) & 1) ^ 1);  // tile it - 2 has left this accumulator
-        tc_fence_after();
-        const uint32_t acc = tmem_d + (uint32_t)(it & 1) * acc_cols;
-        const uint64_t a_off = (uint64_t)((uint32_t)b * (Tc::kOperand >> 4));
-#pragma unroll 3
-        for (int s = 0; s < n_steps; ++s) {
-          const TcIssue e = s_issue[s];
-          if (elect_one()) {
-            umma_bf16(acc + e.col, e.a_hi + a_off, e.b, e.idesc, s > 0 ? 1u : 0u);  // step 0 spans every column
-            umma_bf16(acc + e.col, e.a_lo + a_off, e.b, e.idesc, 1u);
-          }
-        }
-        if (elect_one()) umma_commit(s_mma + b);
-        __syncwarp();
-      }
-      if (cw < kEpi && it > 0) {  // the previous tile's accumulator, while the tensor core works on this one
-        // NB == 1: tile it could only be published (`full`, waited above) after the MMAs of tile it - 1 completed,
-        // and a second look at that barrier could race with the completion of tile it
-        if (NB > 1) mbar_wait(s_mma + (it - 1) % NB, (uint32_t)((it - 1) / NB) & 1);
-        tc_fence_after();
-        epilogue(it - 1, o_prev, g_prev);
-      }
-      o_prev = o_cur;
-      g_prev = g_cur;
-    }
-    if (cw < kEpi && it > 0) {
-      mbar_wait(s_mma + (it - 1) % NB, (uint32_t)((it - 1) / NB) & 1);
-      tc_fence_after();
-      epilogue(it - 1, o_prev, g_prev);
-    }
-    gmax.flush();
-    tc_fence_before();
-    asm volatile("bar.sync 1, %0;" ::"n"(kMelWarps * 32) : "memory");  // every tcgen05.ld is done
-    if (cw == 0) tmem_dealloc(tmem_d, tmem_cols);
-  }
-}
-
-// Position kp of the contraction's (permuted) K axis -> spectrum bin, or -1 for a padding position.
-//   perm_g == 0: identity (operand buffer in bin order; n_fft 256 / 512 body).
-//   perm_g == G: the n_fft = 32 G register FFT leaves lane l with bins l + G m; the transform warps publish the PAIR
-//                (m, m + 1) of a lane as one packed bf16x2 word, so K position 2 G (m >> 1) + 2 l + (m & 1) holds
-//                bin l + G m, and the Nyquist bin sits at position n_fft / 2.
-__host__ __device__ __forceinline__ int tc_bin_of(int kp, int perm_g, int n_bins) {
-  if (perm_g == 0) return kp < n_bins ? kp : -1;
-  const int half = 16 * perm_g;  // n_fft / 2
-  if (kp == half) return half;
-  if (kp > half) return -1;
-  const int j = kp / (2 * perm_g), rem = kp % (2 * perm_g);
-  return (rem >> 1) + perm_g * (2 * j + (rem & 1));
-}
-
-// Banded bf16 hi / lo UMMA B blocks and their step table.  One block.
-__global__ void prepare_tc_kernel(const float* __restrict__ fb, int n_bins, int n_mels, int n_fft, int budget,
-                                  int perm_g, TcPlan* plan, unsigned char* blocks) {
-  __shared__ int s_lo[kTcMaxSteps], s_hi[kTcMaxSteps];
-  __shared__ TcPlan s_plan;
-  const int k_steps = (n_fft / 16 + 2) / 2;  // (2 G + 2) / 2
-  const int n_pad = (n_mels + 15) / 16 * 16;
-  if ((int)threadIdx.x < k_steps) {
-    int lo = n_mels, hi = -1;
-    for (int kp = 16 * threadIdx.x; kp < 16 * (int)threadIdx.x + 16; ++kp) {
-      const int k = tc_bin_of(kp, perm_g, n_bins);
-      if (k < 0) continue;
-      for (int n = 0; n < n_mels; ++n)
-        if (fb[(size_t)k * n_mels + n] != 0.f) {
-          lo = min(lo, n);
-          hi = max(hi, n);
-        }
-    }
-    s_lo[threadIdx.x] = lo;
-    s_hi[threadIdx.x] = hi;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int steps = 0, off = 0;
-    for (int s = 0; s < k_steps; ++s) {
-      int n0, n;
-      if (s == 0) {  // the first MMA clears the accumulator: every column
-        n0 = 0;
-        n = n_pad;
-      } else if (s_hi[s] < 0) {
-        continue;
-      } else {
-        n0 = s_lo[s] / 8 * 8;
-        n = (s_hi[s] + 1 - n0 + 7) / 8 * 8;
-      }
-      s_plan.step[steps] = TcStep{(uint32_t)off, (uint32_t)n, (uint32_t)n0, (uint32_t)s};
-      off += n * 64;
-      ++steps;
-    }
-    s_plan.steps = steps;
-    s_plan.n_pad = n_pad;
-    s_plan.b_bytes = off;
-    s_plan.ok = (off <= budget && off <= kTcWsBBytes && n_pad <= kTcMaxN) ? 1 : 0;
-  }
-  __syncthreads();
-  if (s_plan.ok) {
-    for (int s = 0; s < s_plan.steps; ++s) {
-      const TcStep st = s_plan.step[s];
-      for (int i = threadIdx.x; i < (int)st.n * 16; i += blockDim.x) {
-        const int nl = i >> 4, kk = i & 15;
-        const int n = (int)st.col + nl, k = tc_bin_of(16 * (int)st.kstep + kk, perm_g, n_bins);
-        const float v = (n < n_mels && k >= 0) ? fb[(size_t)k * n_mels + n] : 0.f;
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(h));
-        // operand row of filter nl: 16 (nl / 8) + nl % 8 for F_hi, + 8 for F_lo; 2 n rows x 16 B per k chunk
-        const size_t row = (size_t)(nl >> 3) * 16 + (nl & 7);
-        const size_t o = st.b_off + (size_t)(kk >> 3) * st.n * 32 + row * 16 + (size_t)(kk & 7) * 2;
-        *reinterpret_cast<__nv_bfloat16*>(blocks + o) = h;
-        *reinterpret_cast<__nv_bfloat16*>(blocks + o + 128) = lo;
-      }
-    }
-  }
-  for (int i = threadIdx.x; i < (int)(sizeof(TcPlan) / sizeof(int)); i += blockDim.x)
-    reinterpret_cast<int*>(plan)[i] = reinterpret_cast<const int*>(&s_plan)[i];
-}
-
-// ================================================================================================
-// n_fft = 1024 contraction, second generation (mel_body_tc2).  What changed against mel_body_tc:
-//   * the transform warps publish bf16 hi / lo words DIRECTLY (no fp32 staging, no conversion pass by other warps,
-//     one barrier hop less): a lane packs the powers of its bins (l + 32 m, l + 32 (m + 1)) into one bf16x2 word,
-//     which makes the contraction's K axis a permutation of the spectrum (tc_bin_of) -- the banded filterbank
-//     blocks are built in the same order, so nothing else notices;
-//   * the hi and lo planes of a frame are two ROWS of the same M = 64 operand tile (row group 2 (r / 8) = hi,
-//     + 1 = lo), so ONE tcgen05.mma per k-step produces P_hi F and P_lo F side by side in tensor memory lanes
-//     i and i + 8 of the frame group's lane quadrant, and the epilogue adds them with one shuffle.  Against two
-//     M = 64 instructions per k-step (each reading 64 operand rows of which 24 were real) this halves the
-//     tensor core's shared-memory reads: 48 of the 64 rows are real now.
-//   * the four service warps only issue MMAs (one of them) and run the epilogue (three: one per 8-frame group).
-// ================================================================================================
-struct Tc2 {
-  static constexpr int NW = 12;                       // transform warps
-  static constexpr int kThreads = (NW + kMelWarps) * 32;
-  static constexpr int kFftRegs = 144, kSvcRegs = 80;  // 384*144 + 128*80 = 65536
-  static constexpr int kRows = 2 * NW;                // frames per tile: 24
-  static constexpr int kQuads = (kRows + 7) / 8;      // 8-frame groups == TMEM lane quadrants in use == epilogue warps
-  static constexpr int kChunks = 66;                  // 8-position K chunks: 512 + Nyquist chunk + one of padding
-  static constexpr int kSteps = kChunks / 2;
-  static constexpr int kChunkStride = kQuads * 256 + 16;  // bytes: [hi 128 B | lo 128 B] per frame group; / 16 odd
-  static constexpr int kOperand = ((kChunks * kChunkStride + 1024 + 127) / 128) * 128;  // + the M = 64 over-read
-  static constexpr int kFixed = kOperand + 8 * (NW * Geo<32>::kTileF2 + 32 * 32) + 16 * kRows + 32 * kTcMaxSteps +
-                                8 * (NW + 8) + 16;
-  static constexpr int kBBudget = ((227 * 1024 - kFixed) / 128) * 128;
-  static_assert(kQuads <= 3 && (kChunkStride / 16) % 2 == 1 && kSteps <= kTcMaxSteps, "layout");
-  static_assert(kBBudget >= 40 * 1024, "banded filterbank blocks need room");
-};
-struct __align__(16) TcIssue2 {  // ready-to-issue descriptors of one k-step
-  uint64_t a, b;
-  uint32_t idesc, col, pad0, pad1;
-};
-
-template <int POWER_MODE, int HG, bool KALDI>
-__device__ __forceinline__ void mel_body_tc2(const Pow2Params& p, unsigned char* smem_raw) {
-  constexpr int G = 32;
-  using Ge = Geo<G>;
-  constexpr int NW = Tc2::NW, kRows = Tc2::kRows, kQuads = Tc2::kQuads, kStride = Tc2::kChunkStride;
-  unsigned char* s_a = smem_raw;                                                   // operand buffer
-  unsigned char* s_b = s_a + Tc2::kOperand;                                        // banded B blocks
-  float2* s_tile_all = reinterpret_cast<float2*>(s_b + Tc2::kBBudget);             // [NW][kTileF2]
-  float2* s_tw = s_tile_all + NW * Ge::kTileF2;                                    // [32][G]
-  int64_t* s_slot = reinterpret_cast<int64_t*>(s_tw + 32 * G);                     // [kRows] output offsets
-  int64_t* s_grp = s_slot + kRows;                                                 // [kRows] top_db groups
-  TcIssue2* s_issue = reinterpret_cast<TcIssue2*>(s_grp + kRows);                  // [kTcMaxSteps]
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_issue + kTcMaxSteps);            // [NW] staging
-  uint64_t* s_full = s_bar + NW;                                                   // operand tile published
-  uint64_t* s_mma = s_full + 1;                                                    // its MMAs complete
-  uint64_t* s_tfree = s_mma + 1;                                                   // [2] accumulator read out
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_tfree + 2);
-
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform
-  const int n_steps = p.tc->steps, n_pad = p.tc->n_pad;
-  for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
-  {  // positions nobody publishes (the Nyquist chunk's tail, the padding chunk) stay zero; B blocks come prepared
-    uint4* a4 = reinterpret_cast<uint4*>(s_a);
-    for (int i = tid; i < Tc2::kOperand / 16; i += blockDim.x) a4[i] = make_uint4(0, 0, 0, 0);
-    const uint4* src = reinterpret_cast<const uint4*>(p.tc_b);
-    uint4* b4 = reinterpret_cast<uint4*>(s_b);
-    const int n16 = p.tc->b_bytes / 16;
-    for (int i = tid; i < n16; i += blockDim.x) b4[i] = src[i];
-  }
-  if (tid < n_steps) {
-    const TcStep st = p.tc->step[tid];
-    TcIssue2 o;
-    // A: 64 rows = 8 row groups 128 B apart (hi / lo of four 8-frame groups), the two K chunks kStride apart
-    o.a = umma_smem_desc(smem_u32(s_a) + st.kstep * 2 * kStride, kStride, 128);
-    o.b = umma_smem_desc(smem_u32(s_b) + st.b_off, st.n * 32, 128);  // 2 n rows: per 8 filters, 8 hi rows then 8 lo rows
-    o.idesc = umma_idesc_bf16(64, 2 * (int)st.n);
-    o.col = 2 * st.col;
-    o.pad0 = o.pad1 = 0;
-    s_issue[tid] = o;
-  }
-  if (tid < NW) mbar_init(s_bar + tid, 1);
-  if (tid == 0) {
-    mbar_init(s_full, NW);
-    mbar_init(s_mma, 1);
-    mbar_init(s_tfree + 0, kQuads);
-    mbar_init(s_tfree + 1, kQuads);
-  }
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // B blocks, zeroed buffer -> the tensor core
-  __syncthreads();
-
-  const int64_t stride = (int64_t)gridDim.x * NW;
-  const int64_t u0 = (int64_t)blockIdx.x * NW;
-  const int width = p.out_width;
-
-  if (warp < NW) {
-    // =============================== transform warps ===========================================
-    reg_alloc<Tc2::kFftRegs>();
-    float2* tile = s_tile_all + warp * Ge::kTileF2;
-    float* stage = reinterpret_cast<float*>(tile);
-    uint64_t* bar = s_bar + warp;
-    float wreg[32];
-    load_window<G>(p, lane, wreg);
-    const int half = frame_lead(p, Ge::kNfft);
-    const int l = lane;
-    uint32_t parity = 0;
-    bool staged = false;
-    UnitCursor cur;
-    cur.init(u0 + warp, stride, p.units_per_row);
-    if (bulk_eligible<G>(p, half, cur.u, cur.ub)) {
-      if (lane == 0) issue_bulk<G>(p, half, cur.row, cur.ub, stage, bar);
-      staged = true;
-    }
-    // frames 2 warp (a) and 2 warp + 1 (b) are rows (r & 7) of frame group r >> 3; K position 64 j + 2 l (+1):
-    // chunk 8 j + (l >> 2), byte (l & 3) * 4 of the 16-byte row.  32 lanes -> 8 chunks x 4 words: conflict free.
-    const int row_a = 2 * warp;
-    unsigned char* dst = s_a + (l >> 2) * kStride + (row_a >> 3) * 256 + (row_a & 7) * 16 + (l & 3) * 4;
-    int it = 0;
-    for (int64_t base = u0; base < p.total_units; base += stride, ++it, cur.advance()) {
-      const bool valid = cur.u < p.total_units;
-      float pa[17], pb[17];
-      if (valid)
-        transform_unit<POWER_MODE, G, HG, true, KALDI>(p, wreg, s_tw, tile, stage, bar, parity, staged, cur, half, lane, pa,
-                                                       pb);
-      if (it >= 1) mbar_wait(s_mma, (uint32_t)(it & 1) ^ 1u);  // the tensor core has consumed the previous tile
-      if (valid) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          uint32_t ha, la, hb, lb;
-          split_bf16x2(pa[2 * j], pa[2 * j + 1], ha, la);
-          split_bf16x2(pb[2 * j], pb[2 * j + 1], hb, lb);
-          unsigned char* d = dst + j * (8 * kStride);
-          *reinterpret_cast<uint32_t*>(d) = ha;
-          *reinterpret_cast<uint32_t*>(d + 16) = hb;
-          *reinterpret_cast<uint32_t*>(d + 128) = la;
-          *reinterpret_cast<uint32_t*>(d + 144) = lb;
-        }
-        if (l == 0) {  // bin n_fft / 2 opens chunk 64; its partner position is padding
-          uint32_t ha, la, hb, lb;
-          split_bf16x2(pa[16], 0.f, ha, la);
-          split_bf16x2(pb[16], 0.f, hb, lb);
-          unsigned char* d = dst + 8 * (8 * kStride);
-          *reinterpret_cast<uint32_t*>(d) = ha;
-          *reinterpret_cast<uint32_t*>(d + 16) = hb;
-          *reinterpret_cast<uint32_t*>(d + 128) = la;
-          *reinterpret_cast<uint32_t*>(d + 144) = lb;
-        }
-      }
-      if (l == 0) {
-        const int64_t ta = cur.ub * Ge::kFrames;
-        const int64_t oa = (cur.row * p.frames + ta) * (int64_t)width + p.out_col0;
-        s_slot[row_a] = (valid && ta < p.frames) ? oa : -1;
-        s_slot[row_a + 1] = (valid && ta + 1 < p.frames) ? oa + width : -1;
-        const int64_t g = cur.row / p.rows_per_group;
-        s_grp[row_a] = g;
-        s_grp[row_a + 1] = g;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // my operand words -> the tensor core
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_full);
-    }
-  } else {
-    // ============ service warps: epilogue (the first kQuads of them), MMA issue (the last) ============
-    reg_dealloc<Tc2::kSvcRegs>();  // one setmaxnreg for the whole warpgroup
-    const int cw = warp - NW;      // == TMEM lane quadrant (NW % 4 == 0)
-    static_assert(NW % 4 == 0, "service warp i must own TMEM lane quadrant i");
-    const uint32_t acc_cols = 2 * n_pad;  // one accumulator; two of them alternate
-    const uint32_t tmem_cols =
-        acc_cols <= 16 ? 32u : (acc_cols <= 32 ? 64u : (acc_cols <= 64 ? 128u : (acc_cols <= 128 ? 256u : 512u)));
-    if (cw == 0) tmem_alloc(s_tmem, tmem_cols);
-    tc_fence_before();
-    asm volatile("bar.sync 1, %0;" ::"n"(kMelWarps * 32) : "memory");
-    tc_fence_after();
-    const uint32_t tmem_d = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-    GroupMax gmax{p.stage == B200A_STAGE_FEAT ? p.group_max : nullptr, -1, -CUDART_INF_F};
-    // epilogue thread i < 8 owns frame 8 cw + i: its hi-plane row is TMEM lane 32 cw + i, its lo-plane row lane + 8
-    const int erow = 8 * cw + (lane & 7);
-
-    auto epilogue = [&](int t, int64_t o, int64_t g) {
-      const uint32_t acc = tmem_d + ((uint32_t)(32 * cw) << 16) + (uint32_t)(t & 1) * acc_cols;
-      const bool row_ok = lane < 8 && o >= 0;
-#pragma unroll 1
-      for (int f0 = 0; f0 < n_pad; f0 += 16) {
-        float u[16], w[16], v[16];
-        tmem_ld16(acc + 2 * f0, u);
-        tmem_ld16(acc + 2 * f0 + 16, w);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          v[q] = u[q] + u[q + 8];          // x F_hi + x F_lo
-          v[q + 8] = w[q] + w[q + 8];
-        }
-#pragma unroll
-        for (int q = 0; q < 16; ++q) v[q] += __shfl_down_sync(0xffffffffu, v[q], 8);  // P_hi row + P_lo row
-        if (p.k_log) {  // Kaldi fbank: log(max(mel, FLT_EPSILON)), kaldi.py:629-631
-#pragma unroll
-          for (int q = 0; q < 16; ++q) v[q] = 0.69314718055994531f * __log2f(fmaxf(v[q], kKaldiEps));
-        }
-        if (p.stage == B200A_STAGE_FEAT) {
-          float mx = -CUDART_INF_F;
-          const float scale = p.log_mels ? 0.69314718055994531f : p.db_mult * 0.30102999566398120f;
-          const float offs = p.log_mels ? 0.f : p.db_offset;
-#pragma unroll
-          for (int q = 0; q < 16; ++q) {
-            const float arg = p.log_mels ? v[q] + 1e-6f : fmaxf(v[q], p.db_amin);
-            v[q] = fmaf(scale, __log2f(arg), -offs);
-            if (f0 + q < p.n_mels) mx = fmaxf(mx, v[q]);
-          }
-          gmax.add(g, mx, row_ok);
-        }
-        if (row_ok) {
-          float* dsto = p.out + o + f0;
-          if (p.out_vec >= 4 && f0 + 16 <= p.n_mels) {
-#pragma unroll
-            for (int q = 0; q < 16; q += 4)
-              *reinterpret_cast<float4*>(dsto + q) = make_float4(v[q], v[q + 1], v[q + 2], v[q + 3]);
-          } else {
-#pragma unroll
-            for (int q = 0; q < 16; ++q)
-              if (f0 + q < p.n_mels) dsto[q] = v[q];
-          }
-        }
-      }
-      tc_fence_before();  // my tcgen05.ld are done before this accumulator is handed back
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_tfree + (t & 1));
-    };
-
-    int it = 0;
-    int64_t o_prev = -1, g_prev = -1;
-    for (int64_t base = u0; base < p.total_units; base += stride, ++it) {
-      mbar_wait(s_full, (uint32_t)it & 1u);
-      if (cw == kMelWarps - 1) {
-        // ---- issue: D[it & 1][:, 2 n0 : 2 n0 + 2 N] += [P_hi ; P_lo] [F_hi | F_lo], ONE instruction per k-step ----
-        if (it >= 2) mbar_wait(s_tfree + (it & 1), ((uint32_t)(it >> 1) & 1u) ^ 1u);  // tile it - 2 has left this accumulator
-        tc_fence_after();
-        const uint32_t acc = tmem_d + (uint32_t)(it & 1) * acc_cols;
-#pragma unroll 3
-        for (int s = 0; s < n_steps; ++s) {
-          const TcIssue2 e = s_issue[s];
-          if (elect_one()) umma_bf16(acc + e.col, e.a, e.b, e.idesc, s > 0 ? 1u : 0u);  // step 0 spans every column
-        }
-        if (elect_one()) umma_commit(s_mma);
-        __syncwarp();
-      } else if (cw < kQuads) {
-        // the slots of tile `it` must be read before its MMAs complete (then the transform warps overwrite them)
-        int64_t o_cur = -1, g_cur = -1;
-        if (erow < kRows) {
-          o_cur = s_slot[erow];
-          g_cur = s_grp[erow];
-        }
-        if (it > 0) {  // tile it could only be published after the MMAs of tile it - 1 completed (single operand buffer)
-          tc_fence_after();
-          epilogue(it - 1, o_prev, g_prev);
-        }
-        o_prev = o_cur;
-        g_prev = g_cur;
-      }
-    }
-    if (cw < kQuads && cw != kMelWarps - 1 && it > 0) {
-      mbar_wait(s_mma, (uint32_t)(it - 1) & 1u);
-      tc_fence_after();
-      epilogue(it - 1, o_prev, g_prev);
-    }
-    gmax.flush();
-    tc_fence_before();
-    asm volatile("bar.sync 1, %0;" ::"n"(kMelWarps * 32) : "memory");  // every tcgen05.ld is done
-    if (cw == 0) tmem_dealloc(tmem_d, tmem_cols);
-  }
-}
-
-int tc_b_budget(int n_fft) {
-  return n_fft == 1024 ? Tc2::kBBudget : (n_fft == 512 ? TcGeo<16>::kBBudget : TcGeo<8>::kBBudget);
-}
-
-// The mel / MFCC-feature kernel: tcgen05 contraction when the prepared plan says the banded filterbank fits
-// shared memory (every real mel / linear filterbank does), mma.sync contraction otherwise.
-template <int POWER_MODE, int G, int HG, bool KALDI>
-__global__ void __launch_bounds__(TcGeo<G>::kThreads, 1) stft_pow2_mel_kernel(const Pow2Params p) {
+__global__ void __launch_bounds__((kWarps + kMelWarps) * 32, 1) stft_pow2_mel_kernel(const Pow2Params p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  // 512 threads start with 128 registers each: 8 x 32 x 192 + 4 x 32 x 96 + 4 x 32 x 24 <= 65536
-  constexpr int kMmaFftRegs = TcGeo<G>::kThreads == 512 ? 192 : kFftRegs;
-  if (p.tc != nullptr && p.tc->ok) {
-    if constexpr (G == 32) mel_body_tc2<POWER_MODE, HG, KALDI>(p, smem_raw);
-    else mel_body_tc<POWER_MODE, G, HG, KALDI>(p, smem_raw);
-  } else {
-    mel_body_mma<POWER_MODE, G, HG, kMmaFftRegs, KALDI>(p, smem_raw);
-  }
+  mel_body_mma<POWER_MODE, G, HG, kFftRegs, KALDI>(p, smem_raw);
 }
 
 // ================================================================================================
@@ -1998,15 +1279,6 @@ static_assert(kMaxItemsPerWarp * kMelWarps >= kMaxItems,
 
 }  // namespace
 
-// mel stages of n_fft <= 1024 run their contraction on tcgen05 unless B200A_TC=0 asks for the mma.sync path
-static bool tc_enabled(const b200a_frontend_desc& d) {
-  static const bool enabled = [] {
-    const char* e = std::getenv("B200A_TC");
-    return !(e && e[0] == '0');
-  }();
-  return enabled && d.n_fft <= 1024 && d.onesided && d.n_mels > 0 && d.n_mels <= kTcMaxN;
-}
-
 size_t pow2_workspace_extra(const b200a_frontend_desc* d) {
   if (!pow2_applicable(*d)) return 0;
   const size_t base = ws_layout(*d).total;
@@ -2028,24 +1300,10 @@ int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaSt
                                               mel_tiles(d->n_mels), reinterpret_cast<MelPlan*>(base + e.plan),
                                               reinterpret_cast<float4*>(base + e.frags));
   }
-  if (tc_enabled(*d)) {
-    prepare_tc_kernel<<<1, 256, 0, stream>>>(reinterpret_cast<const float*>(base + l.fb), d->n_fft / 2 + 1, d->n_mels,
-                                             d->n_fft, tc_b_budget(d->n_fft), d->n_fft == 1024 ? 32 : 0,
-                                             reinterpret_cast<TcPlan*>(base + e.tc_plan), base + e.tc_b);
-  }
   return launch_status();
 }
 
-static int num_sms() {
-  static int cached = 0;
-  if (cached == 0) {
-    int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      return -1;
-    cached = n > 0 ? n : 148;
-  }
-  return cached;
-}
+static int num_sms() { return device_sm_count(); }
 
 // persistent: one resident CTA per SM, units dealt round-robin (every CTA gets the same count +-1)
 static int64_t persistent_grid(const Pow2Params& p, int warps = kWarps) {
@@ -2084,14 +1342,12 @@ static int launch_mel(const Pow2Params& p, cudaStream_t stream) {
                       sizeof(int64_t) * 4 * Ge::kSlots + sizeof(uint64_t) * (kWarps + 4) + sizeof(MelPlan) +
                       sizeof(float4) * 32 * kFragSmemSteps;
   if (smem > 227 * 1024) return B200A_EUNSUPPORTED;
-  static_assert(TcGeo<G>::kFixed + TcGeo<G>::kBBudget <= 227 * 1024 && TcGeo<G>::kBBudget >= 24 * 1024, "tcgen05 layout");
-  constexpr int kThreads = TcGeo<G>::kThreads;
   auto kern = p.kaldi ? stft_pow2_mel_kernel<POWER_MODE, G, -1, true> : stft_pow2_mel_kernel<POWER_MODE, G, HG, false>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
     return B200A_ECUDA;
-  const int64_t grid = persistent_grid(p, p.tc != nullptr ? TcGeo<G>::NW : kWarps);
+  const int64_t grid = persistent_grid(p);
   if (grid < 0) return B200A_ECUDA;
-  kern<<<(unsigned)grid, kThreads, p.tc != nullptr ? (size_t)227 * 1024 : smem, stream>>>(p);
+  kern<<<(unsigned)grid, (kWarps + kMelWarps) * 32, smem, stream>>>(p);
   return launch_status();
 }
 
@@ -2168,8 +1424,6 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   p.plan = reinterpret_cast<const MelPlan*>(base + e.plan);
   p.frags = reinterpret_cast<const float4*>(base + e.frags);
   p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
-  p.tc = tc_enabled(*d) ? reinterpret_cast<const TcPlan*>(base + e.tc_plan) : nullptr;
-  p.tc_b = base + e.tc_b;
   p.hop = d->hop;
   p.pad = d->pad;
   p.center = d->center;

@@ -18,13 +18,11 @@
 // Fallback (resample_direct_kernel): one output per thread over the phase's live taps, for ratios whose
 // tables or tiles do not fit (new' > 1024, orig' > ~1100) or mis-aligned inputs.
 //
-// Preferred kernel for odd orig' (resample_simt_kernel, e.g. 44.1 -> 16 kHz): the pruned FIR is only ~68 flop per
-// output sample, far below what keeps the legacy tensor path busy with error-compensated TF32 (3 MMAs per tile,
-// "math pipe throttle" in profiles/r1_resample_v4.txt), so it runs as a register-tiled FP32 product on packed
-// FFMA2 instead: a thread owns ONE frame of each of two adjacent 32-frame half-chunks x a group of 8 phases,
-// lanes are consecutive frames (stride orig' words: conflict-free for odd orig'), the 8 taps of a step are one
-// 32-byte broadcast read, and the two frames ride in the two halves of an f32x2 register pair:
-//     acc[q] (frame a | frame b) += (x_a[i] | x_b[i]) * tap[q][i]      (FFMA2 with a scalar-broadcast operand)
+// SIMT variant for odd orig' (resample_simt_kernel, opt-in, e.g. 44.1 -> 16 kHz): the pruned FIR is only ~68 flop
+// per output sample, so it runs as a register-tiled FP32 product: a thread owns ONE frame of each of two adjacent
+// 32-frame half-chunks x a group of 8 phases, lanes are consecutive frames (stride orig' words: conflict-free for odd
+// orig'), the 8 taps of a step are one 32-byte broadcast read, and the two frames are a register pair (f32x2.cuh):
+//     acc[q] (frame a | frame b) += (x_a[i] | x_b[i]) * tap[q][i]
 // Half-chunks stream through a 3-slot ring of bulk asynchronous copies.  Step s pairs half-chunks (s-1, s) and
 // handles the phase groups of parity s & 1, so every half-chunk meets both parities (once as the newer, once as
 // the older member of a pair) and a slot is free for the next copy as soon as its second step ends.
@@ -58,16 +56,14 @@ struct RsHeader {
   int32_t simt_tap_floats;  // size of the SIMT tap table (floats)
   int32_t total_steps16;    // 16-tap steps over all groups (bf16 fragments)
   int32_t r3_ok;            // 1: every group of 4 phases spans at most kR3Len taps (resample_r3_kernel applies)
-  int32_t tc_ok;            // 1: the banded tcgen05 plan fits (resample_tc_kernel applies)
-  int32_t reserved[4];
+  int32_t reserved[5];
 };
 static_assert(sizeof(RsHeader) == 64, "header is 64 bytes");
 
 struct RsLayout {
-  size_t header, support, tiles, frags, frags16, sgroups, staps, r3base, r3taps, tcplan, tcblocks, total;
+  size_t header, support, tiles, frags, frags16, sgroups, staps, r3base, r3taps, total;
 };
 
-constexpr int kTcBBudgetBytes = 64 * 1024;  // banded tap blocks of the tcgen05 kernel
 constexpr int kR3Len = 44;      // taps per phase quad held in registers (34 live + 3 x 2.76 drift at 441:160, padded)
 constexpr int kR3Warps = 8;     // warps per CTA == phase quads per CTA (a multiple of 4: registers are granted per 4 warps)
 constexpr int kR3MaxCluster = 8;
@@ -104,10 +100,6 @@ inline RsLayout rs_layout(int new_r, int taps) {
   off = align_up(off + sizeof(int) * quads, 256);
   l.r3taps = off;
   off = align_up(off + sizeof(float4) * kR3Len * quads, 256);
-  l.tcplan = off;  // (spare) + the banded bf16 tap blocks of resample_tc_kernel
-  off = align_up(off + 1024, 256);
-  l.tcblocks = off;
-  off = align_up(off + (size_t)kTcBBudgetBytes, 256);
   l.total = off;
   return l;
 }
@@ -230,7 +222,7 @@ struct RsParams {
   int xs_floats;            // floats per staging buffer
   int frag_smem_bytes;      // shared memory granted to the fragment copy (0: read them from global)
   int row_spread;           // 1, 2 or 4: frame distance of the 8 rows one A-fragment load touches
-  int skip_if_r3_ok;        // launched behind resample_r3_kernel (1) / resample_tc_kernel (2): leave when the header says that kernel did the work
+  int skip_if_r3_ok;        // launched behind resample_r3_kernel: leave when the header says that kernel did the work
 };
 
 // Fill one staging buffer with the samples frames [f0, f0 + 32) of `row` need:
@@ -294,7 +286,7 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
 }
 
 // BF16 == false: m16n8k8 TF32 x 3 (2^-21 relative);  BF16 == true: m16n8k16 bf16 x 3 (2^-16 relative, half the
-// tensor-pipe time: the TF32 variant is throttled by the math pipe, profiles/r1_resample_v4.txt)
+// tensor-pipe time: the TF32 variant issues three MMAs per tile)
 template <bool BF16>
 __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_mma_kernel(const RsParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -304,7 +296,7 @@ __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_mma_kernel(const
   float4* s_frags = reinterpret_cast<float4*>(s_tiles + ((p.n_tiles + 3) & ~3));  // optional
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if ((p.skip_if_r3_ok == 1 && p.hdr->r3_ok != 0) || (p.skip_if_r3_ok == 2 && p.hdr->tc_ok != 0)) return;
+  if (p.skip_if_r3_ok && p.hdr->r3_ok != 0) return;
   for (int i = tid; i < p.n_tiles; i += blockDim.x) s_tiles[i] = p.tiles[i];
   const int total_steps = BF16 ? p.hdr->total_steps16 : p.hdr->total_steps;
   const bool frags_in_smem = (size_t)total_steps * 512 <= (size_t)p.frag_smem_bytes;
@@ -706,9 +698,9 @@ __global__ void resample_r3_plan_kernel(const float* __restrict__ kernel, const 
 // ================================================================================================
 // Cluster kernel (resample_r3_kernel): the taps never leave the register file.
 //   A register-tiled FIR is bound by shared-memory wavefronts unless BOTH operands of an FMA are reused from
-//   registers (docs/KERNEL_NOTES.md).  Here a warp owns ONE quad of 4 output phases for the whole kernel and keeps
+//   registers.  Here a warp owns ONE quad of 4 output phases for the whole kernel and keeps
 //   its 4 x kR3Len taps in 176 registers; lanes are the 32 frames of a tile, so the only shared-memory traffic is one
-//   conflict-free 4-byte read per tap position, feeding two FFMA2 (4 phases) with the sample as the broadcast operand.
+//   conflict-free 4-byte read per tap position, feeding four FFMA (4 phases) with the sample as the broadcast operand.
 //   160 phases = 40 quads need 40 such warps; at ~200 registers per thread an SM holds 8 (registers are granted per 4
 //   warps: 10 x 200 does not fit), so a CLUSTER of 5 CTAs covers the phases and shares every staged tile: each CTA
 //   fetches a fifth of the tile's samples with ONE bulk copy that is MULTICAST into the same offset of all the CTAs'
@@ -929,582 +921,9 @@ resample_direct_kernel(const float* __restrict__ wave, int64_t length, int64_t r
   }
 }
 
-// ================================================================================================
-// tcgen05 kernel (resample_tc_kernel): the banded product  Y[f][j] = sum_i X[f][i] K[j][i]  on the 5th-generation
-// tensor cores.
-//   The strided view X[f][i] = xp[f orig' + i] cannot be described to the tensor core (its rows are orig' samples apart,
-//   a K-major core matrix wants them 16 bytes apart), so twelve CONVERT warps materialise it per 32-frame tile as a
-//   K-major bf16 operand in shared memory -- the error-compensated hi and lo planes of a frame being two ROWS of the
-//   same M = 64 tile, like the mel contraction (frontend_pow2.cu, mel_body_tc2) -- from the tile's contiguous
-//   samples, which a producer warp stages with bulk asynchronous copies in four 8-frame units (a unit's buffer is
-//   re-filled with the next tile's unit as soon as its convert pass is over).  That is an 8 % expansion (475 taps per
-//   441 new samples), read conflict free (lane = frame x 4 consecutive chunks; frames orig' words apart, orig' odd) and
-//   written as whole 16-byte core-matrix rows.  The operand is double buffered: tile n + 1 is converted while the
-//   tensor core multiplies tile n.
-//   One thread issues, per 16-tap k-step, TWO tcgen05.mma (taps_hi, taps_lo accumulate into the same columns) whose
-//   B operand holds only the phases that have live taps in that step, banded like the mel filterbank: 60 instructions
-//   of N = 8..32 per tile instead of 960 legacy HMMAs.  The accumulator (<= 160 columns) is double buffered in tensor
-//   memory; eight epilogue warps (two per TMEM lane quadrant, half the columns each) read it (tcgen05.ld), add the
-//   hi / lo ROWS of a frame with one shuffle and store 64 bytes per thread.
-//   Shared memory at 441:160: 2 x 60 KB operand + 43 KB taps + 4 x 14 KB staged; HBM traffic = the algorithmic bytes.
-//   Arithmetic: bf16 x 3 (x_hi k_hi + x_hi k_lo + x_lo k_hi + x_lo k_lo), FP32 accumulate: ~5e-6 of the peak.
-// ================================================================================================
-constexpr int kTcFrames = 32;          // frames per tile (x 2 planes = the 64 rows of one MMA)
-constexpr int kTcUnit = 8;             // frames per staged unit
-constexpr int kTcUnits = kTcFrames / kTcUnit;
-constexpr int kTcSlots = kTcUnits;  // staged units: slot u holds unit u of the current / next tile
-constexpr int kTcMaxKSteps = 30;       // 16-tap k-steps
-constexpr int kTcAStride = 1024;       // bytes per 8-tap chunk: 8 row groups x 128 B ([hi | lo] of four 8-frame groups)
-// Warp roles by scheduler (warp % 4): the issuer shares its scheduler with one epilogue warp and the (mostly
-// sleeping) producer only -- a tcgen05.mma costs ~10 issue slots of that one thread, and behind five busy warps the 61
-// instructions of a tile took 6100 cycles instead of 1800.
-//   warps 0-3 epilogue (TMEM lane quadrant = warp), 7 issuer, 11 producer, the other warps with warp % 4 != 3 convert
-//   (12 of them); warp 15 has no role
-#ifndef B200A_TC_EPI
-#define B200A_TC_EPI 4
-#endif
-#ifndef B200A_TC_PACKED_SHFL
-#define B200A_TC_PACKED_SHFL 0  // measured: 5 % fewer L1TEX cycles, no time gained, 2.3x the rounding error
-#endif
-constexpr int kTcConvWarps = 12, kTcEpiWarps = B200A_TC_EPI;  // 4: one per TMEM lane quadrant; 8: two, half the columns each
-constexpr int kTcWarps = kTcEpiWarps + 15;
-constexpr int kTcThreads = kTcWarps * 32;
-constexpr int kTcIssuerWarp = kTcEpiWarps + 3, kTcProducerWarp = kTcEpiWarps + 7;
-#ifndef B200A_TC_PREFETCH
-#define B200A_TC_PREFETCH 0
-#endif
-constexpr int kTcPrefetchTiles = B200A_TC_PREFETCH;  // tiles pulled into L2 ahead of the staged one (measured: no gain)
-constexpr int kTcMaxPhases = 160;      // columns of one accumulator
-constexpr int kTcAccStride = 256;      // TMEM columns between the two accumulators
-constexpr int kTcSmemLimit = 227 * 1024;
-constexpr int kTcIssueBytes = 2 * (2 * kTcMaxKSteps + 2) * 16;  // per accumulator / operand buffer: one uint4 per MMA
-
-struct RsTcSmem {  // byte offsets into dynamic shared memory
-  int n_chunks, a_bytes, zero_off, b_off, b_room, x_off, slot_floats, issue_off, bar_off, total;
-};
-__host__ __device__ inline RsTcSmem rs_tc_smem(int orig_r, int taps) {
-  RsTcSmem m;
-  m.n_chunks = 2 * ((taps + 15) / 16);
-  m.a_bytes = m.n_chunks * kTcAStride;  // one operand buffer; two of them at offset 0
-  m.zero_off = 2 * m.a_bytes;           // one all-zero k-step (the accumulator is cleared by multiplying with it)
-  m.b_off = m.zero_off + 2 * kTcAStride;
-  m.slot_floats = ((kTcUnit - 1) * orig_r + 8 * m.n_chunks + 3 + 3 + 8 + 3) & ~3;  // span + shift + round-up + slack
-  const int tail = kTcSlots * m.slot_floats * 4 + kTcIssueBytes + 256;  // + barriers and the unit records
-  int room = (kTcSmemLimit - m.b_off - tail) & ~127;
-  if (room > kTcBBudgetBytes) room = kTcBBudgetBytes;
-  m.b_room = room;  // (<= 0: does not fit)
-  m.x_off = m.b_off + (room > 0 ? room : 0);
-  m.issue_off = m.x_off + kTcSlots * m.slot_floats * 4;
-  m.bar_off = m.issue_off + kTcIssueBytes;
-  m.total = m.bar_off + 256;
-  return m;
-}
-
-struct RsTcStep {
-  uint32_t b_off;  // byte offset of the step's tap blocks: [taps_hi: n rows][taps_lo: n rows], each K-major
-  uint32_t n;      // phases covered (multiple of 8)
-  uint32_t col;    // first phase (multiple of 8)
-  uint32_t kstep;  // 16-tap step of the A operand
-};
-// The band structure, computed on the HOST from (orig', new', width) alone so that the issuing thread reads its
-// descriptors from kernel parameters (uniform loads, no register -> uniform-register moves): phase j can have live
-// taps only in (j orig'/new', j orig'/new' + 2 width) -- the window of the reference kernel is zero outside +-lowpass
-// width and width = ceil(that width x orig'/cutoff) (functional.py:1467-1472, 1514-1519).  The plan kernel checks the
-// measured support against this band and clears hdr->tc_ok when a caller's kernel does not honour it.
-struct RsTcSteps {
-  int ok, steps, b_bytes, n_pad;
-  RsTcStep step[kTcMaxKSteps];
-};
-inline void rs_tc_band(int j, int orig_r, int new_r, int width, int& first, int& last) {  // live taps of phase j: [first, last]
-  first = (int)(((int64_t)j * orig_r) / new_r);
-  last = (int)(((int64_t)j * orig_r + new_r - 1) / new_r) + 2 * width;
-}
-inline RsTcSteps rs_tc_steps(int orig_r, int new_r, int width) {
-  RsTcSteps t{};
-  const int taps = 2 * width + orig_r, k_steps = (taps + 15) / 16;
-  const RsTcSmem m = rs_tc_smem(orig_r, taps);
-  if (k_steps > kTcMaxKSteps || new_r > kTcMaxPhases || m.b_room <= 0) return t;
-  int off = 0;
-  for (int s = 0; s < k_steps; ++s) {
-    const int t0 = 16 * s, t1 = t0 + 16;
-    int lo = new_r, hi = -1;
-    for (int j = 0; j < new_r; ++j) {
-      int first, last;
-      rs_tc_band(j, orig_r, new_r, width, first, last);
-      if (first < t1 && last >= t0) {
-        if (j < lo) lo = j;
-        hi = j;
-      }
-    }
-    if (hi < 0) continue;
-    const int n0 = lo / 8 * 8, n = (hi + 1 - n0 + 7) / 8 * 8;
-    t.step[t.steps++] = RsTcStep{(uint32_t)off, (uint32_t)n, (uint32_t)n0, (uint32_t)s};
-    off += n * 64;
-  }
-  t.b_bytes = off;
-  t.n_pad = (new_r + 7) / 8 * 8;
-  // the accumulator is cleared by multiplying an all-zero A k-step with the first n_pad rows of the tap blocks
-  t.ok = (t.steps > 0 && off <= m.b_room && off >= t.n_pad * 32) ? 1 : 0;
-  return t;
-}
-
-// One MMA of a tile as the issuing thread needs it (low descriptor words relative to the operand bases)
-struct RsTcMma {
-  uint32_t a_lo, b_lo, idesc, col;
-};
-struct RsTcIssueTab {
-  int count, n_pad, b_bytes, count_lo;  // count_lo: MMAs of the low-K half (k-steps < lo_chunks / 2)
-  int lo_chunks, pad0, pad1, pad2;
-  RsTcMma clear;
-  RsTcMma m[2 * kTcMaxKSteps];
-};
-constexpr uint32_t kTcDescHi = (128u >> 4) | (1u << 14);  // SBO = 128 bytes, descriptor version 1 (bit 46)
-inline RsTcIssueTab rs_tc_issue_tab(const RsTcSteps& t, int n_chunks) {
-  RsTcIssueTab tab{};
-  tab.count = 2 * t.steps;
-  tab.n_pad = t.n_pad;
-  tab.b_bytes = t.b_bytes;
-  tab.lo_chunks = (n_chunks / 4 + 1) / 2 * 4;  // whole items (4 chunks = 2 k-steps)
-  tab.count_lo = 0;
-  for (int s = 0; s < t.steps; ++s)
-    if ((int)t.step[s].kstep * 2 < tab.lo_chunks) tab.count_lo = 2 * (s + 1);
-  tab.clear = RsTcMma{(uint32_t)(kTcAStride >> 4) << 16, (uint32_t)((t.n_pad * 16) >> 4) << 16,
-                      umma_idesc_bf16(64, t.n_pad), 0u};
-  for (int s = 0; s < t.steps; ++s)
-    for (int pl = 0; pl < 2; ++pl) {
-      const RsTcStep& st = t.step[s];
-      RsTcMma& e = tab.m[2 * s + pl];
-      e.a_lo = ((st.kstep * 2 * kTcAStride) >> 4) | ((uint32_t)(kTcAStride >> 4) << 16);
-      e.b_lo = ((st.b_off + pl * st.n * 32) >> 4) | ((uint32_t)((st.n * 16) >> 4) << 16);
-      e.idesc = umma_idesc_bf16(64, (int)st.n);
-      e.col = st.col;
-    }
-  return tab;
-}
-
-// Fills the banded bf16 hi / lo tap blocks of the host-side plan and checks every phase's measured support against
-// the band the plan assumes.
-__global__ void resample_tc_plan_kernel(const float* __restrict__ kernel, const int2* __restrict__ support, int orig_r,
-                                        int new_r, int width, int taps, const RsTcSteps plan, RsHeader* hdr,
-                                        unsigned char* blocks) {
-  __shared__ int s_bad;
-  if (threadIdx.x == 0) s_bad = plan.ok ? 0 : 1;
-  __syncthreads();
-  if (plan.ok) {
-    for (int j = threadIdx.x; j < new_r; j += blockDim.x) {
-      const int2 sp = support[j];
-      const int first = (int)(((int64_t)j * orig_r) / new_r);
-      const int last = (int)(((int64_t)j * orig_r + new_r - 1) / new_r) + 2 * width;
-      if (sp.y > 0 && (sp.x < first || sp.x + sp.y - 1 > last)) s_bad = 1;
-    }
-    for (int s = 0; s < plan.steps; ++s) {
-      const RsTcStep st = plan.step[s];
-      for (int i = threadIdx.x; i < (int)st.n * 16; i += blockDim.x) {
-        const int nl = i >> 4, kk = i & 15;
-        const int j = (int)st.col + nl, t = 16 * (int)st.kstep + kk;
-        float v = 0.f;
-        if (j < new_r && t < taps) {
-          const int2 sp = support[j];
-          if (t >= sp.x && t < sp.x + sp.y) v = kernel[(size_t)j * taps + t];
-        }
-        uint32_t h, l;
-        rs_split_bf16x2(v, 0.f, h, l);
-        const size_t o = st.b_off + (size_t)(kk >> 3) * st.n * 16 + (size_t)nl * 16 + (size_t)(kk & 7) * 2;
-        *reinterpret_cast<uint16_t*>(blocks + o) = (uint16_t)(h & 0xffffu);
-        *reinterpret_cast<uint16_t*>(blocks + o + (size_t)st.n * 32) = (uint16_t)(l & 0xffffu);
-      }
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) hdr->tc_ok = s_bad ? 0 : 1;
-}
-
-struct RsTcParams {
-  long long* trace;  // B200A_TC_TRACE builds: [16 tiles][16 events] clock64 stamps of CTA 0 (else unused)
-  const float* wave;
-  int64_t rows, length, row_stride;
-  float* out;
-  int64_t out_row_stride, out_len;
-  const RsHeader* hdr;
-  const unsigned char* blocks;
-  int orig_r, new_r, width, taps;
-  int64_t frames, tiles_per_row, total_tiles;
-  int out_vec;
-};
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]), "=f"(v[8]),
-        "=f"(v[9]), "=f"(v[10]), "=f"(v[11]), "=f"(v[12]), "=f"(v[13]), "=f"(v[14]), "=f"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-// after tcgen05.wait::ld: ties the registers to the wait so that no consumer is scheduled ahead of it
-__device__ __forceinline__ void tmem_ld_pin(float (&v)[16]) {
-  asm volatile(""
-               : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]),
-                 "+f"(v[8]), "+f"(v[9]), "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15])
-               :
-               : "memory");
-}
-
-#ifdef B200A_TC_TRACE
-#define TC_STAMP(n, ev) do { if (blockIdx.x == 0 && (n) < 16 && lane == 0 && p.trace) p.trace[(n) * 16 + (ev)] = clock64(); } while (0)
-#else
-#define TC_STAMP(n, ev) do { } while (0)
-#endif
-
-__global__ void __launch_bounds__(kTcThreads, 1) resample_tc_kernel(const RsTcParams p, const __grid_constant__ RsTcIssueTab tab,
-                                                                    int require_flag) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  if (require_flag && p.hdr->tc_ok == 0) return;  // (uniform) the mma.sync kernel launched next does the work
-  const RsTcSmem m = rs_tc_smem(p.orig_r, p.taps);
-  unsigned char* s_a = smem_raw;                                              // [2][n_chunks][1024]
-  unsigned char* s_zero = smem_raw + m.zero_off;                              // [2][1024]
-  unsigned char* s_b = smem_raw + m.b_off;                                    // tap blocks
-  float* s_x = reinterpret_cast<float*>(smem_raw + m.x_off);                  // [kTcSlots][slot_floats]
-  uint4* s_issue = reinterpret_cast<uint4*>(smem_raw + m.issue_off);          // [2][2 kTcMaxKSteps + 2]
-  uint64_t* s_full = reinterpret_cast<uint64_t*>(smem_raw + m.bar_off);       // [4] staged unit landed
-  uint64_t* s_cdone = s_full + kTcSlots;                                      // [4] unit u converted by every warp (slot u free)
-  uint64_t* s_aready = s_cdone + kTcSlots;                                    // [2] operand b complete (all convert warps)
-  uint64_t* s_mma = s_aready + 2;                                             // [2] MMAs of buffer b complete: D[b] valid, A[b] free
-  uint64_t* s_accfree = s_mma + 2;                                            // [2] accumulator b read out
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_accfree + 2);
-  int* s_shift = reinterpret_cast<int*>(smem_raw + m.bar_off + 192);          // [4] slot index of the unit's sample T0
-
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int n_pad = tab.n_pad;
-  const int n_chunks = m.n_chunks;
-  {
-    uint4* a4 = reinterpret_cast<uint4*>(s_a);
-    for (int i = tid; i < m.b_off / 16; i += blockDim.x) a4[i] = make_uint4(0, 0, 0, 0);  // both operands + the zero k-step
-    const uint4* src = reinterpret_cast<const uint4*>(p.blocks);
-    uint4* b4 = reinterpret_cast<uint4*>(s_b);
-    for (int i = tid; i < tab.b_bytes / 16; i += blockDim.x) b4[i] = src[i];
-    uint4* x4 = reinterpret_cast<uint4*>(s_x);  // frames past the end of a row are converted from whatever the slot holds: keep it finite
-    for (int i = tid; i < kTcSlots * m.slot_floats / 4; i += blockDim.x) x4[i] = make_uint4(0, 0, 0, 0);
-  }
-  // issue records {A descriptor low word, B descriptor low word, instruction descriptor, D column}, final for each
-  // of the two (operand, accumulator) buffers: the issuing thread spends one 16-byte load + four moves per MMA
-  if (tid <= tab.count) {
-    const RsTcMma e = tid == 0 ? tab.clear : tab.m[tid - 1];
-    const uint32_t b_base = smem_u32(s_b) >> 4;
-    for (int b = 0; b < 2; ++b) {
-      const uint32_t a_base = (tid == 0 ? smem_u32(s_zero) : smem_u32(s_a) + (uint32_t)(b * m.a_bytes)) >> 4;
-      s_issue[b * (2 * kTcMaxKSteps + 2) + tid] =
-          make_uint4(e.a_lo + a_base, e.b_lo + b_base, e.idesc, (uint32_t)(b * kTcAccStride) + e.col);
-    }
-  }
-  if (tid == 0) {
-    for (int i = 0; i < kTcSlots; ++i) {
-      mbar_init(s_full + i, 1);
-      mbar_init(s_cdone + i, kTcConvWarps);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(s_aready + i, kTcConvWarps);
-      mbar_init(s_mma + i, 1);
-      mbar_init(s_accfree + i, kTcEpiWarps);
-    }
-  }
-  if (warp == 0) tmem_alloc(s_tmem, 512);  // two accumulators of <= 160 columns, kTcAccStride apart
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-
-  // tiles of this CTA: t = blockIdx.x + n gridDim.x; unit u covers frames f0 + 8 u .. + 7
-  auto tile_of = [&](int n, int64_t& row, int64_t& f0) {
-    const int64_t t = blockIdx.x + (int64_t)n * gridDim.x;
-    if (t >= p.total_tiles) return false;
-    if (p.total_tiles < ((int64_t)1 << 31)) {
-      const uint32_t r = (uint32_t)t / (uint32_t)p.tiles_per_row;
-      row = r;
-      f0 = (int64_t)((uint32_t)t - r * (uint32_t)p.tiles_per_row) * kTcFrames;
-    } else {
-      row = t / p.tiles_per_row;
-      f0 = (t - row * p.tiles_per_row) * kTcFrames;
-    }
-    return true;
-  };
-
-  if (warp < kTcEpiWarps) {
-    // ============ epilogue warps: TMEM lane quadrant warp % 4; with eight of them, column half warp / 4 ===========
-    const int cw = warp & 3, ch = warp >> 2;
-    const int split = kTcEpiWarps == 8 ? (n_pad / 32 + 1) / 2 * 32 : n_pad;  // whole 32-column passes: [0, split), [split, n_pad)
-    const int j_first = ch ? split : 0, j_last = ch ? n_pad : (split < n_pad ? split : n_pad);
-    int64_t row, f0;
-    for (int n = 0; tile_of(n, row, f0); ++n) {
-      const int b = n & 1;
-      if (warp == 0) TC_STAMP(n, 0);
-      mbar_wait(s_mma + b, (uint32_t)(n >> 1) & 1u);
-      if (warp == 0) TC_STAMP(n, 1);
-      tc_fence_after();
-      const uint32_t acc = tmem_d + ((uint32_t)(32 * cw) << 16) + (uint32_t)(b * kTcAccStride);
-      const int64_t f = f0 + 8 * cw + (lane & 7);  // lanes 0-7: hi rows of frames 8 cw .. 8 cw + 7, lanes 8-15: their lo rows
-      const bool own = lane < 8 && f < p.frames;
-      float* orow = p.out + row * p.out_row_stride + f * p.new_r;
-      const int64_t n0 = f * p.new_r;
-      auto store16 = [&](int j, const float (&y)[16]) {
-        if (p.out_vec && j + 16 <= j_last && j + 16 <= p.new_r && n0 + j + 16 <= p.out_len) {
-#pragma unroll
-          for (int q = 0; q < 16; q += 4)
-            *reinterpret_cast<float4*>(orow + j + q) = make_float4(y[q], y[q + 1], y[q + 2], y[q + 3]);
-        } else {
-#pragma unroll
-          for (int q = 0; q < 16; ++q)
-            if (j + q < j_last && j + q < p.new_r && n0 + j + q < p.out_len) orow[j + q] = y[q];
-        }
-      };
-      auto finish32 = [&](int j, float (&u)[16], float (&w)[16]) {
-#if B200A_TC_PACKED_SHFL
-        // x_hi row + x_lo row.  The x_lo row is a 2^-9 correction: it crosses the lanes as bf16 pairs (2^-18 of the
-        // result), which halves the shuffles -- the shared-memory / shuffle pipe is the busiest unit of this kernel.
-#pragma unroll
-        for (int q = 0; q < 16; q += 2) {
-          uint32_t pu, pw;
-          asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(pu) : "f"(u[q + 1]), "f"(u[q]));
-          asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(pw) : "f"(w[q + 1]), "f"(w[q]));
-          pu = __shfl_down_sync(0xffffffffu, pu, 8);
-          pw = __shfl_down_sync(0xffffffffu, pw, 8);
-          u[q] += __uint_as_float(pu << 16);
-          u[q + 1] += __uint_as_float(pu & 0xffff0000u);
-          w[q] += __uint_as_float(pw << 16);
-          w[q + 1] += __uint_as_float(pw & 0xffff0000u);
-        }
-#else
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-          u[q] += __shfl_down_sync(0xffffffffu, u[q], 8);  // x_hi row + x_lo row
-          w[q] += __shfl_down_sync(0xffffffffu, w[q], 8);
-        }
-#endif
-        if (own) {
-          store16(j, u);
-          store16(j + 16, w);
-        }
-      };
-      // two register sets: the tensor-memory load of the next 32 columns is in flight while these are summed and stored
-      float ua[16], wa[16], ub[16], wb[16];
-      tmem_ld16_nowait(acc + j_first, ua);
-      tmem_ld16_nowait(acc + j_first + 16, wa);  // (columns past n_pad: allocated, never stored)
-#pragma unroll 1
-      for (int j0 = j_first; j0 < j_last; j0 += 64) {
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        tmem_ld_pin(ua);
-        tmem_ld_pin(wa);
-        if (j0 + 32 < j_last) {
-          tmem_ld16_nowait(acc + j0 + 32, ub);
-          tmem_ld16_nowait(acc + j0 + 48, wb);
-        }
-        finish32(j0, ua, wa);
-        if (j0 + 32 < j_last) {
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          tmem_ld_pin(ub);
-          tmem_ld_pin(wb);
-          if (j0 + 64 < j_last) {
-            tmem_ld16_nowait(acc + j0 + 64, ua);
-            tmem_ld16_nowait(acc + j0 + 80, wa);
-          }
-          finish32(j0 + 32, ub, wb);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (warp == 0) TC_STAMP(n, 2);
-      if (lane == 0) mbar_arrive(s_accfree + b);
-    }
-    tc_fence_before();
-    asm volatile("bar.sync 1, %0;" ::"n"(kTcEpiWarps * 32) : "memory");
-    if (warp == 0) tmem_dealloc(tmem_d, 512);
-  } else if (warp == kTcIssuerWarp) {
-    // ============ issuer warp ======================================================================================
-    const bool leader = elect_one();  // ONE thread issues every instruction of the CTA
-    auto desc = [](uint32_t lo) { return ((uint64_t)kTcDescHi << 32) | lo; };
-    int64_t row, f0;
-    for (int n = 0; tile_of(n, row, f0); ++n) {
-      const int b = n & 1;
-      const uint4* rec = s_issue + b * (2 * kTcMaxKSteps + 2);
-      mbar_wait(s_aready + b, (uint32_t)(n >> 1) & 1u);  // every convert warp is through with the tile: operand complete
-      TC_STAMP(n, 10);
-      if (n >= 2) mbar_wait(s_accfree + b, (uint32_t)((n >> 1) - 1) & 1u);  // tile n - 2 has left this accumulator
-      TC_STAMP(n, 11);
-      tc_fence_after();
-      if (leader) {
-        {
-          const uint4 e = rec[0];
-          umma_bf16(tmem_d + e.w, desc(e.x), desc(e.y), e.z, 0u);  // clear: D = 0 x taps
-        }
-#pragma unroll 4
-        for (int s = 1; s <= tab.count; ++s) {
-          const uint4 e = rec[s];
-          umma_bf16(tmem_d + e.w, desc(e.x), desc(e.y), e.z, 1u);
-        }
-        umma_commit(s_mma + b);
-      }
-      __syncwarp();
-      TC_STAMP(n, 12);
-    }
-  } else if (warp == kTcProducerWarp) {
-    // ============ producer warp: unit u of tile n + 1 follows unit u of tile n into slot u ==========================
-    // Everything a convert warp reads is put into the slot here: the 16-byte aligned middle by ONE bulk copy, and at
-    // the ends of a row the few samples around it and the zeros beyond the signal by this warp (interior units: none).
-    auto stage_unit = [&](int n, int u) {
-      int64_t row, f0;
-      if (!tile_of(n, row, f0)) return;
-      const int slot = u;
-      const float* x = p.wave + row * p.row_stride;
-      const int64_t T0 = (f0 + kTcUnit * u) * p.orig_r - p.width;
-      const int a0 = (int)((reinterpret_cast<uintptr_t>(x) >> 2) & 3);
-      const int shift = (int)((a0 + (T0 & 3)) & 3);  // slot index of sample T0: the bulk copy keeps its 16-byte phase
-      // frames of the unit that exist; the others are converted from stale (finite) slot contents and never stored
-      int64_t nv = p.frames - (f0 + kTcUnit * u);
-      nv = nv < 0 ? 0 : (nv > kTcUnit ? kTcUnit : nv);
-      const int span_v = nv > 0 ? (int)(nv - 1) * p.orig_r + 8 * n_chunks : 0;
-      int64_t lo = T0 < 0 ? 0 : T0, hi = T0 + span_v;
-      if (hi > p.length) hi = p.length;
-      if (lo > p.length) lo = p.length;
-      if (hi < lo) hi = lo;
-      // 16-byte boundaries OUTSIDE [lo, hi) where the signal has them, inside at the ends of a row
-      const int back = (int)((a0 + lo) & 3), fwd = (int)((4 - ((a0 + hi) & 3)) & 3);
-      int64_t lo_a = lo - back >= 0 ? lo - back : lo + ((4 - back) & 3);
-      int64_t hi_a = hi + fwd <= p.length ? hi + fwd : hi - ((a0 + hi) & 3);
-      if (hi_a < lo_a) hi_a = lo_a;
-      float* xs = s_x + slot * m.slot_floats;
-      const int first = (int)(lo_a - T0) + shift, end = (int)(hi_a - T0) + shift;  // staged by the bulk copy: [first, end)
-      for (int i = shift + lane; i < first; i += 32) {
-        const int64_t g = T0 + (i - shift);
-        xs[i] = (g >= 0 && g < p.length) ? __ldg(x + g) : 0.f;
-      }
-      for (int i = (end > shift ? end : shift) + lane; i < shift + span_v; i += 32) {
-        const int64_t g = T0 + (i - shift);
-        xs[i] = (g >= 0 && g < p.length) ? __ldg(x + g) : 0.f;
-      }
-      if (lane == 0) s_shift[slot] = shift;
-      __syncwarp();
-      if (lane == 0) {
-        uint64_t* bar = s_full + slot;
-        if (hi_a > lo_a) {
-          const uint32_t bytes = (uint32_t)(hi_a - lo_a) * 4u;
-          mbar_expect_tx(bar, bytes);  // (release: the stores above are visible to whoever sees the phase complete)
-          bulk_g2s(xs + first, x + lo_a, bytes, bar);
-        } else {
-          mbar_arrive(bar);
-        }
-      }
-    };
-    // Shared memory holds one tile of samples (57 KB per SM, 8 MB over the GPU): less than HBM latency x bandwidth,
-    // so the tiles after the staged one are pulled into L2 ahead of time.
-    auto prefetch_tile = [&](int n) {
-      int64_t row, f0;
-      if (kTcPrefetchTiles == 0 || !tile_of(n, row, f0)) return;
-      const float* x = p.wave + row * p.row_stride;
-      const int64_t T0 = f0 * p.orig_r - p.width;
-      int64_t lo = T0 < 0 ? 0 : T0, hi = T0 + (int64_t)(kTcFrames - 1) * p.orig_r + 8 * n_chunks;
-      if (hi > p.length) hi = p.length;
-      lo += (4 - ((reinterpret_cast<uintptr_t>(x + lo) >> 2) & 3)) & 3;  // 16-byte aligned start, whole 16-byte pieces
-      const int64_t cnt = (hi - lo) & ~(int64_t)3;
-      if (lane == 0 && cnt > 0) bulk_prefetch_l2(x + lo, (uint32_t)cnt * 4u);
-    };
-    for (int u = 0; u < kTcUnits; ++u) stage_unit(0, u);
-    for (int d = 1; d <= kTcPrefetchTiles; ++d) prefetch_tile(d);
-    int64_t row, f0;
-    for (int n = 0; tile_of(n, row, f0); ++n) {
-      prefetch_tile(n + 1 + kTcPrefetchTiles);
-#pragma unroll 1
-      for (int u = 0; u < kTcUnits; ++u) {
-        mbar_wait(s_cdone + u, (uint32_t)n & 1u);
-        if (u == 0) TC_STAMP(n, 9);
-        stage_unit(n + 1, u);
-      }
-    }
-  } else if ((warp & 3) != 3 && warp >= kTcEpiWarps) {
-    // ============ convert warps: staged samples -> K-major bf16 hi / lo operand ====================================
-    const int cv = ((warp - kTcEpiWarps) >> 2) * 3 + (warp & 3);  // the warps after the epilogue's with warp % 4 != 3 -> 0 .. 11
-    const int fl = lane & 7, cq = lane >> 3;  // frame of the unit; this lane converts chunk 4 it + cq
-    const int ipu = (n_chunks + 3) / 4;       // items per unit (an item = 8 frames x 4 consecutive chunks)
-    const int lane_off = fl * p.orig_r;
-    int64_t row, f0;
-    for (int n = 0; tile_of(n, row, f0); ++n) {
-      const int b = n & 1;
-      if (cv == 0) TC_STAMP(n, 3);
-      if (n >= 2) mbar_wait(s_mma + b, (uint32_t)((n >> 1) - 1) & 1u);  // tile n - 2 has been multiplied: operand b is free
-      if (cv == 0) TC_STAMP(n, 4);
-      unsigned char* abuf = s_a + b * m.a_bytes;
-      int it = cv;  // items of the tile in unit order, dealt round robin: g = u ipu + it belongs to warp g % kTcConvWarps
-#pragma unroll 1
-      for (int u = 0; u < kTcUnits; ++u) {
-        mbar_wait(s_full + u, (uint32_t)n & 1u);  // the unit's samples are staged (every warp waits, items or not)
-        if (cv == 0 && u == 0) TC_STAMP(n, 5);
-        const float* xs = s_x + u * m.slot_floats + s_shift[u] + lane_off;  // this frame's tap 0
-        // frame F = 8 u + fl: hi row in group 2 u, row fl; the lo row 128 bytes on
-        unsigned char* arow = abuf + u * 256 + fl * 16;
-        for (; it < ipu; it += kTcConvWarps) {
-          const int c = 4 * it + cq;  // lanes 8 q .. 8 q + 7 read 8 q words on from lanes 0-7: conflict free for odd orig'
-          if (c < n_chunks) {
-            float v[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) v[t] = xs[8 * c + t];
-            uint4 hi, lo;
-            rs_split_bf16x2(v[0], v[1], hi.x, lo.x);
-            rs_split_bf16x2(v[2], v[3], hi.y, lo.y);
-            rs_split_bf16x2(v[4], v[5], hi.z, lo.z);
-            rs_split_bf16x2(v[6], v[7], hi.w, lo.w);
-            unsigned char* d = arow + c * kTcAStride;
-            *reinterpret_cast<uint4*>(d) = hi;
-            *reinterpret_cast<uint4*>(d + 128) = lo;
-          }
-        }
-        it -= ipu;  // position within the next unit
-        __syncwarp();  // the unit's samples are in registers (or converted): the slot may be re-filled
-        if (lane == 0) mbar_arrive(s_cdone + u);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // my operand rows -> the tensor core
-      __syncwarp();
-      if (cv == 0) TC_STAMP(n, 6);
-      if (lane == 0) mbar_arrive(s_aready + b);
-    }
-  }
-}
-
 }  // namespace
 
 size_t resample_workspace_bytes_impl(int new_r, int taps) { return rs_layout(new_r, taps).total; }
-
-// Host-only: what resample_run_impl will launch for this ratio (nothing touches the device).
-//   info[0] kernel family: 1 tcgen05 (resample_tc_kernel), 2 mma.sync TF32 x 3, 3 direct
-//   info[1] bytes of the banded bf16 tap blocks of the tcgen05 plan (0 if it does not apply)
-//   info[2] dynamic shared memory of the tcgen05 kernel, info[3] its MMAs per 32-frame tile
-int resample_plan_info_impl(int orig_r, int new_r, int width, int32_t* info) {
-  if (orig_r < 1 || new_r < 1 || width < 0 || info == nullptr) return B200A_EINVAL;
-  const int taps = 2 * width + orig_r;
-  const RsTcSteps steps = rs_tc_steps(orig_r, new_r, width);
-  const RsTcSmem tcm = rs_tc_smem(orig_r, taps);
-  const bool tc = (orig_r & 1) != 0 && steps.ok != 0;
-  const int n_tiles = rs_tiles(new_r);
-  const int xs_floats = (kRsFrames * orig_r + taps + 16 + 4 + 3) & ~3;
-  const size_t smem_fixed = sizeof(float) * 2 * (size_t)xs_floats + 16 + sizeof(RsTile) * ((n_tiles + 3) & ~3);
-  const bool mma = n_tiles <= kRsMaxTiles && smem_fixed + 1024 <= (size_t)kRsSmemBudget;
-  info[0] = tc ? 1 : (mma ? 2 : 3);
-  info[1] = steps.ok ? steps.b_bytes : 0;
-  info[2] = steps.ok ? tcm.total : 0;
-  info[3] = steps.ok ? 2 * steps.steps + 1 : 0;
-  return B200A_OK;
-}
-
-// Host-only: the live-tap band [first, last] the tcgen05 plan assumes for output phase `phase` (see rs_tc_band).
-int resample_tc_band_impl(int orig_r, int new_r, int width, int phase, int32_t* first, int32_t* last) {
-  if (orig_r < 1 || new_r < 1 || width < 0 || phase < 0 || phase >= new_r || first == nullptr || last == nullptr)
-    return B200A_EINVAL;
-  int f, l;
-  rs_tc_band(phase, orig_r, new_r, width, f, l);
-  const int taps = 2 * width + orig_r;
-  *first = f;
-  *last = l < taps - 1 ? l : taps - 1;
-  return B200A_OK;
-}
 
 int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width, void* ws, size_t ws_bytes,
                           cudaStream_t stream) {
@@ -1525,8 +944,6 @@ int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width,
   resample_r3_plan_kernel<<<1, 256, 0, stream>>>(kernel, support, new_r, taps, (new_r + 3) / 4, hdr,
                                                  reinterpret_cast<int*>(base + l.r3base),
                                                  reinterpret_cast<float4*>(base + l.r3taps));
-  resample_tc_plan_kernel<<<1, 256, 0, stream>>>(kernel, support, orig_r, new_r, width, taps,
-                                                 rs_tc_steps(orig_r, new_r, width), hdr, base + l.tcblocks);
   resample_simt_plan_kernel<<<1, 256, 0, stream>>>(kernel, support, new_r, taps, rs_tiles(new_r), hdr,
                                                    reinterpret_cast<RsSimtGroup*>(base + l.sgroups),
                                                    reinterpret_cast<float*>(base + l.staps));
@@ -1543,11 +960,11 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
   const RsLayout l = rs_layout(new_r, taps);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
 
-  // B200A_RS=tc|simt|mma|bf16|direct|r3 forces one kernel family (A/B measurements, tests); default: the first that applies
+  // B200A_RS=simt|mma|bf16|direct|r3 forces one kernel family (A/B measurements, tests); default: the first that applies
   static const int forced = [] {
     const char* e = std::getenv("B200A_RS");
     if (e == nullptr) return 0;
-    return e[0] == 's' ? 1 : (e[0] == 'm' ? 2 : (e[0] == 'd' ? 3 : (e[0] == 'b' ? 4 : (e[0] == 'r' ? 5 : (e[0] == 't' ? 6 : 0)))));
+    return e[0] == 's' ? 1 : (e[0] == 'm' ? 2 : (e[0] == 'd' ? 3 : (e[0] == 'b' ? 4 : (e[0] == 'r' ? 5 : 0))));
   }();
   int dev = 0, sms = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
@@ -1560,7 +977,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
     const int csize = (n_quads + kR3Warps - 1) / kR3Warps;  // CTAs that share a tile: 5 at 441:160
     const int slot_floats = (32 * orig_r + 2 * width + 16 + 3 + 3 + kR3Len) & ~3;
     const size_t smem = sizeof(float) * 3 * (size_t)slot_floats + 64;
-    const bool want = forced == 5;  // measured 1.80 ms at config 3 (cluster-scope barrier latency per 32-frame tile): opt-in only
+    const bool want = forced == 5;  // experiment kept for A/B timing (cluster-scope barrier per 32-frame tile): opt-in only
     if (want && csize <= kR3MaxCluster && smem <= (size_t)227 * 1024 && (reinterpret_cast<uintptr_t>(wave) & 3) == 0 &&
         length + (int64_t)taps + 64 * (int64_t)orig_r < ((int64_t)1 << 31)) {
       R3Params p{};
@@ -1620,76 +1037,13 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
     if (forced == 5 && !r3_launched) return B200A_EUNSUPPORTED;
   }
 
-  // ---- tcgen05 path: banded bf16 x 3 product, operand built in shared memory per 32-frame tile --------------------
-  bool tc_launched = false;
-  {
-    const RsTcSmem tcm = rs_tc_smem(orig_r, taps);
-    const size_t smem = (size_t)tcm.total;
-    // default for odd orig' (conflict-free frame-per-lane reads) whenever the plan fits: 0.283 vs 0.391 ms at config 3.
-    // Chosen by the RATIO alone, never by the batch, so that a row's result does not depend on what it is batched with.
-    // bf16 x 3 arithmetic: ~6e-6 of the output peak against ~1e-6 for the TF32 x 3 kernel below.
-    const bool want = forced == 6 || (forced == 0 && (orig_r & 1) != 0);
-    const RsTcSteps steps = rs_tc_steps(orig_r, new_r, width);
-    if (want && steps.ok &&
-        (reinterpret_cast<uintptr_t>(wave) & 3) == 0 && length + (int64_t)taps + 64 * (int64_t)orig_r < ((int64_t)1 << 31)) {
-      RsTcParams p{};
-      p.wave = wave;
-      p.rows = rows;
-      p.length = length;
-      p.row_stride = row_stride;
-      p.out = out;
-      p.out_row_stride = out_row_stride;
-      p.out_len = out_len;
-      p.hdr = reinterpret_cast<const RsHeader*>(base + l.header);
-      p.blocks = base + l.tcblocks;
-      p.orig_r = orig_r;
-      p.new_r = new_r;
-      p.width = width;
-      p.taps = taps;
-      p.frames = (out_len + new_r - 1) / new_r;
-      p.tiles_per_row = (p.frames + kTcFrames - 1) / kTcFrames;
-      p.total_tiles = rows * p.tiles_per_row;
-      p.out_vec = (new_r % 4 == 0 && out_row_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) ? 1 : 0;
-      if (cudaFuncSetAttribute(resample_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-        return B200A_ECUDA;
-      int64_t grid = p.total_tiles < sms ? p.total_tiles : sms;
-      if (grid < 1) grid = 1;
-#ifdef B200A_TC_TRACE
-      static long long* trace_dev = nullptr;
-      if (trace_dev == nullptr) cudaMalloc(&trace_dev, sizeof(long long) * 256);
-      cudaMemsetAsync(trace_dev, 0, sizeof(long long) * 256, stream);
-      p.trace = trace_dev;
-#endif
-      resample_tc_kernel<<<(unsigned)grid, kTcThreads, smem, stream>>>(p, rs_tc_issue_tab(steps, tcm.n_chunks), 1);
-#ifdef B200A_TC_TRACE
-      {
-        long long h[256];
-        cudaStreamSynchronize(stream);
-        cudaMemcpy(h, trace_dev, sizeof(h), cudaMemcpyDeviceToHost);
-        static int shown = 0;
-        if (shown++ == 3) {
-          const long long t0 = h[3];
-          std::fprintf(stderr, "[tc trace] tile: epi(wait got done) conv(start full loFree hiFree done) - prod(cd0) issue(alo accfree issued)\n");
-          for (int n = 0; n < 16; ++n) {
-            std::fprintf(stderr, "[tc trace] %2d:", n);
-            for (int e = 0; e < 13; ++e) std::fprintf(stderr, " %7lld", h[n * 16 + e] ? h[n * 16 + e] - t0 : -1);
-            std::fprintf(stderr, "\n");
-          }
-        }
-      }
-#endif
-      if (cudaPeekAtLastError() != cudaSuccess) return launch_status();
-      tc_launched = true;  // the mma.sync kernel below runs only if the device-side plan did not fit
-    }
-  }
-
   // ---- packed-FP32 SIMT path: odd orig' (conflict-free frame-per-lane reads) and the 3-slot ring fits -------------
   {
     const int n_groups = rs_tiles(new_r);
     const int slot_floats = (32 * orig_r + 2 * width + 3 + 8 + 3) & ~3;  // span + alignment shift + zero-tap over-read
     const size_t ring_bytes = sizeof(float) * 3 * (size_t)slot_floats;
     const size_t fixed = ring_bytes + sizeof(RsSimtGroup) * (size_t)n_groups + 64;
-    const bool want = forced == 1;  // measured slower than the tensor-pipe kernel (0.446 vs 0.391 ms at config 3): opt-in only
+    const bool want = forced == 1;  // variant kept for A/B timing against the tensor-pipe kernel: opt-in only
     if (want && fixed + 8192 <= (size_t)227 * 1024 && (reinterpret_cast<uintptr_t>(wave) & 3) == 0 &&
         length + (int64_t)taps + 64 * (int64_t)orig_r < ((int64_t)1 << 31)) {
       RsSimtParams p{};
@@ -1761,8 +1115,8 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
     // device-side step count with the room granted here), otherwise they are read through L1
     p.frag_smem_bytes = (int)(((size_t)kRsSmemBudget - smem_fixed) & ~(size_t)511);  // everything that is left
     const size_t smem = smem_fixed + p.frag_smem_bytes;
-    // default: TF32 x 3 (2^-21 relative).  B200A_RS=bf16 selects the bf16 x 3 variant: measured 5 % faster at config 3
-    // (0.371 vs 0.391 ms) for 30x the rounding error, so it stays opt-in
+    // default: TF32 x 3 (2^-21 relative).  B200A_RS=bf16 selects the bf16 x 3 variant (2^-16 relative, ~30x the rounding
+    // error), opt-in for A/B timing
     auto kern = forced == 4 ? resample_mma_kernel<true> : resample_mma_kernel<false>;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return B200A_ECUDA;
@@ -1782,7 +1136,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
       if (worst < best_conf) { best_conf = worst; best_spread = spread; }
     }
     p.row_spread = best_spread;
-    p.skip_if_r3_ok = r3_launched ? 1 : (tc_launched ? 2 : 0);
+    p.skip_if_r3_ok = r3_launched ? 1 : 0;
     // warps: n_tiles items (phase groups) per tile; prefer the largest count that divides them evenly
     const int items = n_tiles;
     int warps = 8;

@@ -1,7 +1,7 @@
 """Drop-in ``torchaudio.functional`` surface of the hot path, backed by libb200audio.so.
 
 Same names, argument order, defaults and error behaviour as the reference
-(/root/reference/src/torchaudio/functional/functional.py):
+(pytorch/audio/src/torchaudio/functional/functional.py):
 ``spectrogram`` (54-145), ``melscale_fbanks`` (518-587), ``linear_fbanks`` (590-633),
 ``create_dct`` (636-667), ``amplitude_to_DB`` (356-404), ``resample`` (1435-1490) and the two
 private helpers ``transforms`` imports (``_get_sinc_resample_kernel`` 1305-1402,
@@ -159,7 +159,7 @@ def inverse_spectrogram(
         raise ValueError("Expected `spectrogram` to be complex dtype.")
     if not spectrogram.is_cuda:
         raise RuntimeError(
-            f"audio_b200: spectrogram is on '{spectrogram.device}'. This package runs only hand-written sm_100a CUDA "
+            f"audio_b200: spectrogram is on '{spectrogram.device}'. This package runs only hand-written sm_90a CUDA "
             "kernels; there is no CPU or ATen fallback -- move the tensor (and the module) to a CUDA device."
         )
     if spectrogram.dtype != torch.complex64:
@@ -287,7 +287,7 @@ def phase_vocoder(complex_specgrams: Tensor, rate: float, phase_advance: Tensor)
     if not complex_specgrams.is_cuda:
         raise RuntimeError(
             f"audio_b200: complex_specgrams is on '{complex_specgrams.device}'. This package runs only hand-written "
-            "sm_100a CUDA kernels; there is no CPU or ATen fallback -- move the tensor (and the module) to a CUDA device."
+            "sm_90a CUDA kernels; there is no CPU or ATen fallback -- move the tensor (and the module) to a CUDA device."
         )
     if complex_specgrams.dtype != torch.complex64:
         raise TypeError(f"audio_b200: complex_specgrams must be complex64 (got {complex_specgrams.dtype})")

@@ -1,7 +1,7 @@
 """Host-buffer pipeline: run a front-end module over waveforms that live in (pinned) HOST memory.
 
-A B200 turns 256 x 10 s of audio into mel features in a fraction of a millisecond, but the same
-batch takes ~3 ms to cross PCIe.  ``HostPipeline`` splits the batch into row chunks and keeps three
+An H100 turns 256 x 10 s of audio into mel features in a fraction of a millisecond, but the same
+batch takes milliseconds to cross PCIe.  ``HostPipeline`` splits the batch into row chunks and keeps three
 CUDA streams busy -- host->device copies, the fused kernel, device->host copies -- so the end-to-end
 time approaches the slower of the two PCIe directions instead of their sum plus the compute.
 Consecutive calls overlap too: the H2D copies of call k+1 start while the D2H copies of call k drain.

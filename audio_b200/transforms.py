@@ -1,12 +1,12 @@
 """Drop-in ``torchaudio.transforms`` modules of the hot path, backed by libb200audio.so.
 
 Class names, constructor signatures, attribute / buffer / sub-module names and error
-behaviour follow /root/reference/src/torchaudio/transforms/_transforms.py
+behaviour follow pytorch/audio/src/torchaudio/transforms/_transforms.py
 (Spectrogram 25-123, AmplitudeToDB 300-346, MelScale 349-415, MelSpectrogram 506-622,
 MFCC 625-709, Resample 899-980), so ``state_dict``s interchange with torchaudio's and
 existing call sites keep working after ``import audio_b200.transforms as T``.
 
-``forward`` launches hand-written sm_100a kernels through the C ABI; MelSpectrogram and MFCC
+``forward`` launches hand-written sm_90a kernels through the C ABI; MelSpectrogram and MFCC
 do NOT chain their sub-modules' forwards (that would round-trip the (B, T, n_fft/2+1) power
 spectrum through HBM) -- they read the sub-modules' buffers and launch the fused kernel.
 """
@@ -649,7 +649,7 @@ def _install_reference_switch() -> None:
         raise ImportError("B200A_REFERENCE=1 needs an importable torchaudio to route the transforms to") from exc
     warnings.warn(
         "B200A_REFERENCE=1: audio_b200.transforms modules run torchaudio's reference implementation "
-        f"(torchaudio {getattr(__import__('torchaudio'), '__version__', '?')}); the B200 kernels are bypassed",
+        f"(torchaudio {getattr(__import__('torchaudio'), '__version__', '?')}); the CUDA kernels are bypassed",
         stacklevel=2,
     )
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- MelSpectrogram frames/s on BASELINE.json config 2, at 1..8 B200, plus every other BASELINE config.
+"""bench.py -- MelSpectrogram frames/s on BASELINE.json config 2, at 1..8 H100, plus every other BASELINE config.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the fused front end over one batch of synthetic waveforms:
@@ -18,12 +18,17 @@ collective is on this path).  Prints ONE JSON line on rank 0.
             256 x 160000 per GPU (batch-global top_db: at N > 1 the NCCL all-reduce(MAX) of the running maximum
             is INSIDE the timed region), C5 fused STFT+mel sweep n_fft in {256, 512, 1024, 2048} (hop = n_fft/4)
   cpu_baseline  the reference's CPU path (installed torchaudio wheel, hot-path source identical to
-            /root/reference) or, if that cannot be imported, the numpy oracle port -- rank 0, N = 1 only
+            pytorch/audio at the pinned version) or, if that cannot be imported, the numpy oracle port -- rank 0, N = 1 only
   --impl reference   the same reference CPU path as its own arm: the FULL 256 x 160000 batch per step
+  --dump-outputs DIR after the timed steps, rank 0 writes what each timed path returned in its last timed step, as
+            float32: DIR/mel_spectrogram.npy (256, 80, 626) in full, and rows DUMP_ROWS[name] (a fixed, seeded sample)
+            of C3 resample.npy, C4 mfcc.npy and C5 mel_nfft{256,512,2048}.npy, 59 MB in all; the inputs are seeded, so
+            two builds can be compared output for output
 """
 import argparse
 import json
 import os
+import random
 import subprocess
 import sys
 import threading
@@ -40,20 +45,20 @@ FRAMES = 1 + LENGTH // HOP  # 626
 RS_ROWS, RS_LEN, RS_ORIG, RS_NEW = 1024, 220500, 44100, 16000
 RS_OUT = 80000
 E2E_WINDOWS = 5
+# --dump-outputs: rows of each larger output that are written (seeded, sorted, the same in every run)
+DUMP_ROWS = {name: sorted(random.Random(7).sample(range(rows), n)) for name, rows, n in
+             (("resample", RS_ROWS, 8), ("mfcc", BATCH, 16), ("mel_nfft256", BATCH, 2), ("mel_nfft512", BATCH, 4),
+              ("mel_nfft2048", BATCH, 8))}
 WORKLOAD = "MelSpectrogram n_fft=1024 hop=256 n_mels=80, batch=256x16kHzx10s fp32 per GPU (BASELINE configs[1])"
 # SURVEY.md 8(d): compulsory traffic of the fused op = waveform in + features out + constant tables
 ALGO_BYTES = 4 * (BATCH * LENGTH + BATCH * FRAMES * N_MELS) + 4 * (N_FFT + (N_FFT // 2 + 1) * N_MELS)
-# dram__bytes_read.sum + dram__bytes_write.sum of one launch of the fused kernel (ncu --set full capture):
-# the write-back of part of the 51 MB output is still in L2 at kernel end
-NCU_DRAM_BYTES = 196_650_752
-NCU_DRAM_SOURCE = "ncu --set full, profiles/r2_mel_v3_tc2_prefetch.txt (dram read 163.99 MB + write 32.66 MB per launch)"
 
 
 def workload_config(world):
     """`config` of the JSON line -- identical for the b200 and the reference arm."""
     return {"workload": WORKLOAD, "global_batch": world * BATCH, "frames_per_step": world * BATCH * FRAMES,
             "parallelism": f"batch shard x{world}, no collective",
-            "l2": "input 163.8 MB per step > 126 MB L2 (no flush needed)"}
+            "l2": "input 163.8 MB per step > 50 MB L2 of an H100 (no flush needed)"}
 
 
 def measured_peaks():
@@ -62,7 +67,7 @@ def measured_peaks():
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -72,10 +77,7 @@ class ClockSampler:
     Read through NVML inside this process (pynvml = nvidia_ml_py, the library nvidia-smi itself sits on); the nvidia-smi
     BINARY (a driver attach per sample) is only the fallback when NVML cannot be imported.  ONE sampler per job
     (rank 0) covers every GPU of the job, and it is PAUSED inside the launch-bound end-to-end section (sampled right
-    before and right after it): the e2e number of the same code moved between 3.04 ms (twice), 3.9, 12.4 and 32.8 ms
-    per step from box to box at N = 1 and was 6.75 ms at N = 8 with a sampler in every rank, against 4.35 ms in
-    tools/h2d_probe.py, which has no sampler.  The cause was not isolated inside the round's GPU budget; keeping
-    driver queries out of that 60 ms window removes the one suspect this file controls."""
+    before and right after it), so that no driver query competes with the host work that section measures."""
 
     FIELDS = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -173,11 +175,30 @@ class ClockSampler:
                 "window": "headline timed region and configs sections; the e2e section is bracketed (sampler paused inside)"}
 
 
+def device_info(index):
+    """Name, SM count and enforced power limit of the GPU the numbers were measured on (the limit through NVML when
+    it can be imported)."""
+    import torch
+
+    p = torch.cuda.get_device_properties(index)
+    info = {"name": p.name, "sms": p.multi_processor_count, "power_limit_w": None}
+    try:
+        import pynvml
+
+        pynvml.nvmlInit()
+        bdf = f"{p.pci_domain_id:08x}:{p.pci_bus_id:02x}:{p.pci_device_id:02x}.0"
+        h = pynvml.nvmlDeviceGetHandleByPciBusId(bdf.encode())
+        info["power_limit_w"] = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
+    except Exception:  # noqa: BLE001
+        pass
+    return info
+
+
 # ---- the reference on the host ---------------------------------------------------------------------------------
 def _reference_module(kind, **kw):
     """(callable(x) running the reference's CPU path, kind, description)."""
     try:
-        import torchaudio  # the image's wheel: functional.py byte-identical to /root/reference's
+        import torchaudio  # the installed wheel: functional.py byte-identical to the pinned reference's
 
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
@@ -264,7 +285,7 @@ def run_reference(args):
     print(json.dumps(line))
 
 
-# ---- the B200 arm ------------------------------------------------------------------------------------------------
+# ---- the GPU arm -------------------------------------------------------------------------------------------------
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -293,16 +314,18 @@ def run_b200(args):
         torch.cuda.synchronize()
 
     K, W = args.steps, max(args.warmup, 3)
+    last = [None]
 
     def time_steps(fn, steps=K, warm=W):
-        """ms per step: `warm` untimed steps, then `steps` steps between two CUDA events, barrier + sync on both sides."""
+        """ms per step: `warm` untimed steps, then `steps` steps between two CUDA events, barrier + sync on both sides.
+        The result of the last call is kept in `last[0]`."""
         for _ in range(warm):
-            fn()
+            last[0] = fn()
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            last[0] = fn()
         e1.record()
         barrier()
         return e0.elapsed_time(e1) / steps
@@ -323,7 +346,15 @@ def run_b200(args):
     with torch.inference_mode(), ClockSampler([local] if world == 1 else range(world), active=(rank == 0)) as clocks:
         # ---- headline: config 2, inputs resident -------------------------------------------------------------
         ms_step = time_steps(lambda: mel(x))
-        y = mel(x)
+        y = last[0]  # what the last timed step returned
+        dumps = {} if args.dump_outputs and rank == 0 else None
+
+        def keep(name, out):  # outside the timed region: the last timed step's output, or its sampled rows
+            if dumps is not None:
+                rows = DUMP_ROWS.get(name)
+                dumps[name] = (out if rows is None else out[rows]).float().cpu()
+
+        keep("mel_spectrogram", y)
 
         # ---- end to end: pinned host -> device, fused kernel, device -> pinned host ----------------------------
         from audio_b200.pipeline import HostPipeline
@@ -366,6 +397,7 @@ def run_b200(args):
         if world > 1:
             mf.process_group = dist.group.WORLD
         ms_c4 = time_steps(lambda: mf(x))
+        keep("mfcc", last[0])
         mf_local = T.MFCC(SAMPLE_RATE, n_mfcc=N_MFCC, melkwargs=dict(n_fft=N_FFT, hop_length=HOP, n_mels=N_MELS)).to(dev)
         ms_c4_local = time_steps(lambda: mf_local(x)) if world > 1 else ms_c4
         c4_bytes = 4 * (BATCH * LENGTH + BATCH * FRAMES * N_MFCC) + 4 * (N_FFT + 513 * N_MELS + N_MELS * N_MFCC)
@@ -380,6 +412,8 @@ def run_b200(args):
                 warnings.simplefilter("ignore")  # n_fft = 256 leaves two of the 80 mel filters empty (reference warns too)
                 m5 = T.MelSpectrogram(SAMPLE_RATE, n_fft=n_fft, hop_length=hop, n_mels=N_MELS).to(dev)
             ms5 = ms_step if n_fft == N_FFT else time_steps(lambda: m5(x))
+            if n_fft != N_FFT:
+                keep(f"mel_nfft{n_fft}", last[0])
             sweep.append((n_fft, hop, fr, ms5, 4 * (BATCH * LENGTH + BATCH * fr * N_MELS) + 4 * (n_fft + (n_fft // 2 + 1) * N_MELS)))
             del m5
         del x, y
@@ -389,6 +423,8 @@ def run_b200(args):
         rs = T.Resample(RS_ORIG, RS_NEW, resampling_method="sinc_interp_kaiser").to(dev)
         xr = torch.randn(RS_ROWS, RS_LEN, device=dev, generator=g)
         ms_c3 = time_steps(lambda: rs(xr))
+        keep("resample", last[0])
+        last[0] = None
         c3_bytes = 4 * (RS_ROWS * RS_LEN + RS_ROWS * RS_OUT) + 4 * 160 * 475
         del xr, rs
         torch.cuda.empty_cache()
@@ -423,8 +459,8 @@ def run_b200(args):
             "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": ms_step, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": workload_config(world),
-            "roofline": dict(roof(ALGO_BYTES, ms_step), traffic=NCU_DRAM_BYTES, traffic_source=NCU_DRAM_SOURCE,
-                             peak_source=peak_src, kernel="fused STFT+mel kernel (one launch per step)"),
+            "roofline": dict(roof(ALGO_BYTES, ms_step), peak_source=peak_src,
+                             kernel="fused STFT+mel kernel (one launch per step)"),
             "e2e": {"value": frames_job / (ms_e2e * 1e-3), "unit": "frames/s",
                     "h2d_bytes_per_step": BATCH * LENGTH * 4, "d2h_bytes_per_step": BATCH * FRAMES * N_MELS * 4,
                     "ms_per_step": ms_e2e, "windows_ms_per_step": [round(w, 4) for w in e2e_windows],
@@ -432,6 +468,7 @@ def run_b200(args):
                     "api": "audio_b200.pipeline.HostPipeline(chunk_rows=64)",
                     "numa": numa},
             "gpu_launches": K,
+            "device": device_info(local),
             "clocks": clock_summary,
             "configs": configs,
         }
@@ -451,6 +488,12 @@ def run_b200(args):
             for c in configs:
                 if c["key"] in cpu:
                     c["cpu_baseline"] = cpu[c["key"]]
+        if dumps is not None:
+            import numpy as np
+
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, t in dumps.items():
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.numpy().astype(np.float32))
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
@@ -462,7 +505,11 @@ def main():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write each timed path's output of its last timed step (larger ones: a seeded row sample) to DIR")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

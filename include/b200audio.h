@@ -1,5 +1,5 @@
 /*
- * b200audio.h -- C ABI of libb200audio.so, the sm_100a implementation of torchaudio's DSP
+ * b200audio.h -- C ABI of libb200audio.so, the sm_90a implementation of torchaudio's DSP
  * front-end hot path (STFT -> |.|^p -> mel -> dB/log -> DCT, and the polyphase sinc resampler).
  *
  * This is the drop-in boundary.  pytorch/audio has no native op for this path (it is Python
@@ -24,7 +24,7 @@
  * the tensors the reference returns (logical (..., bin, t) with strides (.., 1, n_bins):
  * functional.py:123-137 and transforms/_transforms.py:413 produce transposed views).
  *
- * Citations below are relative to /root/reference/src/torchaudio/.
+ * Citations below are relative to src/torchaudio/ of the pytorch/audio tree.
  */
 #ifndef B200AUDIO_H
 #define B200AUDIO_H
@@ -104,16 +104,6 @@ int64_t b200a_resample_len(int64_t length, int32_t orig_r, int32_t new_r);
  * is (numerically) zero.  ~2*lpw*orig'/min(orig',new') taps.  Returns 0 or B200A_EINVAL. */
 int b200a_resample_support(int32_t orig_r, int32_t new_r, int32_t lowpass_filter_width, double rolloff, int32_t phase,
                            int32_t* first, int32_t* count);
-/* Which kernel b200a_resample_run launches for a ratio, decided on the host from (orig', new', width) alone (never from
- * the batch: a row's result does not depend on what it is batched with).  info[0] = 1 tcgen05 banded product (odd
- * orig', taps and bands fit shared memory), 2 mma.sync TF32x3, 3 direct; info[1] = bytes of the tcgen05 plan's banded
- * bf16 tap blocks, info[2] = its dynamic shared memory, info[3] = tcgen05.mma instructions per 32-frame tile.
- * No reference counterpart (conv1d picks its own algorithm, functional.py:1421).  Returns 0 or B200A_EINVAL. */
-int b200a_resample_plan_info(int32_t orig_r, int32_t new_r, int32_t width, int32_t* info);
-/* The live-tap band [first, last] the tcgen05 plan assumes for output phase `phase`: (phase*orig'/new',
- * phase*orig'/new' + 2*width), a superset of b200a_resample_support for kernels built like functional.py:1359-1400
- * (checked on the device against the caller's kernel by b200a_resample_prepare).  Returns 0 or B200A_EINVAL. */
-int b200a_resample_tc_band(int32_t orig_r, int32_t new_r, int32_t width, int32_t phase, int32_t* first, int32_t* last);
 
 /* ---- fused front end -------------------------------------------------------------------- */
 /* Bytes of caller-owned device workspace that b200a_frontend_prepare fills for this descriptor. */

@@ -10,13 +10,13 @@ Parity status: PINNED.  ``tests/test_oracle_golden.py`` checks every function
 here against (a) the librosa golden vectors the reference's own test-suite
 holds (``test/torchaudio_unittest/assets/librosa_expected_results``, converted
 by ``tests/golden/make_golden.py``) and (b) outputs of the reference itself
-(``/root/reference/src`` imported in the build container by the same script).
+(``pytorch/audio/src`` imported by the same script).
 
 The arithmetic of the reference lives in PyTorch/ATen (third-party, not under
-/root/reference; torch 2.11.0 here): ``torch.stft`` -> ``at::stft`` ->
+pytorch/audio; torch 2.11.0 here): ``torch.stft`` -> ``at::stft`` ->
 ``_fft_r2c`` (MKL DFTI), ``matmul``, ``conv1d``.  Their *published* definitions
 are restated below; every function cites the reference call site it follows
-(paths relative to /root/reference).
+(paths relative to pytorch/audio).
 """
 from __future__ import annotations
 

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY: imported by tests/, never by the product (audio_b200/ has no CPU path).
 
-Follows /root/reference/src/torchaudio/compliance/kaldi.py; every function cites the lines it restates.
+Follows pytorch/audio/src/torchaudio/compliance/kaldi.py; every function cites the lines it restates.
 Parity PINNED: tests/test_kaldi.py checks this file against the 311 Kaldi-binary outputs the reference's own
 tests hold (test/torchaudio_unittest/assets/kaldi_expected_results, consumed by
 compliance/kaldi/kaldi_compatibility_impl.py:20-48 with rtol 1e-4) and against outputs of the reference

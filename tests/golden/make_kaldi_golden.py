@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Generate the committed Kaldi fixtures under tests/golden/ (needs /root/reference; run once in the build container):
+"""Generate the committed Kaldi fixtures under tests/golden/ (needs a pytorch/audio checkout named by AUDIO_REFERENCE; run once):
 
     python tests/golden/make_kaldi_golden.py
 
@@ -8,7 +8,7 @@
    rtol 1e-4 (compliance/kaldi/kaldi_compatibility_impl.py:20-48), the option sets they were produced with
    (assets/kaldi_test_{fbank,mfcc,spectrogram}_args.jsonl, kept as JSON strings) and the 20-sample input
    (assets/kaldi_file.wav, read un-normalised as load_wav(normalize=False) does).
-2. ``kaldi_ref_cases.npz`` -- outputs of the reference itself (/root/reference/src, CPU, float32) on seeded
+2. ``kaldi_ref_cases.npz`` -- outputs of the reference itself (the reference's src/, CPU, float32) on seeded
    signals of realistic length, for option sets the tiny Kaldi cases do not reach (25 ms frames at 16 kHz =
    512-point FFT, 80 mel bins, snip_edges on/off, energy, HTK order, mean subtraction), plus the reference's
    constant tables (windows, mel banks, DCT, lifter) for the bit-identity checks of the host code.
@@ -23,7 +23,7 @@ import wave
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = os.environ["AUDIO_REFERENCE"]  # a pytorch/audio checkout at the pinned version
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(REF, "src"))
 import torchaudio  # noqa: E402

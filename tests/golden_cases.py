@@ -3,7 +3,7 @@
 They restate the parameterisations of the reference's own tests:
 transforms/librosa_compatibility_test_impl.py:17-134 and
 functional/librosa_compatibility_test_impl.py:56-94 (paths under
-/root/reference/test/torchaudio_unittest).
+pytorch/audio/test/torchaudio_unittest).
 """
 import itertools
 
@@ -82,8 +82,12 @@ RESAMPLE = {
     "rs_hann_out": (None, dict(orig_freq=44100, new_freq=16000)),
     "rs_16k_8k": (None, dict(orig_freq=16000, new_freq=8000)),
     "rs_8k_16k": (None, dict(orig_freq=8000, new_freq=16000)),
-    "rs_48k_44k1": (9600, dict(orig_freq=48000, new_freq=44100)),
-    "rs_16k_44k1": (4000, dict(orig_freq=16000, new_freq=44100, resampling_method="sinc_interp_kaiser")),
+    "rs_48k_44k1": (2400, dict(orig_freq=48000, new_freq=44100)),
+    "rs_16k_44k1": (1000, dict(orig_freq=16000, new_freq=44100, resampling_method="sinc_interp_kaiser")),
     "rs_lpw16": (None, dict(orig_freq=16000, new_freq=12000, lowpass_filter_width=16, rolloff=0.9)),
     "rs_short": (7, dict(orig_freq=44100, new_freq=16000)),
 }
+
+# librosa_transforms.npz keeps every second frame of each expected output (tests/golden/make_golden.py); the tests
+# compare the same frames of what they compute
+LIBROSA_FRAMES = slice(None, None, 2)

@@ -145,43 +145,13 @@ def test_resample_large_prime_ratio_uses_fallback():
     assert fun.shape == exp.shape and np.abs(fun - exp).max() <= 5e-3 * np.abs(exp).max()
 
 
-_MMA_CHILD = r"""
-import sys, numpy as np, torch
-sys.path.insert(0, sys.argv[1])
-import audio_b200.transforms as T
-out = {}
-for n_fft, n_mels in ((256, 40), (512, 64), (1024, 80), (1024, 128)):
-    x = torch.randn(5, 9000, generator=torch.Generator().manual_seed(n_fft + n_mels)).cuda()
-    out[f"mel_{n_fft}_{n_mels}"] = T.MelSpectrogram(16000, n_fft=n_fft, hop_length=n_fft // 4, n_mels=n_mels).cuda()(x).cpu().numpy()
-x = torch.randn(2, 3, 7000, generator=torch.Generator().manual_seed(5)).cuda()
-out["mfcc"] = T.MFCC(16000, n_mfcc=20, melkwargs=dict(n_fft=512, hop_length=160, n_mels=64)).cuda()(x).cpu().numpy()
-np.savez(sys.argv[2], **out)
-"""
-
-
-def test_tcgen05_and_mma_sync_contractions_agree(tmp_path):
-    """The mel stage has two bodies: tcgen05 (bf16 hi/lo operands, default for real filterbanks) and mma.sync
-    (TF32 hi/lo; dense filterbanks, or B200A_TC=0).  Same inputs through both, each against the fp64 oracle and
-    against each other (the switch is read once per process, hence the child)."""
-    import os
-    import subprocess
-    import sys
-
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    res = {}
-    for tag, val in (("tc", "1"), ("mma", "0")):
-        path = str(tmp_path / f"{tag}.npz")
-        subprocess.run([sys.executable, "-c", _MMA_CHILD, root, path], env=dict(os.environ, B200A_TC=val), check=True,
-                       timeout=300)
-        res[tag] = np.load(path)
-    for key in res["tc"].files:
-        a, b = res["tc"][key], res["mma"][key]
-        assert a.shape == b.shape
-        assert np.abs(a - b).max() <= 3e-5 * np.abs(b).max(), key
+def test_mma_sync_contraction_against_oracle():
+    """The fused mel stage contracts each power tile with the filterbank on mma.sync (TF32 hi/lo operands): every
+    register-FFT size, narrow and wide filterbanks, against the fp64 oracle."""
     for n_fft, n_mels in ((256, 40), (512, 64), (1024, 80), (1024, 128)):
-        x = torch.randn(5, 9000, generator=torch.Generator().manual_seed(n_fft + n_mels)).numpy()
+        x = torch.randn(5, 9000, generator=torch.Generator().manual_seed(n_fft + n_mels))
+        got = T.MelSpectrogram(16000, n_fft=n_fft, hop_length=n_fft // 4, n_mels=n_mels).to(DEV)(x.to(DEV)).cpu().numpy()
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
-            exp = O.mel_spectrogram(x, sample_rate=16000, n_fft=n_fft, hop_length=n_fft // 4, n_mels=n_mels)
-        for tag in ("tc", "mma"):
-            scaled_tol_close(res[tag][f"mel_{n_fft}_{n_mels}"], exp, what=f"{tag} {n_fft}/{n_mels}")
+            exp = O.mel_spectrogram(x.numpy(), sample_rate=16000, n_fft=n_fft, hop_length=n_fft // 4, n_mels=n_mels)
+        scaled_tol_close(got, exp, what=f"mma {n_fft}/{n_mels}")

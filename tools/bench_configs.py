@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Per-config throughput table for BASELINE.json configs 2-5 on ONE GPU (inputs resident in HBM).
 
-Not the driver's bench contract (that is bench.py); this fills the table in DESIGN.md / profiles/.
-    python tools/bench_configs.py [--quick] [--out profiles/r1_configs.json]
+Not the benchmark's JSON line (that is bench.py); a per-config table for kernel work.
+    python tools/bench_configs.py [--quick] [--out configs.json]
 For every config: kernel time (CUDA events, median of blocks of back-to-back launches), throughput,
 algorithmic bytes (SURVEY.md 8d) / time vs the measured HBM peak, and the torchaudio CPU reference on a
 bounded sample of the same workload.
@@ -28,7 +28,7 @@ def hbm_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
             return float(json.load(fh)["hbm_gbs"])
     except Exception:
-        return 6650.0
+        return 3350.0  # H100 SXM data-sheet HBM3 bandwidth, not measured
 
 
 def time_gpu(fn, iters=20, blocks=5):

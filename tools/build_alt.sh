@@ -5,6 +5,6 @@ set -e
 name=$1; shift
 cd "$(dirname "$0")/.."
 B=audio_b200/build
-nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --expt-relaxed-constexpr "$@" -c audio_b200/csrc/frontend_pow2.cu -o $B/frontend_pow2_$name.o
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o $B/libb200audio_$name.so $B/api.o $B/frontend_generic.o $B/frontend_pow2_$name.o $B/resample.o $B/standalone.o
+nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --expt-relaxed-constexpr "$@" -c audio_b200/csrc/frontend_pow2.cu -o $B/frontend_pow2_$name.o
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o $B/libb200audio_$name.so $B/api.o $B/frontend_generic.o $B/frontend_pow2_$name.o $B/resample.o $B/standalone.o
 ls -la $B/libb200audio_$name.so

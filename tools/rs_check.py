@@ -1,5 +1,5 @@
 """Compare the resampler kernel families on the same seeded input (run once per B200A_RS value; outputs go to /tmp).
-    B200A_RS=mma python tools/rs_check.py save;  B200A_RS=tc python tools/rs_check.py cmp
+    B200A_RS=mma python tools/rs_check.py save;  B200A_RS=bf16 python tools/rs_check.py cmp
 """
 import sys
 import torch

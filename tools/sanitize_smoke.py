@@ -1,7 +1,7 @@
 """Small invocations of every kernel family for compute-sanitizer:
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py
 (racecheck reports the mbarrier-synchronised hand-offs of the warp-specialised kernels as hazards: it does not model
-mbarrier / tcgen05.commit ordering; memcheck and initcheck are the meaningful tools here)."""
+mbarrier ordering; memcheck and initcheck are the meaningful tools here)."""
 import os
 import sys
 
