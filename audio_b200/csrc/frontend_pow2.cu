@@ -52,7 +52,6 @@ struct Geo {
   static constexpr int kRowLd = G + 1;          // float2 pitch of one transpose row (bank-conflict free)
   static constexpr int kRegion = 32 * (G + 1) + (G == 8 ? 8 : 0);  // float2 per lane group (skewed for G = 8)
   static constexpr int kTileF2 = kGroups * kRegion;                // float2 per warp
-  static constexpr int kStageFloats = 2 * kTileF2;                 // a staged unit must fit the tile
   static constexpr int kSlots = kWarps * kFrames;                  // frames finished per CTA iteration
   static constexpr int kPitch = ((kBins + 7 - 4 + 31) / 32) * 32 + 4;  // floats per power row, == 4 (mod 32)
   static constexpr int kLogG = G == 32 ? 5 : (G == 16 ? 4 : 3);
@@ -302,15 +301,15 @@ __device__ __forceinline__ void issue_bulk(const Pow2Params& p, int half, int64_
 // One warp, one unit (32/G frame pairs): samples -> windowed complex signals -> n_fft-point FFTs -> the
 // power spectra.  On return lane (group gi, l) holds bins k = l + G m in pa[m] / pb[m] (m < 16) of frames
 // t0 + 2 gi and t0 + 2 gi + 1, and lanes with l == 0 bin n_fft/2 in [16].
-//   stage      where a prefetched unit was staged (aliases `tile` when STAGE_IS_TILE)
-//   STAGE_IS_TILE  the staging buffer is the transpose tile itself: the NEXT unit's bulk copy is issued
-//                  only after pass 2 has read the tile back
-template <int POWER_MODE, int G, int HG, bool STAGE_IS_TILE, bool KALDI>
+// The staging buffer is the warp's transpose tile itself: the NEXT unit's bulk copy is issued only after
+// pass 2 has read the tile back.
+template <int POWER_MODE, int G, int HG, bool KALDI>
 __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float (&wreg)[32], const float2* s_tw,
-                                               float2* tile, float* stage, uint64_t* bar, uint32_t& parity,
-                                               bool& staged, const UnitCursor& cur, int half, int lane,
-                                               float (&pa)[17], float (&pb)[17]) {
+                                               float2* tile, uint64_t* bar, uint32_t& parity, bool& staged,
+                                               const UnitCursor& cur, int half, int lane, float (&pa)[17],
+                                               float (&pb)[17]) {
   using Ge = Geo<G>;
+  float* stage = reinterpret_cast<float*>(tile);
   const int gi = lane / G, l = lane % G;
   const int64_t row = cur.row, t0 = cur.ub * Ge::kFrames;
   const int64_t ta = t0 + 2 * gi, tb = ta + 1;
@@ -469,17 +468,10 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
     });
     __syncwarp();
   }
-  if constexpr (!STAGE_IS_TILE) {  // separate staging buffer: prefetch right away
-    staged = next_staged;
-    if (staged && lane == 0) issue_bulk<G>(p, half, cur.nrow, cur.nub, stage, bar);
-  }
 
   // the inter-pass twiddles: kTwAhead loads are in flight before the last butterfly stage, and every multiply
   // issues the load kTwAhead positions ahead of it, so no multiply waits for its own load
-#ifndef B200A_TW_AHEAD
-#define B200A_TW_AHEAD 8
-#endif
-  constexpr int kTwAhead = B200A_TW_AHEAD;
+  constexpr int kTwAhead = 8;
   fft_regs<32, 0, 0, 4>(a);
   float2 tw[32];
   static_for<kTwAhead>([&](auto ki) {
@@ -501,12 +493,10 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
     a[q * G + brev<Ge::kLogG>(g)] = grp_tile[(l + G * q) * Ge::kRowLd + g];
   });
   __syncwarp();
-  if constexpr (STAGE_IS_TILE) {  // the tile is free until the next unit's transpose: stage into it
-    staged = next_staged;
-    if (staged && lane == 0) {
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads above -> async write
-      issue_bulk<G>(p, half, cur.nrow, cur.nub, stage, bar);
-    }
+  staged = next_staged;  // the tile is free until the next unit's transpose: stage into it
+  if (staged && lane == 0) {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads above -> async write
+    issue_bulk<G>(p, half, cur.nrow, cur.nub, stage, bar);
   }
 
   static_for<Ge::kGroups>([&](auto qi) { fft_regs<G, decltype(qi)::value * G>(a); });
@@ -570,14 +560,13 @@ __device__ __forceinline__ void load_window(const Pow2Params& p, int lane, float
 // ------------------------------------------------------------------------------------------------
 // Spectrogram kernel: 8 independent warps, power spectra straight to global memory.
 // ------------------------------------------------------------------------------------------------
-template <int POWER_MODE, int G, int HG, int NW, bool STAGE_IS_TILE, bool KALDI>
+template <int POWER_MODE, int G, int HG, int NW, bool KALDI>
 __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2Params p) {
   using Ge = Geo<G>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2* s_tw = reinterpret_cast<float2*>(smem_raw);                                    // [32][G]
-  float2* s_tile_all = s_tw + 32 * 32;                                                   // [NW][kTileF2]
-  float* s_stage_all = reinterpret_cast<float*>(s_tile_all + NW * Ge::kTileF2);      // [NW][kStageFloats]
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_stage_all + (STAGE_IS_TILE ? 0 : NW * Ge::kStageFloats));  // [NW]
+  float2* s_tile_all = s_tw + 32 * 32;                                                   // [NW][kTileF2] (also staging)
+  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_tile_all + NW * Ge::kTileF2);          // [NW]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
@@ -586,7 +575,7 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   __syncthreads();
 
   float2* tile = s_tile_all + warp * Ge::kTileF2;
-  float* stage = STAGE_IS_TILE ? reinterpret_cast<float*>(tile) : s_stage_all + warp * Ge::kStageFloats;
+  float* stage = reinterpret_cast<float*>(tile);
   uint64_t* bar = s_bar + warp;
   float wreg[32];
   load_window<G>(p, lane, wreg);
@@ -602,8 +591,7 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   }
   for (; cur.u < p.total_units; cur.advance()) {
     float pa[17], pb[17];
-    transform_unit<POWER_MODE, G, HG, STAGE_IS_TILE, KALDI>(p, wreg, s_tw, tile, stage, bar, parity, staged, cur, half, lane, pa,
-                                                            pb);
+    transform_unit<POWER_MODE, G, HG, KALDI>(p, wreg, s_tw, tile, bar, parity, staged, cur, half, lane, pa, pb);
     if constexpr (POWER_MODE == kComplexOut) continue;  // transform_unit has written the complex spectra
     const int64_t ta = cur.ub * Ge::kFrames + 2 * gi;
     const bool has_a = ta < p.frames, has_b = ta + 1 < p.frames;
@@ -777,8 +765,7 @@ __device__ __forceinline__ void mel_body_mma(const Pow2Params& p, unsigned char*
       const bool valid = cur.u < p.total_units;
       float pa[17], pb[17];
       if (valid)
-        transform_unit<POWER_MODE, G, HG, true, KALDI>(p, wreg, s_tw, tile, stage, bar, parity, staged, cur, half, lane, pa,
-                                                pb);
+        transform_unit<POWER_MODE, G, HG, KALDI>(p, wreg, s_tw, tile, bar, parity, staged, cur, half, lane, pa, pb);
       const int b = it & 1;
       if (it >= 2) mbar_wait(s_empty + b, ((it >> 1) & 1) ^ 1);  // the mel warps have drained this buffer
       const int slot_a = Ge::kFrames * warp + 2 * gi;
@@ -1317,14 +1304,13 @@ static int64_t persistent_grid(const Pow2Params& p, int warps = kWarps) {
 template <int POWER_MODE, int G, int HG>
 static int launch_power(const Pow2Params& p, cudaStream_t stream) {
   using Ge = Geo<G>;
-  // the transform is latency bound: as many warps as shared memory (tile + staging buffer each) and the
+  // the transform is latency bound: as many warps as shared memory (one tile each, also the staging buffer) and the
   // register file (168 registers at 12 warps, no spills) allow
   constexpr int NW = 16;
-  constexpr bool kShare = true;  // the staged input lives in the warp's transpose tile
   const size_t smem = sizeof(float2) * (32 * 32 + NW * Ge::kTileF2) + sizeof(uint64_t) * NW;
-  auto kern = stft_pow2_power_kernel<POWER_MODE, G, HG, NW, kShare, false>;
+  auto kern = stft_pow2_power_kernel<POWER_MODE, G, HG, NW, false>;
   if constexpr (POWER_MODE != kComplexOut)
-    if (p.kaldi) kern = stft_pow2_power_kernel<POWER_MODE, G, -1, NW, kShare, true>;
+    if (p.kaldi) kern = stft_pow2_power_kernel<POWER_MODE, G, -1, NW, true>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
     return B200A_ECUDA;
   const int64_t grid = persistent_grid(p, NW);

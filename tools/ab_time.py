@@ -1,6 +1,6 @@
-"""A/B timing of library builds / env switches in sub-processes: C2 mel, Spectrogram, C5 512/256, MFCC, resample.
+"""A/B timing of library builds in sub-processes: C2 mel, Spectrogram, C5 512/256, MFCC.
 
-    python tools/ab_time.py NAME=VALUE[,NAME=VALUE] ...     e.g.  B200A_LIB=audio_b200/build/libb200audio_w0.so  B200A_RS=bf16
+    python tools/ab_time.py NAME=VALUE[,NAME=VALUE] ...     e.g.  - B200A_LIB=/tmp/parent/libb200audio.so
 Each argument is one run with those environment variables set ("-" = no change)."""
 import json
 import os
