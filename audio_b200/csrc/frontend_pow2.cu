@@ -13,11 +13,12 @@
 //                                                                    B = (Z[k] - conj Z[N-k]) / 2i
 //   every lane ends with bins k = l + G m (m < 16) of its two frames; |.|^p -> global (Spectrogram: 16
 //   independent warps per CTA), or -> shared memory for the mel contraction.
-//   mel     warp specialised (any filterbank up to 512 filters): 8 transform warps publish power rows,
-//           4 contraction warps multiply each finished tile with the filterbank on the tensor cores:
+//   mel     (any filterbank up to 512 filters) the power tile times the filterbank on the tensor cores:
 //           mma.sync m16n8k8 TF32 with error-compensated operands (P_hi*F_hi + P_lo*F_hi + P_hi*F_lo,
 //           ~2^-21 relative), visiting only the k-steps where a group of 8 filters is non-zero.
-//           (-> dB / log) -> global.
+//           (-> dB / log) -> global.  n_fft <= 1024: 16 uniform warps at 128 registers, each transforms a unit,
+//           publishes its rows between two CTA barriers and contracts its share of the (16-frame tile, filter group)
+//           items.  n_fft = 2048: 8 transform and 4 contraction warps meeting at mbarriers.
 // Nothing but the waveform is read from HBM and nothing but the final features is written.
 //
 // Reference semantics: src/torchaudio/functional/functional.py:54-145 and
@@ -35,12 +36,15 @@ namespace {
 
 constexpr float kKaldiEps = 1.1920928955078125e-07f;  // numeric_limits<float>::epsilon(), kaldi.py:21-22
 constexpr int kPadSymmetric = 4;  // internal pad mode: x[-1-j] = x[j], x[L+j] = x[L-1-j] (Kaldi snip_edges = false)
-constexpr int kWarps = 8;     // transform warps per CTA
-constexpr int kMelWarps = 4;  // contraction warps per CTA (mel kernel)
+constexpr int kWarps = 8;     // transform warps per CTA (n_fft = 2048 kernels)
+constexpr int kMelWarps = 4;  // contraction warps per CTA (n_fft = 2048 mel kernel)
+constexpr int kUniWarps = 16;  // warps per CTA of the 256 / 512 / 1024-point mel kernel, each transforms and contracts
 constexpr int kMaxItems = 64;  // filter groups (of 8) per contraction
 constexpr int kMaxItemsPerWarp = 32;
+constexpr int kMaxMTiles = 8;  // 16-frame MMA tiles per iteration of the 16-warp mel kernel (n_fft = 256: 128 frames)
 constexpr int kFragSmemSteps = 112;  // filterbank fragments kept in shared memory (x 512 B)
-constexpr int kMaxSlots = 64;
+constexpr int kMaxSlots = 128;
+constexpr int kSmemLimit = 227 * 1024;  // dynamic shared memory per CTA on sm_90
 
 // Geometry of one transform size: G lanes per frame pair.
 template <int G>
@@ -49,12 +53,23 @@ struct Geo {
   static constexpr int kBins = kNfft / 2 + 1;
   static constexpr int kGroups = 32 / G;        // frame pairs per warp
   static constexpr int kFrames = 2 * kGroups;   // frames per warp and iteration ("unit")
-  static constexpr int kRowLd = G + 1;          // float2 pitch of one transpose row (bank-conflict free)
+  static constexpr int kRowLd = G + 1;          // pitch of one transpose row (bank-conflict free)
   static constexpr int kRegion = 32 * (G + 1) + (G == 8 ? 8 : 0);  // float2 per lane group (skewed for G = 8)
   static constexpr int kTileF2 = kGroups * kRegion;                // float2 per warp
-  static constexpr int kSlots = kWarps * kFrames;                  // frames finished per CTA iteration
-  static constexpr int kPitch = ((kBins + 7 - 4 + 31) / 32) * 32 + 4;  // floats per power row, == 4 (mod 32)
+  // the mel kernel transposes real and imaginary parts in two float passes: kRegionF floats per lane group, skewed by
+  // G floats so that the 32 / G groups of a warp hit disjoint banks
+  static constexpr int kRegionF = 32 * (G + 1) + (G < 32 ? G : 0);
+  // floats per warp in the mel kernel: the split transpose, or the staged span of a unit (n_fft + (kFrames-1) hop:
+  // hop <= 512 / 330 / 173 at n_fft = 1024 / 512 / 256), whichever is larger; sized to the shared-memory budget
+  static constexpr int kMelRegion = G == 32 ? 1536 : (G == 16 ? 1504 : 1472);
+  // filterbank fragment steps the mel kernel keeps in shared memory (n_fft = 1024, 80 mels: 91)
+  static constexpr int kMelFragSteps = G == 32 ? 100 : kFragSmemSteps;
+  static constexpr int kSlots = kUniWarps * kFrames;               // frames finished per mel CTA iteration
+  static constexpr int kMTiles = kSlots / 16;                      // 16-frame MMA tiles per iteration
+  // floats per power row: every k-step of 8 bins, and == 4 (mod 8) so the A-fragment loads are bank-conflict free
+  static constexpr int kPitch = (kBins + 7) / 8 * 8 + 4;
   static constexpr int kLogG = G == 32 ? 5 : (G == 16 ? 4 : 3);
+  static_assert(kMelRegion >= kGroups * kRegionF && kMelRegion % 4 == 0, "mel warp region");
 };
 
 // The mel contraction D[16 frames][n_mels] = P[16][bins] * F[bins][n_mels] is cut into ITEMS =
@@ -67,9 +82,13 @@ struct MelItem {
   int frag_off;  // index of the first step in the fragment array
 };
 struct MelPlan {  // built on the device by prepare_mma_kernel
-  int n_tiles, n_items, total_steps, pad;
-  int warp_cnt[kWarps];
-  int warp_items[kWarps][kMaxItemsPerWarp];
+  int n_tiles, n_items, total_steps, n_work;
+  // n_fft = 2048 kernel: the filter groups of each of its kMelWarps contraction warps
+  int warp_cnt[kMelWarps];
+  int warp_items[kMelWarps][kMaxItemsPerWarp];
+  // 16-warp mel kernel: warp w contracts work[work_begin[w] .. work_begin[w + 1]), entries (16-frame tile << 8) | group
+  int work_begin[kUniWarps + 4];
+  unsigned short work[kMaxMTiles * kMaxItems];
   MelItem items[kMaxItems];
 };
 
@@ -302,9 +321,11 @@ __device__ __forceinline__ void issue_bulk(const Pow2Params& p, int half, int64_
 // power spectra.  On return lane (group gi, l) holds bins k = l + G m in pa[m] / pb[m] (m < 16) of frames
 // t0 + 2 gi and t0 + 2 gi + 1, and lanes with l == 0 bin n_fft/2 in [16].
 // The staging buffer is the warp's transpose tile itself: the NEXT unit's bulk copy is issued only after
-// pass 2 has read the tile back.
-template <int POWER_MODE, int G, int HG, bool KALDI>
-__device__ __forceinline__ void transform_unit(const Pow2Params& p, const float (&wreg)[32], const float2* s_tw,
+// pass 2 has read the tile back.  s_win: the window x 1/2 (un-packing) x the normalisation scale, [n_fft].
+// SPLIT: transpose the real parts, then the imaginary parts, through kRegionF floats per lane group (half the
+// shared memory of the float2 transpose, kRegion float2 per lane group).
+template <int POWER_MODE, int G, int HG, bool KALDI, bool SPLIT>
+__device__ __forceinline__ void transform_unit(const Pow2Params& p, const float* s_win, const float2* s_tw,
                                                float2* tile, uint64_t* bar, uint32_t& parity, bool& staged,
                                                const UnitCursor& cur, int half, int lane, float (&pa)[17],
                                                float (&pb)[17]) {
@@ -324,6 +345,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
 
   float2 a[32];
   float2* grp_tile = tile + gi * Ge::kRegion;
+  float* grp_f = stage + gi * (SPLIT ? Ge::kRegionF : 2 * Ge::kRegion);  // the lane group's region as floats
   bool from_stage = staged;
   if (staged) {
     mbar_wait(bar, parity);
@@ -399,11 +421,12 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
       float va = 0.f, vb = 0.f;
       if (n < win) {
         const int np = n > 0 ? n - 1 : 0;
-        va = ((fa[n] - ma) - c * (fa[np] - ma)) * wreg[j];
-        vb = ((fb[n] - mb) - c * (fb[np] - mb)) * wreg[j];
+        const float w = s_win[n];
+        va = ((fa[n] - ma) - c * (fa[np] - ma)) * w;
+        vb = ((fb[n] - mb) - c * (fb[np] - mb)) * w;
       }
       a[brev5(j)] = make_float2(va, vb);
-      if (p.k_energy_mode == 2) {  // wreg carries the un-packing's 1/2
+      if (p.k_energy_mode == 2) {  // s_win carries the un-packing's 1/2
         ea = fmaf(2.f * va, 2.f * va, ea);
         eb = fmaf(2.f * vb, 2.f * vb, eb);
       }
@@ -432,14 +455,15 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
       });
       static_for<32>([&](auto ji) {
         constexpr int j = decltype(ji)::value;
-        a[brev5(j)] = make_float2(v[j] * wreg[j], v[j + (HG >= 0 ? HG : 0)] * wreg[j]);
+        const float w = s_win[lane + 32 * j];
+        a[brev5(j)] = make_float2(v[j] * w, v[j + (HG >= 0 ? HG : 0)] * w);
       });
     } else {
       const float* pa_ptr = stage + 2 * gi * p.hop + l;
       const float* pb_ptr = pa_ptr + p.hop;
       static_for<32>([&](auto ji) {
         constexpr int j = decltype(ji)::value;
-        a[brev5(j)] = scale2(wreg[j], make_float2(pa_ptr[G * j], pb_ptr[G * j]));
+        a[brev5(j)] = scale2(s_win[l + G * j], make_float2(pa_ptr[G * j], pb_ptr[G * j]));
       });
     }
     __syncwarp();  // every lane has consumed the staging buffer
@@ -448,25 +472,29 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
       constexpr int j = decltype(ji)::value;
       const float va = has_a ? __ldg(x + sa + l + G * j) : 0.f;
       const float vb = has_b ? __ldg(x + sb + l + G * j) : 0.f;
-      a[brev5(j)] = scale2(wreg[j], make_float2(va, vb));
+      a[brev5(j)] = scale2(s_win[l + G * j], make_float2(va, vb));
     });
   } else {
-    // edge unit whose span does not fit the staging buffer: gather through the group's tile region with a
-    // rolled loop so the index arithmetic is not replicated 64 times in the instruction stream
+    // edge unit whose span does not fit the staging buffer: gather frame a, then frame b, through the group's region
+    // (n_fft floats) with a rolled loop so the index arithmetic is not replicated 64 times in the instruction stream
+#pragma unroll
+    for (int f = 0; f < 2; ++f) {
+      const int64_t t = ta + f;
 #pragma unroll 1
-    for (int j = 0; j < 32; ++j) {
-      const int n = l + G * j;
-      const int64_t ia = has_a ? source_index(ta * p.hop + n, p.length, p.pad, half, p.pad_mode) : -1;
-      const int64_t ib = has_b ? source_index(tb * p.hop + n, p.length, p.pad, half, p.pad_mode) : -1;
-      grp_tile[n] = make_float2(ia >= 0 ? __ldg(x + ia) : 0.f, ib >= 0 ? __ldg(x + ib) : 0.f);
+      for (int j = 0; j < 32; ++j) {
+        const int n = l + G * j;
+        const int64_t i = t < p.frames ? source_index(t * p.hop + n, p.length, p.pad, half, p.pad_mode) : -1;
+        grp_f[n] = i >= 0 ? __ldg(x + i) : 0.f;
+      }
+      __syncwarp();
+      static_for<32>([&](auto ji) {
+        constexpr int j = decltype(ji)::value;
+        const float v = __fmul_rn(s_win[l + G * j], grp_f[l + G * j]);  // the product scale2 forms
+        if (f == 0) a[brev5(j)].x = v;
+        else a[brev5(j)].y = v;
+      });
+      __syncwarp();
     }
-    __syncwarp();
-    static_for<32>([&](auto ji) {
-      constexpr int j = decltype(ji)::value;
-      const float2 v = grp_tile[l + G * j];
-      a[brev5(j)] = scale2(wreg[j], v);
-    });
-    __syncwarp();
   }
 
   // the inter-pass twiddles: kTwAhead loads are in flight before the last butterfly stage, and every multiply
@@ -479,19 +507,46 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
     tw[k2] = s_tw[k2 * G + l];
   });
   fft_regs<32, 0, 4, 5>(a);  // a[k2] = Y[l][k2]
-  grp_tile[l] = a[0];
-  static_for<31>([&](auto ki) {
-    constexpr int k2 = decltype(ki)::value + 1;
-    if constexpr (k2 + kTwAhead < 32) tw[k2 + kTwAhead] = s_tw[(k2 + kTwAhead) * G + l];
-    grp_tile[k2 * Ge::kRowLd + l] = cmul2(a[k2], tw[k2]);
-  });
-  __syncwarp();
-  // lane l now owns k2 = l + G q, q < 32/G: slot q*G + brev(g) <- element (g, l + G q)
-  static_for<32>([&](auto si) {
-    constexpr int s = decltype(si)::value;
-    constexpr int q = s / G, g = s % G;
-    a[q * G + brev<Ge::kLogG>(g)] = grp_tile[(l + G * q) * Ge::kRowLd + g];
-  });
+  // lane l then owns k2 = l + G q, q < 32/G: slot q*G + brev(g) <- element (g, l + G q)
+  if constexpr (SPLIT) {
+    grp_f[l] = a[0].x;
+    static_for<31>([&](auto ki) {
+      constexpr int k2 = decltype(ki)::value + 1;
+      if constexpr (k2 + kTwAhead < 32) tw[k2 + kTwAhead] = s_tw[(k2 + kTwAhead) * G + l];
+      a[k2] = cmul2(a[k2], tw[k2]);
+      grp_f[k2 * Ge::kRowLd + l] = a[k2].x;
+    });
+    __syncwarp();
+    float re[32];
+    static_for<32>([&](auto si) {
+      constexpr int s = decltype(si)::value;
+      re[s] = grp_f[(l + G * (s / G)) * Ge::kRowLd + s % G];
+    });
+    __syncwarp();
+    static_for<32>([&](auto ki) {
+      constexpr int k2 = decltype(ki)::value;
+      grp_f[k2 * Ge::kRowLd + l] = a[k2].y;
+    });
+    __syncwarp();
+    static_for<32>([&](auto si) {
+      constexpr int s = decltype(si)::value;
+      constexpr int q = s / G, g = s % G;
+      a[q * G + brev<Ge::kLogG>(g)] = make_float2(re[s], grp_f[(l + G * q) * Ge::kRowLd + g]);
+    });
+  } else {
+    grp_tile[l] = a[0];
+    static_for<31>([&](auto ki) {
+      constexpr int k2 = decltype(ki)::value + 1;
+      if constexpr (k2 + kTwAhead < 32) tw[k2 + kTwAhead] = s_tw[(k2 + kTwAhead) * G + l];
+      grp_tile[k2 * Ge::kRowLd + l] = cmul2(a[k2], tw[k2]);
+    });
+    __syncwarp();
+    static_for<32>([&](auto si) {
+      constexpr int s = decltype(si)::value;
+      constexpr int q = s / G, g = s % G;
+      a[q * G + brev<Ge::kLogG>(g)] = grp_tile[(l + G * q) * Ge::kRowLd + g];
+    });
+  }
   __syncwarp();
   staged = next_staged;  // the tile is free until the next unit's transpose: stage into it
   if (staged && lane == 0) {
@@ -548,28 +603,27 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float 
   }
 }
 
-template <int G>
-__device__ __forceinline__ void load_window(const Pow2Params& p, int lane, float (&wreg)[32]) {
-  // window (x 1/2 from the un-packing, x the normalisation scale) for n = l + G j
+// the window x 1/2 (from the un-packing) x the normalisation scale, [n] into shared memory
+__device__ __forceinline__ void load_window(const Pow2Params& p, float* s_win, int n, int tid, int nthreads) {
   const float hs = 0.5f * p.hdr->scale;
-  const int l = lane % G;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) wreg[j] = p.window[l + G * j] * hs;
+  for (int i = tid; i < n; i += nthreads) s_win[i] = p.window[i] * hs;
 }
 
 // ------------------------------------------------------------------------------------------------
-// Spectrogram kernel: 8 independent warps, power spectra straight to global memory.
+// Spectrogram kernel: NW independent warps, power spectra straight to global memory.
 // ------------------------------------------------------------------------------------------------
 template <int POWER_MODE, int G, int HG, int NW, bool KALDI>
 __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2Params p) {
   using Ge = Geo<G>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2* s_tw = reinterpret_cast<float2*>(smem_raw);                                    // [32][G]
-  float2* s_tile_all = s_tw + 32 * 32;                                                   // [NW][kTileF2] (also staging)
+  float* s_win = reinterpret_cast<float*>(s_tw + 32 * 32);                               // [n_fft]
+  float2* s_tile_all = reinterpret_cast<float2*>(s_win + Ge::kNfft);                     // [NW][kTileF2] (also staging)
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_tile_all + NW * Ge::kTileF2);          // [NW]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
+  load_window(p, s_win, Ge::kNfft, tid, blockDim.x);
   if (tid < NW) mbar_init(s_bar + tid, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   __syncthreads();
@@ -577,8 +631,6 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   float2* tile = s_tile_all + warp * Ge::kTileF2;
   float* stage = reinterpret_cast<float*>(tile);
   uint64_t* bar = s_bar + warp;
-  float wreg[32];
-  load_window<G>(p, lane, wreg);
   const int half = frame_lead(p, Ge::kNfft);
   const int gi = lane / G, l = lane % G;
   uint32_t parity = 0;
@@ -591,7 +643,7 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   }
   for (; cur.u < p.total_units; cur.advance()) {
     float pa[17], pb[17];
-    transform_unit<POWER_MODE, G, HG, KALDI>(p, wreg, s_tw, tile, bar, parity, staged, cur, half, lane, pa, pb);
+    transform_unit<POWER_MODE, G, HG, KALDI, false>(p, s_win, s_tw, tile, bar, parity, staged, cur, half, lane, pa, pb);
     if constexpr (POWER_MODE == kComplexOut) continue;  // transform_unit has written the complex spectra
     const int64_t ta = cur.ub * Ge::kFrames + 2 * gi;
     const bool has_a = ta < p.frames, has_b = ta + 1 < p.frames;
@@ -618,200 +670,197 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   }
 }
 
-// One contraction warp's share of a 16-frame power tile: D[16 x 8] = P[16 x bins] * F[bins x 8] for each of its
-// filter groups on the tensor pipe, (dB / log), store.  pw: the tile's 16 power rows (pitch PITCH);
-// slot / grp: output offset (or -1) and top_db group of each of the 16 rows.
+// One filter group of a 16-frame power tile: D[16 x 8] = P[16 x bins] * F[bins x 8] on the tensor pipe, (dB / log),
+// store.  pw: the tile's 16 power rows (pitch PITCH); o_lo / o_hi, g_lo / g_hi: output offset (or -1) and top_db
+// group of rows r and r + 8 (r = lane / 4).
 template <int PITCH>
-__device__ __forceinline__ void contract_tile(const Pow2Params& p, const MelPlan* s_plan, const float4* s_frags,
-                                              bool frags_in_smem, int mw, int lane, const float* pw,
-                                              const int64_t* slot, const int64_t* grp, GroupMax& gmax) {
+__device__ __forceinline__ void contract_item(const Pow2Params& p, const MelItem& mi, const float4* s_frags,
+                                              bool frags_in_smem, int lane, const float* pw, int64_t o_lo,
+                                              int64_t o_hi, int64_t g_lo, int64_t g_hi, GroupMax& gmax) {
   const int r = lane >> 2, c = lane & 3;
-  const int cnt = s_plan->warp_cnt[mw];
-  const int64_t o_lo = slot[r], o_hi = slot[r + 8];
-  const int64_t g_lo = grp[r], g_hi = grp[r + 8];
-  for (int ii = 0; ii < cnt; ++ii) {
-    const MelItem mi = s_plan->items[s_plan->warp_items[mw][ii]];
-    const float* a_lo_row = pw + (size_t)r * PITCH + mi.kstart + c;
-    const float* a_hi_row = a_lo_row + 8 * PITCH;
-    // three independent accumulator chains (hi*hi, lo*hi, hi*lo), summed in a fixed order
-    float d0[4] = {0.f, 0.f, 0.f, 0.f}, d1[4] = {0.f, 0.f, 0.f, 0.f}, d2[4] = {0.f, 0.f, 0.f, 0.f};
-    auto contract = [&](auto in_smem) {
-      const float4* fr = (decltype(in_smem)::value ? s_frags : p.frags) + (size_t)mi.frag_off * 32 + lane;
+  const float* a_lo_row = pw + (size_t)r * PITCH + mi.kstart + c;
+  const float* a_hi_row = a_lo_row + 8 * PITCH;
+  // three independent accumulator chains (hi*hi, lo*hi, hi*lo), summed in a fixed order
+  float d0[4] = {0.f, 0.f, 0.f, 0.f}, d1[4] = {0.f, 0.f, 0.f, 0.f}, d2[4] = {0.f, 0.f, 0.f, 0.f};
+  auto contract = [&](auto in_smem) {
+    const float4* fr = (decltype(in_smem)::value ? s_frags : p.frags) + (size_t)mi.frag_off * 32 + lane;
 #pragma unroll 4
-      for (int s = 0; s < mi.nsteps; ++s) {
-        float4 bf;
-        if constexpr (decltype(in_smem)::value) bf = fr[(size_t)s * 32];
-        else bf = __ldg(fr + (size_t)s * 32);
-        const float av[4] = {a_lo_row[8 * s], a_hi_row[8 * s], a_lo_row[8 * s + 4], a_hi_row[8 * s + 4]};
-        uint32_t hi[4], lo[4];
+    for (int s = 0; s < mi.nsteps; ++s) {
+      float4 bf;
+      if constexpr (decltype(in_smem)::value) bf = fr[(size_t)s * 32];
+      else bf = __ldg(fr + (size_t)s * 32);
+      const float av[4] = {a_lo_row[8 * s], a_hi_row[8 * s], a_lo_row[8 * s + 4], a_hi_row[8 * s + 4]};
+      uint32_t hi[4], lo[4];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) split_tf32(av[q], hi[q], lo[q]);
-        mma_tf32(d0, hi, __float_as_uint(bf.x), __float_as_uint(bf.y));
-        mma_tf32(d1, lo, __float_as_uint(bf.x), __float_as_uint(bf.y));
-        mma_tf32(d2, hi, __float_as_uint(bf.z), __float_as_uint(bf.w));
-      }
-    };
-    if (frags_in_smem) contract(std::true_type{});
-    else contract(std::false_type{});
-    float d[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) d[q] = d0[q] + (d1[q] + d2[q]);
-    const int n0 = 8 * mi.tile + 2 * c;
-    const bool n0_ok = n0 < p.n_mels, n1_ok = n0 + 1 < p.n_mels;
-    if (p.k_log) {  // Kaldi fbank: log(max(mel, FLT_EPSILON)), kaldi.py:629-631
-#pragma unroll
-      for (int q = 0; q < 4; ++q) d[q] = logf(fmaxf(d[q], kKaldiEps));
+      for (int q = 0; q < 4; ++q) split_tf32(av[q], hi[q], lo[q]);
+      mma_tf32(d0, hi, __float_as_uint(bf.x), __float_as_uint(bf.y));
+      mma_tf32(d1, lo, __float_as_uint(bf.x), __float_as_uint(bf.y));
+      mma_tf32(d2, hi, __float_as_uint(bf.z), __float_as_uint(bf.w));
     }
-    if (p.stage == B200A_STAGE_FEAT) {
+  };
+  if (frags_in_smem) contract(std::true_type{});
+  else contract(std::false_type{});
+  float d[4];
 #pragma unroll
-      for (int q = 0; q < 4; ++q)
-        d[q] = p.log_mels ? logf(d[q] + 1e-6f) : p.db_mult * log10f(fmaxf(d[q], p.db_amin)) - p.db_offset;
-      const float m_lo = fmaxf(n0_ok ? d[0] : -CUDART_INF_F, n1_ok ? d[1] : -CUDART_INF_F);
-      const float m_hi = fmaxf(n0_ok ? d[2] : -CUDART_INF_F, n1_ok ? d[3] : -CUDART_INF_F);
-      gmax.add(g_lo, m_lo, o_lo >= 0);
-      gmax.add(g_hi, m_hi, o_hi >= 0);
+  for (int q = 0; q < 4; ++q) d[q] = d0[q] + (d1[q] + d2[q]);
+  const int n0 = 8 * mi.tile + 2 * c;
+  const bool n0_ok = n0 < p.n_mels, n1_ok = n0 + 1 < p.n_mels;
+  if (p.k_log) {  // Kaldi fbank: log(max(mel, FLT_EPSILON)), kaldi.py:629-631
+#pragma unroll
+    for (int q = 0; q < 4; ++q) d[q] = logf(fmaxf(d[q], kKaldiEps));
+  }
+  if (p.stage == B200A_STAGE_FEAT) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      d[q] = p.log_mels ? logf(d[q] + 1e-6f) : p.db_mult * log10f(fmaxf(d[q], p.db_amin)) - p.db_offset;
+    const float m_lo = fmaxf(n0_ok ? d[0] : -CUDART_INF_F, n1_ok ? d[1] : -CUDART_INF_F);
+    const float m_hi = fmaxf(n0_ok ? d[2] : -CUDART_INF_F, n1_ok ? d[3] : -CUDART_INF_F);
+    gmax.add(g_lo, m_lo, o_lo >= 0);
+    gmax.add(g_hi, m_hi, o_hi >= 0);
+  }
+  const bool vec = n1_ok && p.out_vec >= 2;  // 8-byte aligned pair
+  if (o_lo >= 0) {
+    if (vec) *reinterpret_cast<float2*>(p.out + o_lo + n0) = make_float2(d[0], d[1]);
+    else {
+      if (n0_ok) p.out[o_lo + n0] = d[0];
+      if (n1_ok) p.out[o_lo + n0 + 1] = d[1];
     }
-    const bool vec = n1_ok && p.out_vec >= 2;  // 8-byte aligned pair
-    if (o_lo >= 0) {
-      if (vec) *reinterpret_cast<float2*>(p.out + o_lo + n0) = make_float2(d[0], d[1]);
-      else {
-        if (n0_ok) p.out[o_lo + n0] = d[0];
-        if (n1_ok) p.out[o_lo + n0 + 1] = d[1];
-      }
-    }
-    if (o_hi >= 0) {
-      if (vec) *reinterpret_cast<float2*>(p.out + o_hi + n0) = make_float2(d[2], d[3]);
-      else {
-        if (n0_ok) p.out[o_hi + n0] = d[2];
-        if (n1_ok) p.out[o_hi + n0 + 1] = d[3];
-      }
+  }
+  if (o_hi >= 0) {
+    if (vec) *reinterpret_cast<float2*>(p.out + o_hi + n0) = make_float2(d[2], d[3]);
+    else {
+      if (n0_ok) p.out[o_hi + n0] = d[2];
+      if (n1_ok) p.out[o_hi + n0 + 1] = d[3];
     }
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Mel / MFCC-feature kernel, warp specialised: warps 0-7 transform (one unit each per iteration)
-// and publish power rows into a double-buffered shared tile; warps 8-11 contract each finished tile
-// (16, 32 or 64 frames) with the filterbank on the tensor pipe and store the features.  The two groups
-// only meet at the tile's full/empty mbarriers, so the FFT warps never wait for the contraction.
-// ------------------------------------------------------------------------------------------------
-constexpr int kFftRegs = 200, kMelRegs = 96;  // 256*200 + 128*96 = 63488 <= 64512 = 384 * 168
+// The n_fft = 2048 contraction warp mw's share of a 16-frame power tile: its filter groups, one after the other.
+template <int PITCH>
+__device__ __forceinline__ void contract_tile(const Pow2Params& p, const MelPlan* s_plan, const float4* s_frags,
+                                              bool frags_in_smem, int mw, int lane, const float* pw,
+                                              const int64_t* slot, const int64_t* grp, GroupMax& gmax) {
+  const int r = lane >> 2;
+  const int cnt = s_plan->warp_cnt[mw];
+  const int64_t o_lo = slot[r], o_hi = slot[r + 8];
+  const int64_t g_lo = grp[r], g_hi = grp[r + 8];
+  for (int ii = 0; ii < cnt; ++ii)
+    contract_item<PITCH>(p, s_plan->items[s_plan->warp_items[mw][ii]], s_frags, frags_in_smem, lane, pw, o_lo, o_hi,
+                         g_lo, g_hi, gmax);
+}
 
-template <int POWER_MODE, int G, int HG, int FFT_REGS, bool KALDI>
-__device__ __forceinline__ void mel_body_mma(const Pow2Params& p, unsigned char* smem_raw) {
+// ------------------------------------------------------------------------------------------------
+// Mel / MFCC-feature kernel (n_fft = 256 / 512 / 1024): 16 uniform warps.  Every iteration each warp transforms
+// one unit, waits at a CTA barrier until the previous contraction has read the (single) power tile, publishes
+// its power rows, waits at a second barrier and then contracts its share of the tile's (16-frame MMA tile,
+// filter group) items on the tensor pipe and stores the features.  The transform is latency bound, so the warps
+// are not specialised: all 16 run the FFT at 128 registers, which is what hides its stalls.
+// ------------------------------------------------------------------------------------------------
+constexpr int kFftRegs = 200, kMelRegs = 96;  // n_fft = 2048: 256*200 + 128*96 = 63488 <= 64512 = 384 * 168
+
+// shared memory of the 16-warp mel kernel, in the order of the carve-up in mel_body
+template <int G>
+constexpr size_t mel_smem_bytes() {
+  using Ge = Geo<G>;
+  return sizeof(float2) * 32 * G + sizeof(float) * Ge::kNfft + sizeof(float) * kUniWarps * Ge::kMelRegion +
+         sizeof(float) * Ge::kSlots * Ge::kPitch + sizeof(int64_t) * 2 * Ge::kSlots + sizeof(uint64_t) * kUniWarps +
+         sizeof(MelPlan) + sizeof(float4) * 32 * Ge::kMelFragSteps;
+}
+
+template <int POWER_MODE, int G, int HG, bool KALDI>
+__device__ __forceinline__ void mel_body(const Pow2Params& p, unsigned char* smem_raw) {
   using Ge = Geo<G>;
   constexpr int kSlots = Ge::kSlots, kPitch = Ge::kPitch;
   float2* s_tw = reinterpret_cast<float2*>(smem_raw);                              // [32][G]
-  float2* s_tile_all = s_tw + 32 * 32;                                             // [kWarps][kTileF2] (also staging)
-  float* s_pow = reinterpret_cast<float*>(s_tile_all + kWarps * Ge::kTileF2);      // [2][kSlots][kPitch]
-  int64_t* s_slot = reinterpret_cast<int64_t*>(s_pow + 2 * kSlots * kPitch);        // [2][kSlots] out offsets
-  int64_t* s_grp = s_slot + 2 * kSlots;                                            // [2][kSlots] top_db group
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_grp + 2 * kSlots);               // [kWarps] staging
-  uint64_t* s_full = s_bar + kWarps;                                               // [2]
-  uint64_t* s_empty = s_full + 2;                                                  // [2]
-  MelPlan* s_plan = reinterpret_cast<MelPlan*>(s_empty + 2);
-  float4* s_frags = reinterpret_cast<float4*>(s_plan + 1);                         // [<= kFragSmemSteps][32]
+  float* s_win = reinterpret_cast<float*>(s_tw + 32 * G);                          // [n_fft]
+  float* s_region_all = s_win + Ge::kNfft;                                         // [kUniWarps][kMelRegion]
+  float* s_pow = s_region_all + kUniWarps * Ge::kMelRegion;                        // [kSlots][kPitch]
+  int64_t* s_slot = reinterpret_cast<int64_t*>(s_pow + kSlots * kPitch);           // [kSlots] out offsets
+  int64_t* s_grp = s_slot + kSlots;                                                // [kSlots] top_db group
+  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_grp + kSlots);                   // [kUniWarps] staging
+  MelPlan* s_plan = reinterpret_cast<MelPlan*>(s_bar + kUniWarps);
+  float4* s_frags = reinterpret_cast<float4*>(s_plan + 1);                         // [<= kMelFragSteps][32]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
+  load_window(p, s_win, Ge::kNfft, tid, blockDim.x);
   {
     const int* src = reinterpret_cast<const int*>(p.plan);
     int* dst = reinterpret_cast<int*>(s_plan);
     for (int i = tid; i < (int)(sizeof(MelPlan) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
   }
   const int total_steps = p.plan->total_steps;
-  const bool frags_in_smem = total_steps <= kFragSmemSteps;
+  const bool frags_in_smem = total_steps <= Ge::kMelFragSteps;
   if (frags_in_smem)
     for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
   // columns >= n_bins of every power row are read by the last k-step: keep them finite (zero)
-  for (int i = tid; i < 2 * kSlots * (kPitch - Ge::kBins); i += blockDim.x) {
+  for (int i = tid; i < kSlots * (kPitch - Ge::kBins); i += blockDim.x) {
     const int r = i / (kPitch - Ge::kBins), c = i - r * (kPitch - Ge::kBins);
     s_pow[r * kPitch + Ge::kBins + c] = 0.f;
   }
-  if (tid < kWarps) mbar_init(s_bar + tid, 1);
-  if (tid == 0) {
-    mbar_init(s_full + 0, kWarps);
-    mbar_init(s_full + 1, kWarps);
-    mbar_init(s_empty + 0, kMelWarps);
-    mbar_init(s_empty + 1, kMelWarps);
-  }
+  if (tid < kUniWarps) mbar_init(s_bar + tid, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   __syncthreads();
 
-  const int64_t stride = (int64_t)gridDim.x * kWarps;
-  const int64_t u0 = (int64_t)blockIdx.x * kWarps;
+  const int64_t stride = (int64_t)gridDim.x * kUniWarps;
+  const int64_t u0 = (int64_t)blockIdx.x * kUniWarps;
   const int width = p.out_width;
-
-  if (warp < kWarps) {
-    // =============================== transform warps ===========================================
-    reg_alloc<FFT_REGS>();
-    float2* tile = s_tile_all + warp * Ge::kTileF2;
-    float* stage = reinterpret_cast<float*>(tile);
-    uint64_t* bar = s_bar + warp;
-    float wreg[32];
-    load_window<G>(p, lane, wreg);
-    const int half = frame_lead(p, Ge::kNfft);
-    const int gi = lane / G, l = lane % G;
-    uint32_t parity = 0;
-    bool staged = false;
-    UnitCursor cur;
-    cur.init(u0 + warp, stride, p.units_per_row);
-    if (bulk_eligible<G>(p, half, cur.u, cur.ub)) {
-      if (lane == 0) issue_bulk<G>(p, half, cur.row, cur.ub, stage, bar);
-      staged = true;
-    }
-    int it = 0;
-    for (int64_t base = u0; base < p.total_units; base += stride, ++it, cur.advance()) {
-      const bool valid = cur.u < p.total_units;
-      float pa[17], pb[17];
-      if (valid)
-        transform_unit<POWER_MODE, G, HG, KALDI>(p, wreg, s_tw, tile, bar, parity, staged, cur, half, lane, pa, pb);
-      const int b = it & 1;
-      if (it >= 2) mbar_wait(s_empty + b, ((it >> 1) & 1) ^ 1);  // the mel warps have drained this buffer
-      const int slot_a = Ge::kFrames * warp + 2 * gi;
-      float* prow_a = s_pow + (size_t)(b * kSlots + slot_a) * kPitch;
-      float* prow_b = prow_a + kPitch;
-      if (valid) {
+  float2* tile = reinterpret_cast<float2*>(s_region_all + warp * Ge::kMelRegion);
+  float* stage = reinterpret_cast<float*>(tile);
+  uint64_t* bar = s_bar + warp;
+  const int half = frame_lead(p, Ge::kNfft);
+  const int gi = lane / G, l = lane % G;
+  const int work_begin = s_plan->work_begin[warp], work_end = s_plan->work_begin[warp + 1];
+  GroupMax gmax{p.stage == B200A_STAGE_FEAT ? p.group_max : nullptr, -1, -CUDART_INF_F};
+  uint32_t parity = 0;
+  bool staged = false;
+  UnitCursor cur;
+  cur.init(u0 + warp, stride, p.units_per_row);
+  if (bulk_eligible<G>(p, half, cur.u, cur.ub)) {
+    if (lane == 0) issue_bulk<G>(p, half, cur.row, cur.ub, stage, bar);
+    staged = true;
+  }
+  for (int64_t base = u0; base < p.total_units; base += stride, cur.advance()) {
+    const bool valid = cur.u < p.total_units;
+    float pa[17], pb[17];
+    if (valid)
+      transform_unit<POWER_MODE, G, HG, KALDI, true>(p, s_win, s_tw, tile, bar, parity, staged, cur, half, lane, pa, pb);
+    __syncthreads();  // the previous iteration's contraction has read the power tile and the slot table
+    const int slot_a = Ge::kFrames * warp + 2 * gi;
+    float* prow_a = s_pow + (size_t)slot_a * kPitch;
+    float* prow_b = prow_a + kPitch;
+    if (valid) {
 #pragma unroll
-        for (int m = 0; m < 16; ++m) {
-          prow_a[l + G * m] = pa[m];
-          prow_b[l + G * m] = pb[m];
-        }
-        if (l == 0) {
-          prow_a[Ge::kNfft / 2] = pa[16];
-          prow_b[Ge::kNfft / 2] = pb[16];
-        }
+      for (int m = 0; m < 16; ++m) {
+        prow_a[l + G * m] = pa[m];
+        prow_b[l + G * m] = pb[m];
       }
       if (l == 0) {
-        const int64_t ta = cur.ub * Ge::kFrames + 2 * gi;
-        const int64_t oa = (cur.row * p.frames + ta) * (int64_t)width + p.out_col0;
-        s_slot[b * kSlots + slot_a] = (valid && ta < p.frames) ? oa : -1;
-        s_slot[b * kSlots + slot_a + 1] = (valid && ta + 1 < p.frames) ? oa + width : -1;
-        const int64_t g = cur.row / p.rows_per_group;
-        s_grp[b * kSlots + slot_a] = g;
-        s_grp[b * kSlots + slot_a + 1] = g;
+        prow_a[Ge::kNfft / 2] = pa[16];
+        prow_b[Ge::kNfft / 2] = pb[16];
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_full + b);
     }
-  } else {
-    // =============================== contraction warps =========================================
-    reg_dealloc<kMelRegs>();
-    const int mw = warp - kWarps;
-    GroupMax gmax{p.stage == B200A_STAGE_FEAT ? p.group_max : nullptr, -1, -CUDART_INF_F};
-    int it = 0;
-    for (int64_t base = u0; base < p.total_units; base += stride, ++it) {
-      const int b = it & 1;
-      mbar_wait(s_full + b, (it >> 1) & 1);
+    if (l == 0) {
+      const int64_t ta = cur.ub * Ge::kFrames + 2 * gi;
+      const int64_t oa = (cur.row * p.frames + ta) * (int64_t)width + p.out_col0;
+      s_slot[slot_a] = (valid && ta < p.frames) ? oa : -1;
+      s_slot[slot_a + 1] = (valid && ta + 1 < p.frames) ? oa + width : -1;
+      const int64_t g = cur.row / p.rows_per_group;
+      s_grp[slot_a] = g;
+      s_grp[slot_a + 1] = g;
+    }
+    __syncthreads();  // every power row of this iteration is in place
 #pragma unroll 1
-      for (int mt = 0; mt < kSlots / 16; ++mt)  // 16-frame MMA tiles of this iteration
-        contract_tile<kPitch>(p, s_plan, s_frags, frags_in_smem, mw, lane, s_pow + (size_t)(b * kSlots + 16 * mt) * kPitch,
-                              s_slot + b * kSlots + 16 * mt, s_grp + b * kSlots + 16 * mt, gmax);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty + b);
+    for (int i = work_begin; i < work_end; ++i) {
+      const int w = s_plan->work[i], mt = w >> 8;
+      const int64_t* slot = s_slot + 16 * mt;
+      const int64_t* grp = s_grp + 16 * mt;
+      const int r = lane >> 2;
+      contract_item<kPitch>(p, s_plan->items[w & 255], s_frags, frags_in_smem, lane, s_pow + (size_t)16 * mt * kPitch,
+                            slot[r], slot[r + 8], grp[r], grp[r + 8], gmax);
     }
-    gmax.flush();
   }
+  gmax.flush();
 }
 
 // ================================================================================================
@@ -1098,12 +1147,11 @@ __global__ void prepare_tw_eo_kernel(float2* tw_eo) {  // [17][32]: W_2048^(l + 
   }
 }
 
-// The mel / MFCC-feature kernel: 8 transform warps and 4 mma.sync contraction warps (three warpgroups, so each
-// setmaxnreg covers whole warpgroups).
+// The mel / MFCC-feature kernel: 16 warps at 128 registers, each transforming and contracting (mel_body).
 template <int POWER_MODE, int G, int HG, bool KALDI>
-__global__ void __launch_bounds__((kWarps + kMelWarps) * 32, 1) stft_pow2_mel_kernel(const Pow2Params p) {
+__global__ void __launch_bounds__(kUniWarps * 32, 1) stft_pow2_mel_kernel(const Pow2Params p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  mel_body_mma<POWER_MODE, G, HG, kFftRegs, KALDI>(p, smem_raw);
+  mel_body<POWER_MODE, G, HG, KALDI>(p, smem_raw);
 }
 
 // ================================================================================================
@@ -1133,18 +1181,17 @@ __global__ void __launch_bounds__(kIsWarps * 32, 1) istft_pow2_kernel(const Istf
   constexpr int N = Ge::kNfft, NG = Ge::kGroups;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2* s_tw = reinterpret_cast<float2*>(smem_raw);  // [32][G]
-  float2* s_tile_all = s_tw + 32 * G;                  // [kIsWarps][kTileF2]
+  float* s_win = reinterpret_cast<float*>(s_tw + 32 * G);  // [N] window / (N * forward normalisation)
+  float2* s_tile_all = reinterpret_cast<float2*>(s_win + N);  // [kIsWarps][kTileF2]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
+  {
+    const float gain = 1.f / ((float)N * p.hdr->scale);
+    for (int i = tid; i < N; i += blockDim.x) s_win[i] = p.window[i] * gain;
+  }
   __syncthreads();
   float2* grp_tile = s_tile_all + warp * Ge::kTileF2 + (lane / G) * Ge::kRegion;
   const int gi = lane / G, l = lane % G;
-  float wreg[32];
-  {
-    const float gain = 1.f / ((float)N * p.hdr->scale);
-#pragma unroll
-    for (int m = 0; m < 32; ++m) wreg[m] = p.window[l + G * m] * gain;
-  }
   UnitCursor cur;
   cur.init((int64_t)blockIdx.x * kIsWarps + warp, (int64_t)gridDim.x * kIsWarps, p.units_per_row);
   for (; cur.u < p.total_units; cur.advance()) {
@@ -1187,8 +1234,9 @@ __global__ void __launch_bounds__(kIsWarps * 32, 1) istft_pow2_kernel(const Istf
     static_for<32>([&](auto mi) {
       constexpr int m = decltype(mi)::value;
       constexpr int slot = (m % NG) * G + m / NG;
-      if (has_a) fa[G * m] = a[slot].x * wreg[m];
-      if (has_b) fa[N + G * m] = -a[slot].y * wreg[m];
+      const float w = s_win[l + G * m];
+      if (has_a) fa[G * m] = a[slot].x * w;
+      if (has_b) fa[N + G * m] = -a[slot].y * w;
     });
   }
 }
@@ -1206,10 +1254,12 @@ __global__ void prepare_tw2d_kernel(float2* tw2d, int G) {
 
 // Builds the mel contraction plan: per group of 8 filters the 8-bin k-steps its non-zero bins span,
 // groups spread over the contraction warps by descending size; and the filterbank values split
-// into TF32 hi/lo parts in mma.m16n8k8 B-fragment order.
+// into TF32 hi/lo parts in mma.m16n8k8 B-fragment order.  n_mtiles > 0: also the 16-warp kernel's work lists,
+// every (16-frame tile, group) pair of an iteration spread over the kUniWarps warps the same way.
 __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __restrict__ bands, int n_bins, int n_mels,
-                                   int n_tiles, MelPlan* plan, float4* frags) {
-  __shared__ int t_kstart[kMaxItems], t_steps[kMaxItems];
+                                   int n_tiles, int n_mtiles, MelPlan* plan, float4* frags) {
+  __shared__ int t_kstart[kMaxItems], t_steps[kMaxItems], order[kMaxItems];
+  __shared__ unsigned char owner[kMaxMTiles * kMaxItems];
   if (threadIdx.x == 0) {
     int total = 0;
     for (int t = 0; t < n_tiles; ++t) {
@@ -1226,23 +1276,45 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
     plan->n_tiles = n_tiles;
     plan->n_items = n_tiles;
     plan->total_steps = total;
-    plan->pad = 0;
+    plan->n_work = n_mtiles * n_tiles;
     // longest-processing-time-first assignment of the groups to the contraction warps
-    int load[kWarps];
+    int load[kUniWarps], cnt[kUniWarps];
     bool used[kMaxItems];
-    for (int w = 0; w < kWarps; ++w) { load[w] = 0; plan->warp_cnt[w] = 0; }
+    for (int w = 0; w < kMelWarps; ++w) { load[w] = 0; plan->warp_cnt[w] = 0; }
     for (int i = 0; i < n_tiles; ++i) used[i] = false;
     for (int k = 0; k < n_tiles; ++k) {
       int best = -1;
       for (int i = 0; i < n_tiles; ++i)
         if (!used[i] && (best < 0 || t_steps[i] > t_steps[best])) best = i;
       used[best] = true;
+      order[k] = best;
       int w = 0;
       for (int q = 1; q < kMelWarps; ++q)
         if (load[q] < load[w] || (load[q] == load[w] && plan->warp_cnt[q] < plan->warp_cnt[w])) w = q;
       plan->warp_items[w][plan->warp_cnt[w]++] = best;
       load[w] += t_steps[best] + 2;  // + epilogue cost
     }
+    // the same for the (tile, group) pairs over the 16 uniform warps, then listed warp by warp
+    for (int w = 0; w < kUniWarps; ++w) { load[w] = 0; cnt[w] = 0; }
+    for (int k = 0; k < n_tiles; ++k)
+      for (int mt = 0; mt < n_mtiles; ++mt) {
+        int w = 0;
+        for (int q = 1; q < kUniWarps; ++q)
+          if (load[q] < load[w] || (load[q] == load[w] && cnt[q] < cnt[w])) w = q;
+        owner[k * n_mtiles + mt] = (unsigned char)w;
+        ++cnt[w];
+        load[w] += t_steps[order[k]] + 2;
+      }
+    int begin = 0;
+    for (int w = 0; w < kUniWarps; ++w) {
+      plan->work_begin[w] = begin;
+      begin += cnt[w];
+      cnt[w] = plan->work_begin[w];  // fill cursor
+    }
+    for (int w = kUniWarps; w < kUniWarps + 4; ++w) plan->work_begin[w] = begin;
+    for (int k = 0; k < n_tiles; ++k)
+      for (int mt = 0; mt < n_mtiles; ++mt)
+        plan->work[cnt[owner[k * n_mtiles + mt]]++] = (unsigned short)((mt << 8) | order[k]);
   }
   __syncthreads();
   int off = 0;
@@ -1282,9 +1354,10 @@ int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaSt
   prepare_tw2d_kernel<<<(32 * G + 255) / 256, 256, 0, stream>>>(reinterpret_cast<float2*>(base + e.tw2d), G);
   if (d->n_fft == 2048) prepare_tw_eo_kernel<<<3, 256, 0, stream>>>(reinterpret_cast<float2*>(base + e.tw_eo));
   if (d->n_mels > 0 && mel_tiles(d->n_mels) <= kMaxItems) {
+    const int n_mtiles = d->n_fft == 2048 ? 0 : kUniWarps * 2 * (32 / G) / 16;  // Geo<G>::kMTiles
     prepare_mma_kernel<<<1, 256, 0, stream>>>(reinterpret_cast<const float*>(base + l.fb),
                                               reinterpret_cast<const int2*>(base + l.bands), d->n_fft / 2 + 1, d->n_mels,
-                                              mel_tiles(d->n_mels), reinterpret_cast<MelPlan*>(base + e.plan),
+                                              mel_tiles(d->n_mels), n_mtiles, reinterpret_cast<MelPlan*>(base + e.plan),
                                               reinterpret_cast<float4*>(base + e.frags));
   }
   return launch_status();
@@ -1307,7 +1380,7 @@ static int launch_power(const Pow2Params& p, cudaStream_t stream) {
   // the transform is latency bound: as many warps as shared memory (one tile each, also the staging buffer) and the
   // register file (168 registers at 12 warps, no spills) allow
   constexpr int NW = 16;
-  const size_t smem = sizeof(float2) * (32 * 32 + NW * Ge::kTileF2) + sizeof(uint64_t) * NW;
+  const size_t smem = sizeof(float2) * (32 * 32 + NW * Ge::kTileF2) + sizeof(float) * Ge::kNfft + sizeof(uint64_t) * NW;
   auto kern = stft_pow2_power_kernel<POWER_MODE, G, HG, NW, false>;
   if constexpr (POWER_MODE != kComplexOut)
     if (p.kaldi) kern = stft_pow2_power_kernel<POWER_MODE, G, -1, NW, true>;
@@ -1323,17 +1396,16 @@ template <int POWER_MODE, int G, int HG>
 static int launch_mel(const Pow2Params& p, cudaStream_t stream) {
   using Ge = Geo<G>;
   static_assert(sizeof(MelPlan) % 16 == 0, "fragment array must stay 16-byte aligned");
-  static_assert(Ge::kSlots <= kMaxSlots, "slot tables");
-  const size_t smem = sizeof(float2) * (32 * 32 + kWarps * Ge::kTileF2) + sizeof(float) * 2 * Ge::kSlots * Ge::kPitch +
-                      sizeof(int64_t) * 4 * Ge::kSlots + sizeof(uint64_t) * (kWarps + 4) + sizeof(MelPlan) +
-                      sizeof(float4) * 32 * kFragSmemSteps;
-  if (smem > 227 * 1024) return B200A_EUNSUPPORTED;
+  static_assert(Ge::kSlots <= kMaxSlots && Ge::kMTiles <= kMaxMTiles, "slot tables");
+  static_assert((Ge::kSlots * Ge::kPitch) % 4 == 0, "slot tables and plan stay 16-byte aligned");
+  constexpr size_t smem = mel_smem_bytes<G>();
+  static_assert(smem <= kSmemLimit, "16-warp mel kernel exceeds the shared-memory budget");
   auto kern = p.kaldi ? stft_pow2_mel_kernel<POWER_MODE, G, -1, true> : stft_pow2_mel_kernel<POWER_MODE, G, HG, false>;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess)
     return B200A_ECUDA;
-  const int64_t grid = persistent_grid(p);
+  const int64_t grid = persistent_grid(p, kUniWarps);
   if (grid < 0) return B200A_ECUDA;
-  kern<<<(unsigned)grid, (kWarps + kMelWarps) * 32, smem, stream>>>(p);
+  kern<<<(unsigned)grid, kUniWarps * 32, smem, stream>>>(p);
   return launch_status();
 }
 
@@ -1422,9 +1494,14 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   p.db_amin = d->db_amin;
   p.db_offset = d->db_offset;
   // bulk staging needs 16-byte aligned sources and sizes (every unit starts at a multiple of
-  // frames_per_unit*hop, minus half + pad) and the unit's span must fit the staging buffer
+  // frames_per_unit*hop, minus half + pad) and the unit's span must fit the staging buffer: the warp's mel region,
+  // or the Spectrogram kernel's float2 transpose tile
+  const bool mel = stage >= B200A_STAGE_MEL;
   const int half = d->center ? d->n_fft / 2 : 0;
-  const int stage_floats = 2 * (32 / G) * (32 * (G + 1) + (G == 8 ? 8 : 0));
+  const int stage_floats = !mel    ? 2 * (32 / G) * (32 * (G + 1) + (G == 8 ? 8 : 0))
+                           : G == 8  ? Geo<8>::kMelRegion
+                           : G == 16 ? Geo<16>::kMelRegion
+                                     : Geo<32>::kMelRegion;
   p.bulk_ok = d->hop % 4 == 0 && (half + d->pad) % 4 == 0 && row_stride % 4 == 0 &&
               (reinterpret_cast<uintptr_t>(wave) & 15) == 0 &&
               d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= stage_floats;
@@ -1454,7 +1531,6 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   p.out_vec = (p.out_width % 4 == 0 && p.out_col0 % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0)   ? 4
               : (p.out_width % 2 == 0 && p.out_col0 % 2 == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0) ? 2
                                                                                                               : 1;
-  const bool mel = stage >= B200A_STAGE_MEL;
   if (eo) {
     p.bulk_ok = d->hop % 4 == 0 && (half + d->pad) % 4 == 0 && row_stride % 4 == 0 &&
                 (reinterpret_cast<uintptr_t>(wave) & 15) == 0;
@@ -1495,9 +1571,9 @@ int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float*
     kern<<<grid, kIsWarps * 32, smem, stream>>>(p);
     return launch_status();
   };
-  if (G == 32) return launch(istft_pow2_kernel<32>, sizeof(float2) * (32 * 32 + kIsWarps * Geo<32>::kTileF2));
-  if (G == 16) return launch(istft_pow2_kernel<16>, sizeof(float2) * (32 * 16 + kIsWarps * Geo<16>::kTileF2));
-  return launch(istft_pow2_kernel<8>, sizeof(float2) * (32 * 8 + kIsWarps * Geo<8>::kTileF2));
+  if (G == 32) return launch(istft_pow2_kernel<32>, sizeof(float2) * (32 * 32 + kIsWarps * Geo<32>::kTileF2) + 4 * 1024);
+  if (G == 16) return launch(istft_pow2_kernel<16>, sizeof(float2) * (32 * 16 + kIsWarps * Geo<16>::kTileF2) + 4 * 512);
+  return launch(istft_pow2_kernel<8>, sizeof(float2) * (32 * 8 + kIsWarps * Geo<8>::kTileF2) + 4 * 256);
 }
 
 }  // namespace b200a

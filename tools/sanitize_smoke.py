@@ -1,7 +1,8 @@
 """Small invocations of every kernel family for compute-sanitizer:
     compute-sanitizer --tool memcheck python tools/sanitize_smoke.py
-(racecheck reports the mbarrier-synchronised hand-offs of the warp-specialised kernels as hazards: it does not model
-mbarrier ordering; memcheck and initcheck are the meaningful tools here)."""
+(racecheck reports the mbarrier-synchronised hand-offs as hazards -- the bulk-copy staging of every register-FFT
+kernel and the warp-specialised n_fft = 2048 mel kernel -- because it does not model mbarrier ordering; memcheck and
+initcheck are the meaningful tools here)."""
 import os
 import sys
 
