@@ -1,5 +1,5 @@
-"""``torch.library`` registration of the three hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
-capture tooling see them as ``b200audio::frontend_run`` / ``mfcc_finish`` / ``resample_run``.
+"""``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
+capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``mfcc_finish`` / ``resample_run``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -26,6 +26,10 @@ _LIB = torch.library.Library("b200audio", "DEF")
 _LIB.define(
     "frontend_run(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int stage, int frames, int width, "
     "int row_stride, Tensor(a!)? group_max, int rows_per_group) -> Tensor"
+)
+_LIB.define(
+    "frontend_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int stage, int row_stride, "
+    "Tensor grad_out) -> Tensor"
 )
 _LIB.define(
     "mfcc_finish(Tensor feat, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? group_max, int rows_per_group, "
@@ -80,6 +84,41 @@ def _frontend_run_meta(wave, workspace, desc_i, desc_f, stage, frames, width, ro
     return wave.new_empty(_out_shape(wave, stage, frames, width), dtype=torch.float32)
 
 
+# ---- frontend_backward -------------------------------------------------------------------------------------------
+def _complex_strides(grad_out):
+    """Element strides of a (rows, T, bins, 2) float gradient in complex elements, copying it when the pairs are not
+    adjacent, 8-byte aligned floats."""
+    st = grad_out.stride()
+    if st[3] != 1 or any(s % 2 for s in st[:3]) or grad_out.data_ptr() % 8:
+        grad_out = grad_out.contiguous()
+        st = grad_out.stride()
+    return grad_out, (st[0] // 2, st[1] // 2, st[2] // 2)
+
+
+def _frontend_backward_cuda(wave, workspace, desc_i, desc_f, stage, row_stride, grad_out):
+    d = _unpack_desc(desc_i, desc_f)
+    rows, length = wave.shape
+    dev = wave.device
+    if stage == _lib.STAGE_COMPLEX:
+        grad_out, gs = _complex_strides(grad_out)
+    else:
+        gs = grad_out.stride()
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        grad = torch.empty((rows, length), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_frontend_backward_scratch_bytes(d, stage, rows, length)
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        rc = lib.b200a_frontend_backward(
+            d, workspace.data_ptr(), stage, wave.data_ptr(), rows, length, row_stride, grad_out.data_ptr(), gs[0], gs[1],
+            gs[2], scratch.data_ptr(), grad.data_ptr(), length, _stream(dev))
+    _lib.check(rc, "frontend_backward")
+    return grad
+
+
+def _frontend_backward_meta(wave, workspace, desc_i, desc_f, stage, row_stride, grad_out):
+    return wave.new_empty(wave.shape, dtype=torch.float32)
+
+
 # ---- mfcc_finish -------------------------------------------------------------------------------------------------
 def _mfcc_finish_cuda(feat, workspace, desc_i, desc_f, group_max, rows_per_group, top_db):
     d = _unpack_desc(desc_i, desc_f)
@@ -116,11 +155,13 @@ def _resample_run_meta(wave, workspace, kernel, orig_r, new_r, width, row_stride
 
 
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
+                            ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("mfcc_finish", _mfcc_finish_cuda, _mfcc_finish_meta),
                             ("resample_run", _resample_run_cuda, _resample_run_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
 frontend_run = torch.ops.b200audio.frontend_run
+frontend_backward = torch.ops.b200audio.frontend_backward
 mfcc_finish = torch.ops.b200audio.mfcc_finish
 resample_run = torch.ops.b200audio.resample_run

@@ -5,10 +5,13 @@ memory (``torch.empty``), the current stream, and the device guard.
 """
 from __future__ import annotations
 
+import contextlib
 import math
+import threading
 from typing import Optional, Tuple
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib, _ops
 from ._bookkeeping import resample_len
@@ -26,12 +29,71 @@ def _require_cuda_f32(t: torch.Tensor, what: str) -> None:
         raise TypeError(f"audio_b200: {what} must be float32 (got {t.dtype}); other dtypes are not implemented")
 
 
+_GRAD_STATE = threading.local()
+
+
+def is_differentiable() -> bool:
+    """Whether Spectrogram, MelSpectrogram and F.spectrogram accept inputs that require grad (in this thread)."""
+    return getattr(_GRAD_STATE, "on", False)
+
+
+def set_differentiable(mode: bool) -> None:
+    """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode)."""
+    _GRAD_STATE.on = bool(mode)
+
+
+@contextlib.contextmanager
+def differentiable(mode: bool = True):
+    """Context manager form of :func:`set_differentiable`; restores the previous setting on exit."""
+    prev = is_differentiable()
+    set_differentiable(mode)
+    try:
+        yield
+    finally:
+        set_differentiable(prev)
+
+
 def _no_autograd(t: torch.Tensor) -> None:
     if t.requires_grad and torch.is_grad_enabled():
         raise RuntimeError(
             "audio_b200 kernels are forward-only: the input requires grad. Call under torch.no_grad() / "
-            "torch.inference_mode(), or detach() the input."
+            "torch.inference_mode(), or detach() the input. (Spectrogram, MelSpectrogram and F.spectrogram compute "
+            "waveform gradients inside audio_b200.differentiable().)"
         )
+
+
+def _wants_grad(waveform: torch.Tensor, constants) -> bool:
+    """True when the frontend output must carry a waveform gradient; raises for constant buffers that require grad,
+    whose gradients are not computed."""
+    if not (is_differentiable() and torch.is_grad_enabled()):
+        return False
+    for name, t in constants:
+        if t is not None and t.requires_grad:
+            raise RuntimeError(
+                f"audio_b200: {name} requires grad, but only the waveform gradient is implemented; detach() it "
+                "or register it as a buffer"
+            )
+    return waveform.requires_grad
+
+
+class _FrontendFunction(torch.autograd.Function):
+    """b200audio::frontend_run on the packed (rows, L) waveform, with b200audio::frontend_backward as its backward.
+    The workspace of the forward is kept, so a window or filterbank changed before backward does not change the
+    gradient; the waveform goes through save_for_backward, so in-place edits of it are detected."""
+
+    @staticmethod
+    def forward(ctx, flat, ws, desc_i, desc_f, stage, frames, width, stride):
+        out = _ops.frontend_run(flat, ws, desc_i, desc_f, stage, frames, width, stride, None, 1)
+        ctx.save_for_backward(flat)
+        ctx.ws, ctx.desc_i, ctx.desc_f, ctx.stage, ctx.stride = ws, desc_i, desc_f, stage, stride
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        (flat,) = ctx.saved_tensors
+        grad = _ops.frontend_backward(flat, ctx.ws, ctx.desc_i, ctx.desc_f, ctx.stage, ctx.stride, grad_out)
+        return grad, None, None, None, None, None, None, None
 
 
 def _version_of(t: torch.Tensor) -> int:
@@ -145,10 +207,17 @@ class FrontendPlan:
         waveform: torch.Tensor,
         group_max: Optional[torch.Tensor] = None,
         rows_per_group: int = 1,
+        constants=None,
     ) -> torch.Tensor:
-        """Launch the fused kernel; returns the FRAME-MAJOR result (rows, T, width[, 2])."""
+        """Launch the fused kernel; returns the FRAME-MAJOR result (rows, T, width[, 2]).
+
+        ``constants``: ``(name, tensor)`` pairs of the module buffers the workspace was built from, given by the entry
+        points that support waveform gradients (COMPLEX / POWER / MEL stages); ``None`` keeps the call forward-only.
+        """
         _require_cuda_f32(waveform, "waveform")
-        _no_autograd(waveform)
+        grad = constants is not None and _wants_grad(waveform, constants)
+        if not grad:
+            _no_autograd(waveform)
         if waveform.device != ws.device:
             raise RuntimeError(f"audio_b200: waveform is on {waveform.device} but the module buffers are on {ws.device}")
         lib = _lib.lib()
@@ -166,6 +235,8 @@ class FrontendPlan:
         # through the dispatcher (b200audio::frontend_run, audio_b200/_ops.py): allocates `out`, launches on the
         # current stream of the waveform's device, raises on a negative status
         desc_i, desc_f = self._packed_desc()
+        if grad:
+            return _FrontendFunction.apply(flat, ws, desc_i, desc_f, stage, frames, width, stride)
         return _ops.frontend_run(flat, ws, desc_i, desc_f, stage, frames, width, stride, group_max, rows_per_group)
 
     def mfcc_finish(self, ws, feat, group_max, rows_per_group: int, top_db: Optional[float]) -> torch.Tensor:

@@ -15,6 +15,9 @@ int griffinlim_update_impl(const float*, int64_t, int64_t, int64_t, float, const
                            int64_t, int64_t, int64_t, cudaStream_t);
 int istft_run_impl(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t, float*,
                    float*, int64_t, int64_t, int64_t, cudaStream_t);
+size_t frontend_backward_scratch(const b200a_frontend_desc*, int, int64_t, int64_t);
+int frontend_backward_impl(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
+                           const float*, int64_t, int64_t, int64_t, void*, float*, int64_t, cudaStream_t);
 int frontend_run_pow2(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
                       float*, float*, int64_t, cudaStream_t,
                       const b200a_kaldi_desc* = nullptr);  // returns B200A_EUNSUPPORTED when not applicable
@@ -151,6 +154,49 @@ int b200a_frontend_run(const b200a_frontend_desc* desc, const void* workspace, i
   if (rc != B200A_EUNSUPPORTED) return rc;
   return frontend_run_generic(desc, workspace, stage, wave, rows, length, row_stride, frames, out, group_max,
                               rows_per_group, s);
+}
+
+// Shared checks of the backward entry points; the frame count on success, else a negative status.
+static int64_t backward_frames(const b200a_frontend_desc* desc, int32_t stage, int64_t rows, int64_t length) {
+  int rc = validate_desc(desc);
+  if (rc != B200A_OK) return rc;
+  if (stage < B200A_STAGE_COMPLEX || stage > B200A_STAGE_FEAT) return B200A_EINVAL;
+  if (stage == B200A_STAGE_FEAT) return B200A_EUNSUPPORTED;
+  if (stage == B200A_STAGE_MEL && desc->n_mels <= 0) return B200A_EINVAL;
+  if (stage != B200A_STAGE_COMPLEX && !(desc->power > 0.f)) return B200A_EINVAL;
+  if (rows < 0 || length < 0) return B200A_EINVAL;
+  const int64_t ext = length + 2 * (int64_t)desc->pad;
+  if (desc->center && (desc->pad_mode == B200A_PAD_REFLECT || desc->pad_mode == B200A_PAD_CIRCULAR)) {
+    const int64_t half = desc->n_fft / 2;
+    if (desc->pad_mode == B200A_PAD_REFLECT ? half >= ext : half > ext) return B200A_ESHORT;
+  }
+  const int64_t frames = b200a_num_frames(length, desc->n_fft, desc->hop, desc->center, desc->pad);
+  return frames < 1 ? (int64_t)B200A_ESHORT : frames;
+}
+
+size_t b200a_frontend_backward_scratch_bytes(const b200a_frontend_desc* desc, int32_t stage, int64_t rows, int64_t length) {
+  const int64_t frames = backward_frames(desc, stage, rows, length);
+  if (frames < 1) return 0;
+  return frontend_backward_scratch(desc, stage, rows, frames);
+}
+
+int b200a_frontend_backward(const b200a_frontend_desc* desc, const void* workspace, int32_t stage, const float* wave,
+                            int64_t rows, int64_t length, int64_t row_stride, const float* grad_out, int64_t g_stride_row,
+                            int64_t g_stride_frame, int64_t g_stride_col, void* scratch, float* grad_wave,
+                            int64_t grad_row_stride, b200a_stream stream) {
+  int rc = validate_desc(desc);
+  if (rc != B200A_OK) return rc;
+  if (stage < B200A_STAGE_COMPLEX || stage > B200A_STAGE_FEAT) return B200A_EINVAL;
+  if (stage == B200A_STAGE_FEAT) return B200A_EUNSUPPORTED;
+  if (rows == 0) return B200A_OK;  // empty batch: nothing to enqueue (pointers may be null)
+  if (workspace == nullptr || wave == nullptr || grad_out == nullptr || scratch == nullptr || grad_wave == nullptr)
+    return B200A_EINVAL;
+  if (rows < 0 || length < 0 || row_stride < length || grad_row_stride < length) return B200A_EINVAL;
+  const int64_t frames = backward_frames(desc, stage, rows, length);
+  if (frames < 1) return (int)frames;
+  return frontend_backward_impl(desc, workspace, stage, wave, rows, length, row_stride, frames, grad_out, g_stride_row,
+                                g_stride_frame, g_stride_col, scratch, grad_wave, grad_row_stride,
+                                static_cast<cudaStream_t>(stream));
 }
 
 int b200a_mfcc_finish(const b200a_frontend_desc* desc, const void* workspace, const float* feat, int64_t rows,

@@ -83,6 +83,16 @@ __device__ __forceinline__ int64_t source_index(int64_t i, int64_t length, int p
   return (s >= 0 && s < length) ? s : -1;
 }
 
+// dL/dX of |X|^p for the upstream value s, as torch differentiates abs().pow(p): p |X|^(p-2) X s.  At X = 0 it is 0 for
+// p >= 1 and NaN for p < 1 (0^(p-1) = inf times sgn(0) = 0).
+__device__ __forceinline__ float2 power_vjp(float re, float im, float p, float s) {
+  if (p == 2.f) return make_float2(2.f * re * s, 2.f * im * s);
+  const float mag = hypotf(re, im);
+  if (mag == 0.f) return p < 1.f ? make_float2(CUDART_NAN_F, CUDART_NAN_F) : make_float2(0.f, 0.f);
+  const float c = (p == 1.f ? s : p * powf(mag, p - 1.f) * s) / mag;
+  return make_float2(re * c, im * c);
+}
+
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {
   // total order trick: non-negative floats compare like ints, negative like reversed uints
   if (v >= 0.f) {

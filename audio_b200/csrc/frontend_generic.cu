@@ -828,9 +828,13 @@ __global__ void __launch_bounds__(256) istft_ola_kernel(const float* __restrict_
 int istft_frames_pow2(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t, float*,
                       cudaStream_t);  // frontend_pow2.cu; B200A_EUNSUPPORTED when the size is not 256 / 512 / 1024
 
-int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
-                   int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, float* out,
-                   int64_t out_row_stride, int64_t start, int64_t out_len, cudaStream_t stream) {
+// First half of b200a_istft_run: the windowed time frames w * irfft(spec) / scale of every frame into frame_buf, on the
+// register FFT for n_fft = 256 / 512 / 1024 (onesided descriptors) and the shared-memory Stockham FFT otherwise.  Any
+// n_fft works, odd ones included (bins (N+1)/2 .. N-1 are the Hermitian mirror of 1 .. (N-1)/2): torch.istft's
+// even-size rule is checked by b200a_istft_run, not needed here.
+static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
+                             int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf,
+                             cudaStream_t stream) {
   const WsLayout l = ws_layout(*d);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   IstftParams p{};
@@ -856,17 +860,241 @@ int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* sp
   if (cudaFuncSetAttribute(istft_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
     return B200A_ECUDA;
   const int64_t grid = rows * p.tiles_per_row;
-  if (grid <= 0 || grid > 0x7fffffffLL || rows > 65535) return B200A_EUNSUPPORTED;
+  if (grid <= 0 || grid > 0x7fffffffLL) return B200A_EUNSUPPORTED;
   int rc = istft_frames_pow2(d, ws, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, stream);
   if (rc == B200A_EUNSUPPORTED) {  // any other size: shared-memory Stockham
     istft_frames_kernel<<<(unsigned)grid, 256, smem, stream>>>(p);
     rc = launch_status();
   }
+  return rc;
+}
+
+int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
+                   int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, float* out,
+                   int64_t out_row_stride, int64_t start, int64_t out_len, cudaStream_t stream) {
+  if (rows > 65535) return B200A_EUNSUPPORTED;  // the overlap-add grid keeps rows in blockIdx.y
+  int rc = istft_frames_impl(d, ws, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, stream);
   if (rc != B200A_OK) return rc;
+  const float* window = reinterpret_cast<const float*>(static_cast<const unsigned char*>(ws) + ws_layout(*d).window);
   const int64_t blocks = (out_len + 255) / 256;
   if (blocks > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  istft_ola_kernel<<<dim3((unsigned)blocks, (unsigned)rows), 256, 0, stream>>>(frame_buf, p.window, d->n_fft, d->hop, frames,
+  istft_ola_kernel<<<dim3((unsigned)blocks, (unsigned)rows), 256, 0, stream>>>(frame_buf, window, d->n_fft, d->hop, frames,
                                                                                start, out_len, out, out_row_stride);
+  return launch_status();
+}
+
+// ------------------------------------------------------------------------------------------
+// waveform gradient (b200a_frontend_backward)
+//   X = scale * DFT(w * frame);  G = dL/dX per output bin;  H_k = (G_k + conj G_{N-k}) / 2 (G = 0 outside the output
+//   bins);  dframe = scale * w * N * irfft(H);  overlap-add dframe and fold the padding back onto the source samples.
+// ------------------------------------------------------------------------------------------
+struct SpecVjpParams {
+  float2* spec;  // [rows][frames][n_bins]: the forward spectrum in, H * N * scale^2 out at bins 0 .. N/2
+  const float* grad;
+  int64_t gs_row, gs_frame, gs_col;  // element strides of grad (complex elements for COMPLEX)
+  int* bad;                          // [rows][frames]: 1 where the frame's gradient is NaN
+  const float* fb;                   // [n_bins][n_mels]
+  const int2* bands;                 // [n_mels] non-zero bin range of each filter
+  const WsHeader* hdr;
+  int64_t frames, total;  // total = rows * frames
+  int n_fft, n_bins, n_mels, stage;
+  float power;
+};
+
+// G at bin j of one frame (j < n_bins): the upstream value for COMPLEX, else the power VJP with s_j = g_j or sum_m fb g_m
+__device__ __forceinline__ float2 spec_grad_at(const SpecVjpParams& p, const float2* __restrict__ x, const float* __restrict__ g,
+                                               const int2* s_range, int j) {
+  if (p.stage == B200A_STAGE_COMPLEX) return reinterpret_cast<const float2*>(g)[j * p.gs_col];
+  float s;
+  if (p.stage == B200A_STAGE_MEL) {
+    const int2 r = s_range[j];
+    s = 0.f;
+    for (int m = r.x; m < r.y; ++m) s = fmaf(p.fb[(size_t)j * p.n_mels + m], g[m * p.gs_col], s);
+  } else {
+    s = g[j * p.gs_col];
+  }
+  const float2 v = x[j];
+  return power_vjp(v.x, v.y, p.power, s);
+}
+
+// One warp per frame, grid-stride over the frames of every row.  A lane writes bin k <= N/2 after reading bins k and N-k:
+// no other lane writes N-k (> N/2 unless it is k itself), so the spectrum is overwritten in place.
+__global__ void __launch_bounds__(256) spec_vjp_kernel(const SpecVjpParams p) {
+  extern __shared__ int2 s_range[];  // MEL: filters [x, y) with a non-zero weight at each bin
+  if (p.stage == B200A_STAGE_MEL) {
+    for (int k = threadIdx.x; k < p.n_bins; k += blockDim.x) {
+      int lo = p.n_mels, hi = 0;
+      for (int m = 0; m < p.n_mels; ++m) {
+        const int2 b = p.bands[m];
+        if (b.x <= k && k < b.y) {
+          lo = min(lo, m);
+          hi = m + 1;
+        }
+      }
+      s_range[k] = hi > lo ? make_int2(lo, hi) : make_int2(0, 0);
+    }
+    __syncthreads();
+  }
+  const int lane = threadIdx.x & 31, N = p.n_fft, half_n = N / 2;
+  const float gain = (float)N * p.hdr->scale * p.hdr->scale;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t f = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); f < p.total; f += warps) {
+    const int64_t row = f / p.frames, t = f - row * p.frames;
+    float2* x = p.spec + f * p.n_bins;
+    const float* g = p.grad + row * p.gs_row * (p.stage == B200A_STAGE_COMPLEX ? 2 : 1) +
+                     t * p.gs_frame * (p.stage == B200A_STAGE_COMPLEX ? 2 : 1);
+    bool nan = false;
+    for (int k = lane; k <= half_n; k += 32) {
+      const int km = k == 0 ? 0 : N - k;
+      const float2 gk = spec_grad_at(p, x, g, s_range, k);
+      float2 h;
+      if (km == k) {
+        h = make_float2(gk.x, 0.f);
+      } else {
+        h = make_float2(0.5f * gk.x, 0.5f * gk.y);
+        if (km < p.n_bins) {
+          const float2 gm = spec_grad_at(p, x, g, s_range, km);
+          h = make_float2(h.x + 0.5f * gm.x, h.y - 0.5f * gm.y);
+        }
+      }
+      h = make_float2(h.x * gain, h.y * gain);
+      nan |= isnan(h.x) || isnan(h.y);
+      x[k] = h;
+    }
+    // a NaN bin makes every sample of this frame's gradient NaN, as in torch; zero the spectrum so the frame it is
+    // transformed with (two frames share one complex FFT) stays clean, and let the fold write the NaN
+    const bool bad = __any_sync(0xffffffffu, nan);
+    if (bad)
+      for (int k = lane; k <= half_n; k += 32) x[k] = make_float2(0.f, 0.f);
+    if (lane == 0) p.bad[f] = bad ? 1 : 0;
+  }
+}
+
+// Gradient of the source samples: output-stationary, one thread per sample of one row.  Each padded position i the
+// sample was copied to (itself, its reflect / circular images, or the replicated edge runs) receives sum_t dframe[t][i -
+// t hop]; positions in ascending order, frames in ascending t, no atomics, so the result is reproducible bit for bit
+// and independent of the other rows.  Samples no frame covers get 0.  bad (may be null): frames whose gradient is NaN.
+__global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict__ frame_buf, const int* __restrict__ bad,
+                                                         int n_fft, int hop, int64_t frames, int64_t length, int pad,
+                                                         int half, int pad_mode, int64_t blocks_per_row,
+                                                         float* __restrict__ grad, int64_t grad_row_stride) {
+  const int64_t row = blockIdx.x / blocks_per_row;
+  const int64_t s = (blockIdx.x - row * blocks_per_row) * (int64_t)blockDim.x + threadIdx.x;
+  if (s >= length) return;
+  const float* fb = frame_buf + row * frames * n_fft;
+  const int* fl = bad == nullptr ? nullptr : bad + row * frames;
+  auto at = [&](int64_t i, float acc) {
+    const int64_t t_lo = i - n_fft + 1 <= 0 ? 0 : (i - n_fft + hop) / hop;  // ceil((i - n_fft + 1) / hop)
+    int64_t t_hi = i / hop;
+    if (t_hi > frames - 1) t_hi = frames - 1;
+    for (int64_t t = t_lo; t <= t_hi; ++t) {
+      const float v = fb[t * n_fft + (i - t * hop)];
+      acc += (fl != nullptr && fl[t]) ? CUDART_NAN_F : v;
+    }
+    return acc;
+  };
+  const int64_t ext = length + 2 * (int64_t)pad, j = s + pad;  // j: index in the constant pre-padded signal
+  float acc = 0.f;
+  if (half == 0 || pad_mode == B200A_PAD_CONSTANT) {
+    acc = at(half + j, acc);
+  } else if (pad_mode == B200A_PAD_REFLECT) {
+    if (j >= 1 && j <= half) acc = at(half - j, acc);
+    acc = at(half + j, acc);
+    if (j <= ext - 2 && j > ext - 2 - half) acc = at(half + 2 * (ext - 1) - j, acc);
+  } else if (pad_mode == B200A_PAD_REPLICATE) {
+    if (j == 0)
+      for (int64_t i = 0; i < half; ++i) acc = at(i, acc);
+    acc = at(half + j, acc);
+    if (j == ext - 1)
+      for (int64_t i = half + ext; i < ext + 2 * (int64_t)half; ++i) acc = at(i, acc);
+  } else {  // circular (half <= ext)
+    if (j >= ext - half) acc = at(half + j - ext, acc);
+    acc = at(half + j, acc);
+    if (j < half) acc = at(half + j + ext, acc);
+  }
+  grad[row * grad_row_stride + s] = acc;
+}
+
+// frontend_pow2.cu
+int frontend_run_pow2(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t, float*,
+                      float*, int64_t, cudaStream_t, const b200a_kaldi_desc*);
+bool backward_fused_applicable(const b200a_frontend_desc* d, int stage);
+int frontend_backward_pow2(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
+                           const float*, int64_t, int64_t, int64_t, float*, cudaStream_t);
+
+size_t frontend_backward_scratch(const b200a_frontend_desc* d, int stage, int64_t rows, int64_t frames) {
+  const size_t n = (size_t)rows * (size_t)frames;
+  const size_t frame_bytes = align_up(sizeof(float) * n * d->n_fft, 256);
+  if (backward_fused_applicable(d, stage)) return frame_bytes;
+  const size_t n_bins = d->onesided ? d->n_fft / 2 + 1 : d->n_fft;
+  return align_up(sizeof(float2) * n * n_bins, 256) + frame_bytes + align_up(sizeof(int) * n, 256);
+}
+
+int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                           int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
+                           int64_t gs_frame, int64_t gs_col, void* scratch, float* grad_wave, int64_t grad_row_stride,
+                           cudaStream_t stream) {
+  const WsLayout l = ws_layout(*d);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const int64_t n = rows * frames;
+  unsigned char* sc = static_cast<unsigned char*>(scratch);
+  float* frame_buf;
+  int* bad = nullptr;
+  int rc;
+  if (backward_fused_applicable(d, stage)) {
+    frame_buf = reinterpret_cast<float*>(sc);
+    rc = frontend_backward_pow2(d, ws, stage, wave, rows, length, row_stride, frames, grad, gs_row, gs_frame, gs_col, frame_buf,
+                                stream);
+  } else {
+    // composition: forward complex spectrum -> H * N * scale^2 in place -> the iSTFT frame stage -> fold
+    const int n_bins = d->onesided ? d->n_fft / 2 + 1 : d->n_fft;
+    float2* spec = reinterpret_cast<float2*>(sc);
+    frame_buf = reinterpret_cast<float*>(sc + align_up(sizeof(float2) * (size_t)n * n_bins, 256));
+    bad = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(frame_buf) + align_up(sizeof(float) * (size_t)n * d->n_fft, 256));
+    float* spec_f = reinterpret_cast<float*>(spec);
+    rc = frontend_run_pow2(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames, spec_f, nullptr, 1, stream,
+                           nullptr);
+    if (rc == B200A_EUNSUPPORTED)
+      rc = frontend_run_generic(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames, spec_f, nullptr, 1, stream,
+                                nullptr);
+    if (rc != B200A_OK) return rc;
+    SpecVjpParams p{};
+    p.spec = spec;
+    p.grad = grad;
+    p.gs_row = gs_row;
+    p.gs_frame = gs_frame;
+    p.gs_col = gs_col;
+    p.bad = bad;
+    p.fb = reinterpret_cast<const float*>(base + l.fb);
+    p.bands = reinterpret_cast<const int2*>(base + l.bands);
+    p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+    p.frames = frames;
+    p.total = n;
+    p.n_fft = d->n_fft;
+    p.n_bins = n_bins;
+    p.n_mels = d->n_mels;
+    p.stage = stage;
+    p.power = d->power;
+    const int sms = device_sm_count();
+    if (sms < 0) return B200A_ECUDA;
+    const int64_t want = (n + 7) / 8;
+    const unsigned grid = (unsigned)(want < 8 * (int64_t)sms ? want : 8 * (int64_t)sms);
+    const size_t smem = stage == B200A_STAGE_MEL ? sizeof(int2) * n_bins : 0;
+    if (smem > 48 * 1024 &&
+        cudaFuncSetAttribute(spec_vjp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+      return B200A_ECUDA;
+    spec_vjp_kernel<<<grid, 256, smem, stream>>>(p);
+    rc = launch_status();
+    if (rc != B200A_OK) return rc;
+    rc = istft_frames_impl(d, ws, spec_f, rows, frames, frames * n_bins, 1, n_bins, frame_buf, stream);
+  }
+  if (rc != B200A_OK) return rc;
+  const int64_t bpr = (length + 255) / 256;
+  if (bpr == 0) return B200A_OK;
+  if (rows * bpr > 0x7fffffffLL) return B200A_EUNSUPPORTED;
+  frame_fold_kernel<<<(unsigned)(rows * bpr), 256, 0, stream>>>(frame_buf, bad, d->n_fft, d->hop, frames, length, d->pad,
+                                                                d->center ? d->n_fft / 2 : 0, d->pad_mode, bpr, grad_wave,
+                                                                grad_row_stride);
   return launch_status();
 }
 

@@ -223,6 +223,7 @@ __device__ __forceinline__ int frame_lead(const Pow2Params& p, int n_fft) {
 }
 
 constexpr int kComplexOut = 3;  // POWER_MODE of the complex (power = None) Spectrogram kernel
+constexpr int kSpectra = 4;     // POWER_MODE of the gradient kernel: transform_unit returns the two complex spectra
 
 template <int POWER_MODE>  // 2: |.|^2, 0: general exponent (1 handled inside)
 __device__ __forceinline__ float pow_of(float re, float im, float power) {
@@ -324,11 +325,12 @@ __device__ __forceinline__ void issue_bulk(const Pow2Params& p, int half, int64_
 // pass 2 has read the tile back.  s_win: the window x 1/2 (un-packing) x the normalisation scale, [n_fft].
 // SPLIT: transpose the real parts, then the imaginary parts, through kRegionF floats per lane group (half the
 // shared memory of the float2 transpose, kRegion float2 per lane group).
-template <int POWER_MODE, int G, int HG, bool KALDI, bool SPLIT>
+// POWER_MODE == kSpectra: PT = float2, pa / pb receive the complex bins themselves (bin N/2 with a zero imaginary part).
+template <int POWER_MODE, int G, int HG, bool KALDI, bool SPLIT, typename PT>
 __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float* s_win, const float2* s_tw,
                                                float2* tile, uint64_t* bar, uint32_t& parity, bool& staged,
-                                               const UnitCursor& cur, int half, int lane, float (&pa)[17],
-                                               float (&pb)[17]) {
+                                               const UnitCursor& cur, int half, int lane, PT (&pa)[17],
+                                               PT (&pb)[17]) {
   using Ge = Geo<G>;
   float* stage = reinterpret_cast<float*>(tile);
   const int gi = lane / G, l = lane % G;
@@ -580,6 +582,9 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       float2* oc = reinterpret_cast<float2*>(p.out) + (row * p.frames + ta) * Ge::kBins + l + G * m;
       if (has_a) oc[0] = make_float2(sx.x, sy.x);
       if (has_b) oc[Ge::kBins] = make_float2(sy.y, -sx.y);
+    } else if constexpr (POWER_MODE == kSpectra) {
+      pa[m] = make_float2(sx.x, sy.x);
+      pb[m] = make_float2(sy.y, -sx.y);
     } else if constexpr (POWER_MODE == 2) {  // (|A|^2, |B|^2) as one packed multiply + one packed FMA
       const float2 pw = fma2(sx, sx, mul2(sy, sy));
       pa[m] = pw.x;
@@ -597,6 +602,9 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       if (has_a) oc[0] = make_float2(2.f * a[slot16].x, 0.f);
       if (has_b) oc[Ge::kBins] = make_float2(2.f * a[slot16].y, 0.f);
     }
+  } else if constexpr (POWER_MODE == kSpectra) {
+    pa[16] = make_float2(2.f * a[slot16].x, 0.f);
+    pb[16] = make_float2(2.f * a[slot16].y, 0.f);
   } else {
     pa[16] = pow_of<POWER_MODE>(2.f * a[slot16].x, 0.f, p.power);
     pb[16] = pow_of<POWER_MODE>(2.f * a[slot16].y, 0.f, p.power);
@@ -1241,6 +1249,182 @@ __global__ void __launch_bounds__(kIsWarps * 32, 1) istft_pow2_kernel(const Istf
   }
 }
 
+// ================================================================================================
+// Waveform gradient on the register FFT (n_fft = 256 / 512 / 1024), the first half of b200a_frontend_backward.
+// Per unit a warp recomputes the forward transform from the waveform (transform_unit, the spectra kept complex), forms
+// the per-bin gradient G (upstream value, or p |X|^(p-2) X s with s = g or sum_m fb[k][m] g_m) and its Hermitian part
+// H_k = (G_k + conj G_{N-k}) / 2 in registers, fetches the mirrored half of H with one shuffle per value as the forward
+// un-packing does, and runs the inverse passes of istft_pow2_kernel.  The frame gradients scale * w * N * irfft(H) go
+// to frame_buf; X never leaves the registers.  Units are loaded without the bulk prefetch, so the transpose tile is
+// free for the inverse passes.  A frame with a NaN bin gets NaN everywhere (torch's p < 1 gradient at X = 0).
+// ================================================================================================
+constexpr int kBwWarps = 16;
+
+struct BwdParams {
+  Pow2Params f;      // the forward geometry (bulk_ok = 0)
+  const float* grad;  // upstream gradient, element strides (complex elements for COMPLEX)
+  int64_t gs_row, gs_frame, gs_col;
+  float* frame_buf;  // [rows][frames][n_fft]
+  const float* fb;   // [n_bins][n_mels]
+  const int2* bands;  // [n_mels]
+  int stage;
+};
+
+template <int G>
+constexpr size_t bwd_smem_fixed() {  // twiddles, window, transpose tiles, per-bin filter ranges
+  return sizeof(float2) * (32 * G + kBwWarps * Geo<G>::kTileF2) + sizeof(float) * Geo<G>::kNfft + sizeof(int2) * Geo<G>::kBins;
+}
+
+template <int G, int STAGE>
+__global__ void __launch_bounds__(kBwWarps * 32, 1) stft_pow2_backward_kernel(const BwdParams bp) {
+  using Ge = Geo<G>;
+  constexpr int N = Ge::kNfft, NG = Ge::kGroups;
+  const Pow2Params& p = bp.f;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  float2* s_tw = reinterpret_cast<float2*>(smem_raw);                    // [32][G]
+  float2* s_tile_all = s_tw + 32 * G;                                     // [kBwWarps][kTileF2]
+  float* s_win = reinterpret_cast<float*>(s_tile_all + kBwWarps * Ge::kTileF2);  // [N] window x 1/2 x scale
+  int2* s_range = reinterpret_cast<int2*>(s_win + N);                     // [bins] MEL: filters non-zero at the bin
+  float* s_g_all = reinterpret_cast<float*>(s_range + Ge::kBins);        // [kBwWarps][kFrames][n_mels] MEL
+
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
+  load_window(p, s_win, N, tid, blockDim.x);
+  const int n_mels = p.n_mels;
+  if constexpr (STAGE == B200A_STAGE_MEL) {
+    for (int k = tid; k < Ge::kBins; k += blockDim.x) {
+      int lo = n_mels, hi = 0;
+      for (int m = 0; m < n_mels; ++m) {
+        const int2 b = bp.bands[m];
+        if (b.x <= k && k < b.y) {
+          lo = min(lo, m);
+          hi = m + 1;
+        }
+      }
+      s_range[k] = hi > lo ? make_int2(lo, hi) : make_int2(0, 0);
+    }
+  }
+  __syncthreads();
+
+  float2* tile = s_tile_all + warp * Ge::kTileF2;
+  float2* grp_tile = tile + (lane / G) * Ge::kRegion;
+  float* s_g = s_g_all + (size_t)warp * Ge::kFrames * n_mels;
+  const int half = frame_lead(p, N);
+  const int gi = lane / G, l = lane % G;
+  const unsigned gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (gi * G);
+  uint32_t parity = 0;
+  bool staged = false;
+  UnitCursor cur;
+  cur.init((int64_t)blockIdx.x * kBwWarps + warp, (int64_t)gridDim.x * kBwWarps, p.units_per_row);
+  for (; cur.u < p.total_units; cur.advance()) {
+    float2 xa[17], xb[17];
+    transform_unit<kSpectra, G, -1, false, false>(p, s_win, s_tw, tile, nullptr, parity, staged, cur, half, lane, xa, xb);
+    const int64_t t0 = cur.ub * Ge::kFrames, ta = t0 + 2 * gi, tb = ta + 1;
+    const bool has_a = ta < p.frames, has_b = tb < p.frames;
+    const float* ga = bp.grad + (cur.row * bp.gs_row + ta * bp.gs_frame) * (STAGE == B200A_STAGE_COMPLEX ? 2 : 1);
+    const float* gb = ga + bp.gs_frame * (STAGE == B200A_STAGE_COMPLEX ? 2 : 1);
+    if constexpr (STAGE == B200A_STAGE_MEL) {  // the unit's upstream rows, [kFrames][n_mels]
+      for (int i = lane; i < Ge::kFrames * n_mels; i += 32) {
+        const int f = i / n_mels, m = i - f * n_mels;
+        s_g[i] = t0 + f < p.frames ? bp.grad[cur.row * bp.gs_row + (t0 + f) * bp.gs_frame + m * bp.gs_col] : 0.f;
+      }
+      __syncwarp();
+    }
+    // ---- G -> H for bins k = l + G m (m < 16) and, on l == 0, k = N/2 (m = 16) ----
+    bool nan_a = false, nan_b = false;
+    static_for<17>([&](auto mi) {
+      constexpr int m = decltype(mi)::value;
+      const int k = m < 16 ? l + G * m : N / 2;
+      float2 da = make_float2(0.f, 0.f), db = da;
+      if (m < 16 || l == 0) {
+        if constexpr (STAGE == B200A_STAGE_COMPLEX) {
+          if (has_a) da = reinterpret_cast<const float2*>(ga)[k * bp.gs_col];
+          if (has_b) db = reinterpret_cast<const float2*>(gb)[k * bp.gs_col];
+        } else {
+          float sa = 0.f, sb = 0.f;
+          if constexpr (STAGE == B200A_STAGE_MEL) {
+            const int2 r = s_range[k];
+            const float* ra = s_g + 2 * gi * n_mels;
+            for (int q = r.x; q < r.y; ++q) {
+              const float w = __ldg(bp.fb + (size_t)k * n_mels + q);
+              sa = fmaf(w, ra[q], sa);
+              sb = fmaf(w, ra[n_mels + q], sb);
+            }
+          } else {
+            if (has_a) sa = ga[k * bp.gs_col];
+            if (has_b) sb = gb[k * bp.gs_col];
+          }
+          if (has_a) da = power_vjp(xa[m].x, xa[m].y, p.power, sa);
+          if (has_b) db = power_vjp(xb[m].x, xb[m].y, p.power, sb);
+        }
+      }
+      // H = G / 2 inside, Re G at bins 0 and N/2 (the scale is applied with the window at the end)
+      const bool edge = k == 0 || m == 16;
+      xa[m] = edge ? make_float2(da.x, 0.f) : make_float2(0.5f * da.x, 0.5f * da.y);
+      xb[m] = edge ? make_float2(db.x, 0.f) : make_float2(0.5f * db.x, 0.5f * db.y);
+      nan_a |= isnan(xa[m].x) || isnan(xa[m].y);
+      nan_b |= isnan(xb[m].x) || isnan(xb[m].y);
+    });
+    const bool bad_a = (__ballot_sync(0xffffffffu, nan_a) & gmask) != 0;
+    const bool bad_b = (__ballot_sync(0xffffffffu, nan_b) & gmask) != 0;
+    if (bad_a || bad_b) {  // keep the frame it shares the complex transform with clean
+      static_for<17>([&](auto mi) {
+        constexpr int m = decltype(mi)::value;
+        if (bad_a) xa[m] = make_float2(0.f, 0.f);
+        if (bad_b) xb[m] = make_float2(0.f, 0.f);
+      });
+    }
+    // ---- conj(Z[n]), Z = Ha + i Hb, n = l + G j: j < 16 own bins, j >= 16 the conjugate of bin N - n ----
+    float2 a[32];
+    const int src = (lane & ~(G - 1)) | ((G - l) & (G - 1));
+    static_for<32>([&](auto ji) {
+      constexpr int j = decltype(ji)::value;
+      float2 ha, hb;
+      if constexpr (j < 16) {
+        ha = xa[j];
+        hb = xb[j];
+      } else {
+        // l >= 1: N - n = (G - l) + G (31 - j) on lane src;  l == 0: N - n = G (32 - j), own bin m = 32 - j
+        constexpr int mm = 31 - j, m0 = 32 - j;
+        float4 v = make_float4(__shfl_sync(0xffffffffu, xa[mm].x, src), __shfl_sync(0xffffffffu, xa[mm].y, src),
+                               __shfl_sync(0xffffffffu, xb[mm].x, src), __shfl_sync(0xffffffffu, xb[mm].y, src));
+        if (l == 0) v = make_float4(xa[m0].x, xa[m0].y, xb[m0].x, xb[m0].y);
+        ha = make_float2(v.x, -v.y);
+        hb = make_float2(v.z, -v.w);
+        if (j == 16 && l == 0) {  // bin N/2 itself (real)
+          ha = xa[16];
+          hb = xb[16];
+        }
+      }
+      a[brev5(j)] = make_float2(ha.x - hb.y, -(ha.y + hb.x));
+    });
+    // ---- inverse passes (istft_pow2_kernel) ----
+    fft_regs<32, 0>(a);
+    grp_tile[l] = a[0];
+    static_for<31>([&](auto ki) {
+      constexpr int k2 = decltype(ki)::value + 1;
+      grp_tile[k2 * Ge::kRowLd + l] = cmul2(a[k2], s_tw[k2 * G + l]);
+    });
+    __syncwarp();
+    static_for<32>([&](auto si) {
+      constexpr int s = decltype(si)::value;
+      constexpr int q = s / G, g = s % G;
+      a[q * G + brev<Ge::kLogG>(g)] = grp_tile[(l + G * q) * Ge::kRowLd + g];
+    });
+    __syncwarp();
+    static_for<NG>([&](auto qi) { fft_regs<G, decltype(qi)::value * G>(a); });
+    // a[(m % NG) G + m / NG] = FFT(conj Z)[l + G m] = N (a[n] - i b[n]);  dframe = scale * w * N * irfft(H)
+    float* fa = bp.frame_buf + (cur.row * p.frames + ta) * N + l;
+    static_for<32>([&](auto mi) {
+      constexpr int m = decltype(mi)::value;
+      constexpr int slot = (m % NG) * G + m / NG;
+      const float w = 2.f * s_win[l + G * m];  // window x scale
+      if (has_a) fa[G * m] = bad_a ? CUDART_NAN_F : a[slot].x * w;
+      if (has_b) fa[N + G * m] = bad_b ? CUDART_NAN_F : -a[slot].y * w;
+    });
+  }
+}
+
 // ---- table preparation ------------------------------------------------------------------------
 __global__ void prepare_tw2d_kernel(float2* tw2d, int G) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;  // i = k2 * G + g
@@ -1574,6 +1758,81 @@ int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float*
   if (G == 32) return launch(istft_pow2_kernel<32>, sizeof(float2) * (32 * 32 + kIsWarps * Geo<32>::kTileF2) + 4 * 1024);
   if (G == 16) return launch(istft_pow2_kernel<16>, sizeof(float2) * (32 * 16 + kIsWarps * Geo<16>::kTileF2) + 4 * 512);
   return launch(istft_pow2_kernel<8>, sizeof(float2) * (32 * 8 + kIsWarps * Geo<8>::kTileF2) + 4 * 256);
+}
+
+// Shared memory of the fused gradient kernel, 0 when the descriptor / stage does not take it.
+static size_t backward_smem(const b200a_frontend_desc* d, int stage) {
+  if (!pow2_applicable(*d) || d->n_fft > 1024) return 0;
+  if (stage != B200A_STAGE_COMPLEX && stage != B200A_STAGE_POWER && stage != B200A_STAGE_MEL) return 0;
+  const int G = d->n_fft / 32;
+  const size_t fixed = G == 32 ? bwd_smem_fixed<32>() : G == 16 ? bwd_smem_fixed<16>() : bwd_smem_fixed<8>();
+  const size_t g_rows = stage == B200A_STAGE_MEL ? sizeof(float) * kBwWarps * 2 * (32 / G) * (size_t)d->n_mels : 0;
+  return fixed + g_rows <= (size_t)kSmemLimit ? fixed + g_rows : 0;
+}
+
+bool backward_fused_applicable(const b200a_frontend_desc* d, int stage) { return backward_smem(d, stage) != 0; }
+
+// First half of b200a_frontend_backward for n_fft = 256 / 512 / 1024: frame gradients into frame_buf.
+int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                           int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
+                           int64_t gs_frame, int64_t gs_col, float* frame_buf, cudaStream_t stream) {
+  const size_t smem = backward_smem(d, stage);
+  if (smem == 0) return B200A_EUNSUPPORTED;
+  const WsLayout l = ws_layout(*d);
+  const Pow2Extra e = pow2_layout(*d, l.total);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const int G = d->n_fft / 32;
+  const int frames_per_unit = 2 * (32 / G);
+  BwdParams bp{};
+  Pow2Params& p = bp.f;
+  p.wave = wave;
+  p.length = length;
+  p.row_stride = row_stride;
+  p.frames = frames;
+  p.units_per_row = (frames + frames_per_unit - 1) / frames_per_unit;
+  p.total_units = rows * p.units_per_row;
+  p.window = reinterpret_cast<const float*>(base + l.window);
+  p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
+  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.hop = d->hop;
+  p.pad = d->pad;
+  p.center = d->center;
+  p.pad_mode = d->pad_mode;
+  p.n_mels = stage == B200A_STAGE_MEL ? d->n_mels : 0;
+  p.stage = stage;
+  p.power = d->power;
+  p.bulk_ok = 0;  // the transpose tile doubles as the inverse passes' tile, so nothing is staged into it ahead
+  // edge units gather their span into the tile (the Spectrogram kernel's float2 transpose tile) with 32-bit indices
+  const int stage_floats = 2 * (32 / G) * (32 * (G + 1) + (G == 8 ? 8 : 0));
+  p.stage_ok = d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= stage_floats &&
+               length + 2 * (int64_t)d->pad + d->n_fft < (int64_t)1 << 31;
+  bp.grad = grad;
+  bp.gs_row = gs_row;
+  bp.gs_frame = gs_frame;
+  bp.gs_col = gs_col;
+  bp.frame_buf = frame_buf;
+  bp.fb = reinterpret_cast<const float*>(base + l.fb);
+  bp.bands = reinterpret_cast<const int2*>(base + l.bands);
+  bp.stage = stage;
+  const int sms = num_sms();
+  if (sms < 0) return B200A_ECUDA;
+  const int64_t iters = (p.total_units + kBwWarps - 1) / kBwWarps;
+  const unsigned grid = (unsigned)(iters < sms ? (iters < 1 ? 1 : iters) : sms);
+  auto launch = [&](auto kern) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess)
+      return (int)B200A_ECUDA;
+    kern<<<grid, kBwWarps * 32, smem, stream>>>(bp);
+    return launch_status();
+  };
+  auto by_stage = [&](auto g) {
+    constexpr int GG = decltype(g)::value;
+    if (stage == B200A_STAGE_COMPLEX) return launch(stft_pow2_backward_kernel<GG, B200A_STAGE_COMPLEX>);
+    if (stage == B200A_STAGE_POWER) return launch(stft_pow2_backward_kernel<GG, B200A_STAGE_POWER>);
+    return launch(stft_pow2_backward_kernel<GG, B200A_STAGE_MEL>);
+  };
+  if (G == 32) return by_stage(std::integral_constant<int, 32>{});
+  if (G == 16) return by_stage(std::integral_constant<int, 16>{});
+  return by_stage(std::integral_constant<int, 8>{});
 }
 
 }  // namespace b200a

@@ -7,7 +7,8 @@ Same names, argument order, defaults and error behaviour as the reference
 private helpers ``transforms`` imports (``_get_sinc_resample_kernel`` 1305-1402,
 ``_apply_sinc_resample_kernel`` 1405-1432).
 
-Differences, all explicit (never a silent fallback): CUDA float32 tensors only, forward only.
+Differences, all explicit (never a silent fallback): CUDA float32 tensors only, forward only except the waveform
+gradient of ``spectrogram`` (and of the MelSpectrogram path) inside ``audio_b200.differentiable()``.
 """
 from __future__ import annotations
 
@@ -102,7 +103,7 @@ def spectrogram(
     plan = _plan_for(desc, waveform.device)
     ws = plan.workspace(window, None, None)
     stage = _lib.STAGE_COMPLEX if power is None else _lib.STAGE_POWER
-    return _unpack(plan.run(ws, stage, waveform), waveform)
+    return _unpack(plan.run(ws, stage, waveform, constants=(("window", window),)), waveform)
 
 
 # ---- inverse spectrogram ------------------------------------------------------------------------------------
@@ -408,7 +409,7 @@ def _apply_fbank(specgram: Tensor, fb: Tensor) -> Tensor:
 def mel_spectrogram(plan: FrontendPlan, window: Tensor, fb: Tensor, waveform: Tensor) -> Tensor:
     """Spectrogram + MelScale in ONE kernel: ``(..., time) -> (..., n_mels, time)``."""
     ws = plan.workspace(window, fb, None)
-    return _unpack(plan.run(ws, _lib.STAGE_MEL, waveform), waveform)
+    return _unpack(plan.run(ws, _lib.STAGE_MEL, waveform, constants=(("window", window), ("fb", fb))), waveform)
 
 
 def mfcc(

@@ -90,7 +90,7 @@ class Spectrogram(torch.nn.Module):
             self._plan = plan
         ws = self._plan.workspace(self.window, None, None)
         stage = _lib.STAGE_COMPLEX if self.power is None else _lib.STAGE_POWER
-        return F._unpack(self._plan.run(ws, stage, waveform), waveform)
+        return F._unpack(self._plan.run(ws, stage, waveform, constants=(("window", self.window),)), waveform)
 
 
 class InverseSpectrogram(torch.nn.Module):

@@ -137,6 +137,29 @@ int b200a_frontend_run(const b200a_frontend_desc* desc, const void* workspace, i
                        float* out, float* group_max, int64_t rows_per_group, b200a_stream stream);
 
 /*
+ * Waveform gradient of b200a_frontend_run (the backward of F.spectrogram [+ MelScale]) for stage COMPLEX, POWER or MEL,
+ * with the workspace the forward ran with.  With X = scale * DFT(w * frame) and g the upstream gradient:
+ *   G_k = g_k (COMPLEX), p |X_k|^(p-2) X_k s_k with s_k = g_k (POWER) or sum_m fb[k][m] g_m (MEL); G_k = 0 at X_k = 0
+ *   for p >= 1 and NaN for p < 1 (as torch's abs().pow(p) backward, which then makes the whole frame NaN);
+ *   dframe = scale * w * N * irfft(H),  H_k = (G_k + conj G_{N-k}) / 2,  G = 0 outside the output bins;
+ *   grad_wave = dframe overlap-added onto the padded signal and folded back onto the source samples (reflect mirrors,
+ *   replicate adds to the edge samples, circular wraps, constant and `pad` padding drop); samples no frame covers get 0.
+ *   wave       : the forward's input, as given to b200a_frontend_run
+ *   grad_out   : [rows][T][width] with element strides (stride 0 allowed: expanded gradients); for COMPLEX the strides
+ *                count complex elements, as in b200a_istft_run
+ *   scratch    : caller-owned device memory of b200a_frontend_backward_scratch_bytes(desc, stage, rows, length) bytes
+ *   grad_wave  : [rows] rows of `length` samples, row r at grad_wave + r * grad_row_stride (every sample written)
+ * Deterministic: no atomics, every row independent of the others.  B200A_STAGE_FEAT: B200A_EUNSUPPORTED.
+ */
+int b200a_frontend_backward(const b200a_frontend_desc* desc, const void* workspace, int32_t stage, const float* wave,
+                            int64_t rows, int64_t length, int64_t row_stride, const float* grad_out, int64_t g_stride_row,
+                            int64_t g_stride_frame, int64_t g_stride_col, void* scratch, float* grad_wave,
+                            int64_t grad_row_stride, b200a_stream stream);
+/* Bytes of scratch b200a_frontend_backward needs: rows * T * n_fft floats of frame gradients (n_fft = 256 / 512 / 1024,
+ * one-sided), plus the complex spectrum and a per-frame flag for every other size; 0 for an invalid request. */
+size_t b200a_frontend_backward_scratch_bytes(const b200a_frontend_desc* desc, int32_t stage, int64_t rows, int64_t length);
+
+/*
  * Second MFCC stage: top_db clamp + DCT-II, replaces functional.py:399 + _transforms.py:708.
  *   feat      : [rows][T][n_mels] from B200A_STAGE_FEAT
  *   group_max : [groups] maxima (after any cross-rank all-reduce), NULL or top_db < 0 => no clamp

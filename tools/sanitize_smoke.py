@@ -9,6 +9,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
+import audio_b200  # noqa: E402
 import audio_b200.compliance.kaldi as K  # noqa: E402
 import audio_b200.transforms as T  # noqa: E402
 
@@ -18,6 +19,12 @@ for n_fft in (256, 512, 1024, 2048, 400):
     T.Spectrogram(n_fft=n_fft, hop_length=n_fft // 4).cuda()(x)
     spec = T.Spectrogram(n_fft=n_fft, hop_length=n_fft // 4, power=None).cuda()(x)
     T.InverseSpectrogram(n_fft=n_fft, hop_length=n_fft // 4).cuda()(spec, 12000)
+with audio_b200.differentiable():  # waveform gradients: the fused path (512 / 1024), the composition path (400 / 2048)
+    for mod in (T.MelSpectrogram(16000, n_fft=1024, hop_length=256, n_mels=40), T.Spectrogram(n_fft=512, power=1.0),
+                T.Spectrogram(n_fft=512, power=None), T.MelSpectrogram(16000, n_fft=2048, hop_length=512, n_mels=40),
+                T.Spectrogram(n_fft=400, power=None, onesided=False)):
+        xg = x.clone().requires_grad_()
+        mod.cuda()(xg).abs().sum().backward()
 T.MFCC(16000, n_mfcc=13, melkwargs=dict(n_fft=512, hop_length=160, n_mels=40)).cuda()(x)
 T.MFCC(16000, n_mfcc=40, melkwargs=dict(n_fft=1024, hop_length=256, n_mels=80)).cuda()(x.reshape(1, 3, -1))
 for kw in (dict(num_mel_bins=40, snip_edges=False, use_energy=True), dict(num_mel_bins=23), dict(frame_length=20.0, round_to_power_of_two=False)):
