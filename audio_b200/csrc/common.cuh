@@ -11,6 +11,7 @@ namespace b200a {
 constexpr uint32_t kWsMagic = 0xB200A0D1u;
 constexpr int kMaxStages = 16;
 constexpr int kMaxFft = 8192;
+constexpr float kKaldiEps = 1.1920928955078125e-07f;  // numeric_limits<float>::epsilon(), kaldi.py:21-22
 
 // Device-side header at the start of a front-end workspace.
 struct WsHeader {
@@ -91,6 +92,20 @@ __device__ __forceinline__ float2 power_vjp(float re, float im, float p, float s
   if (mag == 0.f) return p < 1.f ? make_float2(CUDART_NAN_F, CUDART_NAN_F) : make_float2(0.f, 0.f);
   const float c = (p == 1.f ? s : p * powf(mag, p - 1.f) * s) / mag;
   return make_float2(re * c, im * c);
+}
+
+// The filters [x, y) with a non-zero weight at bin k, from each filter's non-zero bin range bands[m] = [x, y); (0, 0)
+// when none is.
+__device__ __forceinline__ int2 filter_range(const int2* bands, int n_mels, int k) {
+  int lo = n_mels, hi = 0;
+  for (int m = 0; m < n_mels; ++m) {
+    const int2 b = bands[m];
+    if (b.x <= k && k < b.y) {
+      lo = min(lo, m);
+      hi = m + 1;
+    }
+  }
+  return hi > lo ? make_int2(lo, hi) : make_int2(0, 0);
 }
 
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {

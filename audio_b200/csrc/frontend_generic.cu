@@ -113,8 +113,6 @@ struct GenericParams {
   float k_preemph, k_energy_floor;
 };
 
-constexpr float kKaldiEps = 1.1920928955078125e-07f;  // numeric_limits<float>::epsilon(), kaldi.py:21-22
-
 // Sample n of Kaldi frame t (kaldi.py:_get_strided).  snip_edges: frames lie inside the signal.  Otherwise the
 // signal is extended by its mirror image on both sides (x[-1-j] = x[j], x[L+j] = x[L-1-j]) and frame t starts
 // at t*shift - (win/2 - shift/2).
@@ -230,10 +228,6 @@ __device__ __forceinline__ float2* stockham_fft(float2* buf0, float2* buf1, cons
     Ns *= R;
   }
   return src;
-}
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
-  return make_float2(fmaf(a.x, b.x, -a.y * b.y), fmaf(a.x, b.y, a.y * b.x));
 }
 
 __device__ __forceinline__ float spectral_power(float re, float im, float power) {
@@ -835,6 +829,9 @@ int istft_frames_pow2(const b200a_frontend_desc*, const void*, const float*, int
 static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
                              int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf,
                              cudaStream_t stream) {
+  const int rc = istft_frames_pow2(d, ws, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, stream);
+  if (rc != B200A_EUNSUPPORTED) return rc;
+  // any other size: shared-memory Stockham
   const WsLayout l = ws_layout(*d);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   IstftParams p{};
@@ -861,12 +858,8 @@ static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const
     return B200A_ECUDA;
   const int64_t grid = rows * p.tiles_per_row;
   if (grid <= 0 || grid > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  int rc = istft_frames_pow2(d, ws, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, stream);
-  if (rc == B200A_EUNSUPPORTED) {  // any other size: shared-memory Stockham
-    istft_frames_kernel<<<(unsigned)grid, 256, smem, stream>>>(p);
-    rc = launch_status();
-  }
-  return rc;
+  istft_frames_kernel<<<(unsigned)grid, 256, smem, stream>>>(p);
+  return launch_status();
 }
 
 int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
@@ -922,17 +915,7 @@ __device__ __forceinline__ float2 spec_grad_at(const SpecVjpParams& p, const flo
 __global__ void __launch_bounds__(256) spec_vjp_kernel(const SpecVjpParams p) {
   extern __shared__ int2 s_range[];  // MEL: filters [x, y) with a non-zero weight at each bin
   if (p.stage == B200A_STAGE_MEL) {
-    for (int k = threadIdx.x; k < p.n_bins; k += blockDim.x) {
-      int lo = p.n_mels, hi = 0;
-      for (int m = 0; m < p.n_mels; ++m) {
-        const int2 b = p.bands[m];
-        if (b.x <= k && k < b.y) {
-          lo = min(lo, m);
-          hi = m + 1;
-        }
-      }
-      s_range[k] = hi > lo ? make_int2(lo, hi) : make_int2(0, 0);
-    }
+    for (int k = threadIdx.x; k < p.n_bins; k += blockDim.x) s_range[k] = filter_range(p.bands, p.n_mels, k);
     __syncthreads();
   }
   const int lane = threadIdx.x & 31, N = p.n_fft, half_n = N / 2;

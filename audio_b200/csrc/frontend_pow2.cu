@@ -34,7 +34,6 @@ namespace b200a {
 
 namespace {
 
-constexpr float kKaldiEps = 1.1920928955078125e-07f;  // numeric_limits<float>::epsilon(), kaldi.py:21-22
 constexpr int kPadSymmetric = 4;  // internal pad mode: x[-1-j] = x[j], x[L+j] = x[L-1-j] (Kaldi snip_edges = false)
 constexpr int kWarps = 8;     // transform warps per CTA (n_fft = 2048 kernels)
 constexpr int kMelWarps = 4;  // contraction warps per CTA (n_fft = 2048 mel kernel)
@@ -318,13 +317,107 @@ __device__ __forceinline__ void issue_bulk(const Pow2Params& p, int half, int64_
   bulk_g2s(dst, src, bytes, bar);
 }
 
+// The (32 G)-point complex FFT of one lane group, in place, as fft_pass1 then fft_pass2: lane l holds x[l + G j] in
+// a[brev5(j)] and ends with X[(l + G q) + 32 k1] in a[q*G + k1].  Between the two calls the group's region is free:
+// a forward kernel stages its next input into it there.
+//
+// fft_pass1: a 32-point DFT over j in registers, the twiddle W^(l * k2) from s_tw ([32][G]), and a transpose through
+// the group's region, after which lane l owns k2 = l + G q.  SPLIT: transpose the real parts, then the imaginary parts,
+// through kRegionF floats (half the shared memory of the float2 transpose, kRegion float2).  kTwAhead: how many
+// twiddle loads are in flight; they are issued before the last butterfly stage, and every multiply issues the load
+// kTwAhead positions ahead of it, so no multiply waits for its own load.  0 loads each twiddle at its multiply.
+template <int G, bool SPLIT, int kTwAhead>
+__device__ __forceinline__ void fft_pass1(float2 (&a)[32], const float2* s_tw, float* region, int l) {
+  using Ge = Geo<G>;
+  fft_regs<32, 0, 0, 4>(a);
+  float2 tw[32];
+  static_for<kTwAhead>([&](auto ki) {
+    constexpr int k2 = decltype(ki)::value + 1;
+    tw[k2] = s_tw[k2 * G + l];
+  });
+  fft_regs<32, 0, 4, 5>(a);  // a[k2] = Y[l][k2]
+  // slot q*G + brev(g) <- element (g, l + G q)
+  if constexpr (SPLIT) {
+    region[l] = a[0].x;
+    static_for<31>([&](auto ki) {
+      constexpr int k2 = decltype(ki)::value + 1;
+      if constexpr (k2 + kTwAhead < 32) tw[k2 + kTwAhead] = s_tw[(k2 + kTwAhead) * G + l];
+      a[k2] = cmul2(a[k2], tw[k2]);
+      region[k2 * Ge::kRowLd + l] = a[k2].x;
+    });
+    __syncwarp();
+    float re[32];
+    static_for<32>([&](auto si) {
+      constexpr int s = decltype(si)::value;
+      re[s] = region[(l + G * (s / G)) * Ge::kRowLd + s % G];
+    });
+    __syncwarp();
+    static_for<32>([&](auto ki) {
+      constexpr int k2 = decltype(ki)::value;
+      region[k2 * Ge::kRowLd + l] = a[k2].y;
+    });
+    __syncwarp();
+    static_for<32>([&](auto si) {
+      constexpr int s = decltype(si)::value;
+      constexpr int q = s / G, g = s % G;
+      a[q * G + brev<Ge::kLogG>(g)] = make_float2(re[s], region[(l + G * q) * Ge::kRowLd + g]);
+    });
+  } else {
+    float2* tile = reinterpret_cast<float2*>(region);
+    tile[l] = a[0];
+    static_for<31>([&](auto ki) {
+      constexpr int k2 = decltype(ki)::value + 1;
+      if constexpr (k2 + kTwAhead < 32) tw[k2 + kTwAhead] = s_tw[(k2 + kTwAhead) * G + l];
+      tile[k2 * Ge::kRowLd + l] = cmul2(a[k2], tw[k2]);
+    });
+    __syncwarp();
+    static_for<32>([&](auto si) {
+      constexpr int s = decltype(si)::value;
+      constexpr int q = s / G, g = s % G;
+      a[q * G + brev<Ge::kLogG>(g)] = tile[(l + G * q) * Ge::kRowLd + g];
+    });
+  }
+  __syncwarp();
+}
+
+// fft_pass2: 32/G G-point DFTs over the former lane index, in registers.
+template <int G>
+__device__ __forceinline__ void fft_pass2(float2 (&a)[32]) {
+  static_for<Geo<G>::kGroups>([&](auto qi) { fft_regs<G, decltype(qi)::value * G>(a); });
+}
+
+// The frames an inverse transform rebuilt: a[(m % NG)*G + m/NG] = FFT(conj Z)[l + G m] = N (a[n] - i b[n]) with
+// Z = A + i B.  Stores sample n = l + G m of frame a (Re) and frame b (-Im) times w_mul * s_win[n] from frame_a, frame
+// a's row of the frame buffer offset by l; a frame marked bad gets NaN instead.
+template <int G>
+__device__ __forceinline__ void store_frame_pair(const float2 (&a)[32], float* frame_a, const float* s_win, float w_mul,
+                                                 int l, bool has_a, bool has_b, bool bad_a, bool bad_b) {
+  constexpr int N = Geo<G>::kNfft, NG = Geo<G>::kGroups;
+  static_for<32>([&](auto mi) {
+    constexpr int m = decltype(mi)::value;
+    constexpr int slot = (m % NG) * G + m / NG;
+    const float w = w_mul * s_win[l + G * m];
+    if (has_a) frame_a[G * m] = bad_a ? CUDART_NAN_F : a[slot].x * w;
+    if (has_b) frame_a[N + G * m] = bad_b ? CUDART_NAN_F : -a[slot].y * w;
+  });
+}
+
+// The inter-pass twiddles [32][G] and the window times gain [32 G] into shared memory.
+template <int G>
+__device__ __forceinline__ void load_fft_tables(const float2* tw2d, const float* window, float gain, float2* s_tw,
+                                                float* s_win) {
+  for (int i = threadIdx.x; i < 32 * G; i += blockDim.x) {
+    s_tw[i] = tw2d[i];
+    s_win[i] = window[i] * gain;
+  }
+}
+
 // One warp, one unit (32/G frame pairs): samples -> windowed complex signals -> n_fft-point FFTs -> the
 // power spectra.  On return lane (group gi, l) holds bins k = l + G m in pa[m] / pb[m] (m < 16) of frames
 // t0 + 2 gi and t0 + 2 gi + 1, and lanes with l == 0 bin n_fft/2 in [16].
 // The staging buffer is the warp's transpose tile itself: the NEXT unit's bulk copy is issued only after
-// pass 2 has read the tile back.  s_win: the window x 1/2 (un-packing) x the normalisation scale, [n_fft].
-// SPLIT: transpose the real parts, then the imaginary parts, through kRegionF floats per lane group (half the
-// shared memory of the float2 transpose, kRegion float2 per lane group).
+// fft_pass1 has read the tile back.  s_win: the window x 1/2 (un-packing) x the normalisation scale, [n_fft].
+// SPLIT: the transpose of fft_pass1, through kRegionF floats per lane group.
 // POWER_MODE == kSpectra: PT = float2, pa / pb receive the complex bins themselves (bin N/2 with a zero imaginary part).
 template <int POWER_MODE, int G, int HG, bool KALDI, bool SPLIT, typename PT>
 __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float* s_win, const float2* s_tw,
@@ -346,7 +439,6 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
   const bool interior = s0 >= 0 && s0 + (last - 1) * p.hop + Ge::kNfft <= p.length;
 
   float2 a[32];
-  float2* grp_tile = tile + gi * Ge::kRegion;
   float* grp_f = stage + gi * (SPLIT ? Ge::kRegionF : 2 * Ge::kRegion);  // the lane group's region as floats
   bool from_stage = staged;
   if (staged) {
@@ -499,64 +591,15 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
     }
   }
 
-  // the inter-pass twiddles: kTwAhead loads are in flight before the last butterfly stage, and every multiply
-  // issues the load kTwAhead positions ahead of it, so no multiply waits for its own load
-  constexpr int kTwAhead = 8;
-  fft_regs<32, 0, 0, 4>(a);
-  float2 tw[32];
-  static_for<kTwAhead>([&](auto ki) {
-    constexpr int k2 = decltype(ki)::value + 1;
-    tw[k2] = s_tw[k2 * G + l];
-  });
-  fft_regs<32, 0, 4, 5>(a);  // a[k2] = Y[l][k2]
-  // lane l then owns k2 = l + G q, q < 32/G: slot q*G + brev(g) <- element (g, l + G q)
-  if constexpr (SPLIT) {
-    grp_f[l] = a[0].x;
-    static_for<31>([&](auto ki) {
-      constexpr int k2 = decltype(ki)::value + 1;
-      if constexpr (k2 + kTwAhead < 32) tw[k2 + kTwAhead] = s_tw[(k2 + kTwAhead) * G + l];
-      a[k2] = cmul2(a[k2], tw[k2]);
-      grp_f[k2 * Ge::kRowLd + l] = a[k2].x;
-    });
-    __syncwarp();
-    float re[32];
-    static_for<32>([&](auto si) {
-      constexpr int s = decltype(si)::value;
-      re[s] = grp_f[(l + G * (s / G)) * Ge::kRowLd + s % G];
-    });
-    __syncwarp();
-    static_for<32>([&](auto ki) {
-      constexpr int k2 = decltype(ki)::value;
-      grp_f[k2 * Ge::kRowLd + l] = a[k2].y;
-    });
-    __syncwarp();
-    static_for<32>([&](auto si) {
-      constexpr int s = decltype(si)::value;
-      constexpr int q = s / G, g = s % G;
-      a[q * G + brev<Ge::kLogG>(g)] = make_float2(re[s], grp_f[(l + G * q) * Ge::kRowLd + g]);
-    });
-  } else {
-    grp_tile[l] = a[0];
-    static_for<31>([&](auto ki) {
-      constexpr int k2 = decltype(ki)::value + 1;
-      if constexpr (k2 + kTwAhead < 32) tw[k2 + kTwAhead] = s_tw[(k2 + kTwAhead) * G + l];
-      grp_tile[k2 * Ge::kRowLd + l] = cmul2(a[k2], tw[k2]);
-    });
-    __syncwarp();
-    static_for<32>([&](auto si) {
-      constexpr int s = decltype(si)::value;
-      constexpr int q = s / G, g = s % G;
-      a[q * G + brev<Ge::kLogG>(g)] = grp_tile[(l + G * q) * Ge::kRowLd + g];
-    });
-  }
-  __syncwarp();
+  // the float2 transpose's region is grp_f, addressed from the tile: through grp_f, ptxas spills 8 B instead of 4 B in
+  // the n_fft = 1024 general-power Spectrogram kernel
+  fft_pass1<G, SPLIT, 8>(a, s_tw, SPLIT ? grp_f : reinterpret_cast<float*>(tile + gi * Ge::kRegion), l);
   staged = next_staged;  // the tile is free until the next unit's transpose: stage into it
   if (staged && lane == 0) {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads above -> async write
     issue_bulk<G>(p, half, cur.nrow, cur.nub, stage, bar);
   }
-
-  static_for<Ge::kGroups>([&](auto qi) { fft_regs<G, decltype(qi)::value * G>(a); });
+  fft_pass2<G>(a);
   // a[q*G + k1] = Z[(l + G q) + 32 k1]; bin k = l + G m with m = q + (32/G) k1  <->  slot (m % NG)*G + m / NG
 
   // ---- un-pack the two spectra: need Z[N - k] for k = l + G m, m = 0..15 (+ bin N/2 on l == 0) ----
@@ -611,12 +654,6 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
   }
 }
 
-// the window x 1/2 (from the un-packing) x the normalisation scale, [n] into shared memory
-__device__ __forceinline__ void load_window(const Pow2Params& p, float* s_win, int n, int tid, int nthreads) {
-  const float hs = 0.5f * p.hdr->scale;
-  for (int i = tid; i < n; i += nthreads) s_win[i] = p.window[i] * hs;
-}
-
 // ------------------------------------------------------------------------------------------------
 // Spectrogram kernel: NW independent warps, power spectra straight to global memory.
 // ------------------------------------------------------------------------------------------------
@@ -630,8 +667,10 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_tile_all + NW * Ge::kTileF2);          // [NW]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // the tables of load_fft_tables, written out: through the helper the n_fft = 1024 general-power variant spills more
   for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
-  load_window(p, s_win, Ge::kNfft, tid, blockDim.x);
+  const float hs = 0.5f * p.hdr->scale;  // the window x 1/2 (un-packing) x scale
+  for (int i = tid; i < Ge::kNfft; i += blockDim.x) s_win[i] = p.window[i] * hs;
   if (tid < NW) mbar_init(s_bar + tid, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   __syncthreads();
@@ -757,6 +796,26 @@ __device__ __forceinline__ void contract_tile(const Pow2Params& p, const MelPlan
                          g_lo, g_hi, gmax);
 }
 
+// The mel kernels' tables: copies the MelPlan into shared memory, stages the filterbank fragments when the plan has at
+// most max_steps k-steps (returns whether it did), and zeroes columns [bins, pitch) of the `slots` power rows, which the
+// last k-step reads.
+__device__ __forceinline__ bool load_mel_plan(const Pow2Params& p, MelPlan* s_plan, float4* s_frags, int max_steps,
+                                              float* s_pow, int slots, int pitch, int bins) {
+  const int tid = threadIdx.x;
+  const int* src = reinterpret_cast<const int*>(p.plan);
+  int* dst = reinterpret_cast<int*>(s_plan);
+  for (int i = tid; i < (int)(sizeof(MelPlan) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
+  const int total_steps = p.plan->total_steps;
+  const bool frags_in_smem = total_steps <= max_steps;
+  if (frags_in_smem)
+    for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
+  for (int i = tid; i < slots * (pitch - bins); i += blockDim.x) {
+    const int r = i / (pitch - bins), c = i - r * (pitch - bins);
+    s_pow[r * pitch + bins + c] = 0.f;
+  }
+  return frags_in_smem;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Mel / MFCC-feature kernel (n_fft = 256 / 512 / 1024): 16 uniform warps.  Every iteration each warp transforms
 // one unit, waits at a CTA barrier until the previous contraction has read the (single) power tile, publishes
@@ -790,22 +849,8 @@ __device__ __forceinline__ void mel_body(const Pow2Params& p, unsigned char* sme
   float4* s_frags = reinterpret_cast<float4*>(s_plan + 1);                         // [<= kMelFragSteps][32]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
-  load_window(p, s_win, Ge::kNfft, tid, blockDim.x);
-  {
-    const int* src = reinterpret_cast<const int*>(p.plan);
-    int* dst = reinterpret_cast<int*>(s_plan);
-    for (int i = tid; i < (int)(sizeof(MelPlan) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
-  }
-  const int total_steps = p.plan->total_steps;
-  const bool frags_in_smem = total_steps <= Ge::kMelFragSteps;
-  if (frags_in_smem)
-    for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
-  // columns >= n_bins of every power row are read by the last k-step: keep them finite (zero)
-  for (int i = tid; i < kSlots * (kPitch - Ge::kBins); i += blockDim.x) {
-    const int r = i / (kPitch - Ge::kBins), c = i - r * (kPitch - Ge::kBins);
-    s_pow[r * kPitch + Ge::kBins + c] = 0.f;
-  }
+  load_fft_tables<G>(p.tw2d, p.window, 0.5f * p.hdr->scale, s_tw, s_win);  // the window x 1/2 (un-packing) x scale
+  const bool frags_in_smem = load_mel_plan(p, s_plan, s_frags, Ge::kMelFragSteps, s_pow, kSlots, kPitch, Ge::kBins);
   if (tid < kUniWarps) mbar_init(s_bar + tid, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   __syncthreads();
@@ -933,20 +978,7 @@ __device__ __forceinline__ void transform_frame_eo(const Pow2Params& p, const fl
     __syncwarp();
   }
 
-  fft_regs<32, 0>(a);
-  tile[lane] = a[0];
-  static_for<31>([&](auto ki) {
-    constexpr int k2 = decltype(ki)::value + 1;
-    const float2 w = s_tw[k2 * 32 + lane];
-    const float2 v = a[k2];
-    tile[k2 * 33 + lane] = cmul2(v, w);
-  });
-  __syncwarp();
-  static_for<32>([&](auto gi) {
-    constexpr int g = decltype(gi)::value;
-    a[brev5(g)] = tile[lane * 33 + g];
-  });
-  __syncwarp();
+  fft_pass1<32, false, 0>(a, s_tw, stage, lane);
   staged = next_ok && eo_frame_bulk_ok(p, half, next_t);
   if (staged && lane == 0) {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -954,7 +986,7 @@ __device__ __forceinline__ void transform_frame_eo(const Pow2Params& p, const fl
     mbar_expect_tx(bar, kEoN * 4u);
     bulk_g2s(stage, src, kEoN * 4u, bar);
   }
-  fft_regs<32, 0>(a);  // a[k1] = Z[lane + 32 k1]
+  fft_pass2<32>(a);  // a[k1] = Z[lane + 32 k1]
 
   const int src_lane = (32 - lane) & 31;
   static_for<16>([&](auto ki) {
@@ -1066,19 +1098,7 @@ __global__ void __launch_bounds__((kWarps + kMelWarps) * 32, 1) stft2048_mel_ker
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   eo_load_tables(p, tw_eo, s_win, s_tw, s_tw2, tid, blockDim.x);
-  {
-    const int* src = reinterpret_cast<const int*>(p.plan);
-    int* dst = reinterpret_cast<int*>(s_plan);
-    for (int i = tid; i < (int)(sizeof(MelPlan) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
-  }
-  const int total_steps = p.plan->total_steps;
-  const bool frags_in_smem = total_steps <= kEoFragSteps;
-  if (frags_in_smem)
-    for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
-  for (int i = tid; i < kEoSlots * (kEoPitch - kEoBins); i += blockDim.x) {
-    const int r = i / (kEoPitch - kEoBins), c = i - r * (kEoPitch - kEoBins);
-    s_pow[r * kEoPitch + kEoBins + c] = 0.f;
-  }
+  const bool frags_in_smem = load_mel_plan(p, s_plan, s_frags, kEoFragSteps, s_pow, kEoSlots, kEoPitch, kEoBins);
   if (tid < kWarps) mbar_init(s_bar + tid, 1);
   if (tid == 0) {
     mbar_init(s_full, kWarps);
@@ -1166,9 +1186,11 @@ __global__ void __launch_bounds__(kUniWarps * 32, 1) stft_pow2_mel_kernel(const 
 // Inverse STFT frames on the register FFT (n_fft = 256 / 512 / 1024): the first half of b200a_istft_run.
 // A lane group rebuilds the PAIR of frames (a, b) from their two Hermitian spectra with ONE complex transform:
 //   Z[k] = A[k] + i B[k] (k <= N/2),  Z[N-k] = conj(A[k]) + i conj(B[k]);  z = IFFT(Z) = a + i b
-// computed as conj(FFT(conj Z)) / N with the forward passes of transform_unit (32-point register DFT, twiddle,
-// transpose through the padded tile, G-point register DFTs).  Lane l loads bins n = l + G j and ends with time
-// samples n = l + G m, which it multiplies by window / (N * forward normalisation) and stores to the frame buffer.
+// computed as conj(FFT(conj Z)) / N with the forward passes (32-point register DFT, twiddle, transpose through the
+// padded tile, then fft_pass2).  Pass 1 is fft_pass1<G, false, 0> written out: through fft_pass1 the n_fft = 1024
+// kernel took 1.92 ms instead of 1.61 ms for a 256 x 160000-sample inverse (H100 80GB HBM3, 400 W limit).  Lane l
+// loads bins n = l + G j and ends with time samples n = l + G m, which store_frame_pair multiplies by
+// window / (N * forward normalisation) and stores to the frame buffer.
 // C2R semantics: the imaginary parts of bins 0 and N/2 are ignored.
 // ================================================================================================
 struct IstftPow2Params {
@@ -1184,19 +1206,20 @@ struct IstftPow2Params {
 constexpr int kIsWarps = 16;
 
 template <int G>
+constexpr size_t istft_smem() {  // twiddles, window, transpose tiles
+  return sizeof(float2) * (32 * G + kIsWarps * Geo<G>::kTileF2) + sizeof(float) * Geo<G>::kNfft;
+}
+
+template <int G>
 __global__ void __launch_bounds__(kIsWarps * 32, 1) istft_pow2_kernel(const IstftPow2Params p) {
   using Ge = Geo<G>;
-  constexpr int N = Ge::kNfft, NG = Ge::kGroups;
+  constexpr int N = Ge::kNfft;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2* s_tw = reinterpret_cast<float2*>(smem_raw);  // [32][G]
   float* s_win = reinterpret_cast<float*>(s_tw + 32 * G);  // [N] window / (N * forward normalisation)
   float2* s_tile_all = reinterpret_cast<float2*>(s_win + N);  // [kIsWarps][kTileF2]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
-  {
-    const float gain = 1.f / ((float)N * p.hdr->scale);
-    for (int i = tid; i < N; i += blockDim.x) s_win[i] = p.window[i] * gain;
-  }
+  load_fft_tables<G>(p.tw2d, p.window, 1.f / ((float)N * p.hdr->scale), s_tw, s_win);
   __syncthreads();
   float2* grp_tile = s_tile_all + warp * Ge::kTileF2 + (lane / G) * Ge::kRegion;
   const int gi = lane / G, l = lane % G;
@@ -1236,16 +1259,8 @@ __global__ void __launch_bounds__(kIsWarps * 32, 1) istft_pow2_kernel(const Istf
       a[q * G + brev<Ge::kLogG>(g)] = grp_tile[(l + G * q) * Ge::kRowLd + g];
     });
     __syncwarp();
-    static_for<NG>([&](auto qi) { fft_regs<G, decltype(qi)::value * G>(a); });
-    // a[(m % NG) G + m / NG] = FFT(conj Z)[l + G m] = N (a[n] - i b[n])
-    float* fa = p.frame_buf + (cur.row * p.frames + ta) * N + l;
-    static_for<32>([&](auto mi) {
-      constexpr int m = decltype(mi)::value;
-      constexpr int slot = (m % NG) * G + m / NG;
-      const float w = s_win[l + G * m];
-      if (has_a) fa[G * m] = a[slot].x * w;
-      if (has_b) fa[N + G * m] = -a[slot].y * w;
-    });
+    fft_pass2<G>(a);
+    store_frame_pair<G>(a, p.frame_buf + (cur.row * p.frames + ta) * N + l, s_win, 1.f, l, has_a, has_b, false, false);
   }
 }
 
@@ -1254,7 +1269,7 @@ __global__ void __launch_bounds__(kIsWarps * 32, 1) istft_pow2_kernel(const Istf
 // Per unit a warp recomputes the forward transform from the waveform (transform_unit, the spectra kept complex), forms
 // the per-bin gradient G (upstream value, or p |X|^(p-2) X s with s = g or sum_m fb[k][m] g_m) and its Hermitian part
 // H_k = (G_k + conj G_{N-k}) / 2 in registers, fetches the mirrored half of H with one shuffle per value as the forward
-// un-packing does, and runs the inverse passes of istft_pow2_kernel.  The frame gradients scale * w * N * irfft(H) go
+// un-packing does, and runs the inverse transform of istft_pow2_kernel.  The frame gradients scale * w * N * irfft(H) go
 // to frame_buf; X never leaves the registers.  Units are loaded without the bulk prefetch, so the transpose tile is
 // free for the inverse passes.  A frame with a NaN bin gets NaN everywhere (torch's p < 1 gradient at X = 0).
 // ================================================================================================
@@ -1267,7 +1282,6 @@ struct BwdParams {
   float* frame_buf;  // [rows][frames][n_fft]
   const float* fb;   // [n_bins][n_mels]
   const int2* bands;  // [n_mels]
-  int stage;
 };
 
 template <int G>
@@ -1278,7 +1292,7 @@ constexpr size_t bwd_smem_fixed() {  // twiddles, window, transpose tiles, per-b
 template <int G, int STAGE>
 __global__ void __launch_bounds__(kBwWarps * 32, 1) stft_pow2_backward_kernel(const BwdParams bp) {
   using Ge = Geo<G>;
-  constexpr int N = Ge::kNfft, NG = Ge::kGroups;
+  constexpr int N = Ge::kNfft;
   const Pow2Params& p = bp.f;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2* s_tw = reinterpret_cast<float2*>(smem_raw);                    // [32][G]
@@ -1288,26 +1302,14 @@ __global__ void __launch_bounds__(kBwWarps * 32, 1) stft_pow2_backward_kernel(co
   float* s_g_all = reinterpret_cast<float*>(s_range + Ge::kBins);        // [kBwWarps][kFrames][n_mels] MEL
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
-  load_window(p, s_win, N, tid, blockDim.x);
+  load_fft_tables<G>(p.tw2d, p.window, 0.5f * p.hdr->scale, s_tw, s_win);
   const int n_mels = p.n_mels;
-  if constexpr (STAGE == B200A_STAGE_MEL) {
-    for (int k = tid; k < Ge::kBins; k += blockDim.x) {
-      int lo = n_mels, hi = 0;
-      for (int m = 0; m < n_mels; ++m) {
-        const int2 b = bp.bands[m];
-        if (b.x <= k && k < b.y) {
-          lo = min(lo, m);
-          hi = m + 1;
-        }
-      }
-      s_range[k] = hi > lo ? make_int2(lo, hi) : make_int2(0, 0);
-    }
-  }
+  if constexpr (STAGE == B200A_STAGE_MEL)
+    for (int k = tid; k < Ge::kBins; k += blockDim.x) s_range[k] = filter_range(bp.bands, n_mels, k);
   __syncthreads();
 
   float2* tile = s_tile_all + warp * Ge::kTileF2;
-  float2* grp_tile = tile + (lane / G) * Ge::kRegion;
+  float* region = reinterpret_cast<float*>(tile) + (lane / G) * 2 * Ge::kRegion;
   float* s_g = s_g_all + (size_t)warp * Ge::kFrames * n_mels;
   const int half = frame_lead(p, N);
   const int gi = lane / G, l = lane % G;
@@ -1398,30 +1400,10 @@ __global__ void __launch_bounds__(kBwWarps * 32, 1) stft_pow2_backward_kernel(co
       }
       a[brev5(j)] = make_float2(ha.x - hb.y, -(ha.y + hb.x));
     });
-    // ---- inverse passes (istft_pow2_kernel) ----
-    fft_regs<32, 0>(a);
-    grp_tile[l] = a[0];
-    static_for<31>([&](auto ki) {
-      constexpr int k2 = decltype(ki)::value + 1;
-      grp_tile[k2 * Ge::kRowLd + l] = cmul2(a[k2], s_tw[k2 * G + l]);
-    });
-    __syncwarp();
-    static_for<32>([&](auto si) {
-      constexpr int s = decltype(si)::value;
-      constexpr int q = s / G, g = s % G;
-      a[q * G + brev<Ge::kLogG>(g)] = grp_tile[(l + G * q) * Ge::kRowLd + g];
-    });
-    __syncwarp();
-    static_for<NG>([&](auto qi) { fft_regs<G, decltype(qi)::value * G>(a); });
-    // a[(m % NG) G + m / NG] = FFT(conj Z)[l + G m] = N (a[n] - i b[n]);  dframe = scale * w * N * irfft(H)
-    float* fa = bp.frame_buf + (cur.row * p.frames + ta) * N + l;
-    static_for<32>([&](auto mi) {
-      constexpr int m = decltype(mi)::value;
-      constexpr int slot = (m % NG) * G + m / NG;
-      const float w = 2.f * s_win[l + G * m];  // window x scale
-      if (has_a) fa[G * m] = bad_a ? CUDART_NAN_F : a[slot].x * w;
-      if (has_b) fa[N + G * m] = bad_b ? CUDART_NAN_F : -a[slot].y * w;
-    });
+    // ---- the inverse transform, as in istft_pow2_kernel: dframe = scale * w * N * irfft(H) (2 s_win = window x scale) ----
+    fft_pass1<G, false, 0>(a, s_tw, region, l);
+    fft_pass2<G>(a);
+    store_frame_pair<G>(a, bp.frame_buf + (cur.row * p.frames + ta) * N + l, s_win, 2.f, l, has_a, has_b, bad_a, bad_b);
   }
 }
 
@@ -1547,15 +1529,24 @@ int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaSt
   return launch_status();
 }
 
-static int num_sms() { return device_sm_count(); }
-
-// persistent: one resident CTA per SM, units dealt round-robin (every CTA gets the same count +-1)
-static int64_t persistent_grid(const Pow2Params& p, int warps = kWarps) {
-  const int sms = num_sms();
+// persistent: one resident CTA per SM, units dealt round-robin (every CTA gets the same count +-1); -1 when the SM
+// count cannot be read
+static int64_t persistent_grid(int64_t total_units, int warps) {
+  const int sms = device_sm_count();
   if (sms < 0) return -1;
-  const int64_t iters = (p.total_units + warps - 1) / warps;
+  const int64_t iters = (total_units + warps - 1) / warps;
   const int64_t grid = iters < sms ? iters : sms;
   return grid < 1 ? 1 : grid;
+}
+
+// Raises the kernel's dynamic shared-memory limit to kSmemLimit and launches it on `grid` CTAs (grid < 0: the
+// persistent_grid error).
+template <typename Kernel, typename... Args>
+static int launch_kernel(Kernel kern, int64_t grid, int threads, size_t smem, cudaStream_t stream, const Args&... args) {
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess || grid < 0)
+    return B200A_ECUDA;
+  kern<<<(unsigned)grid, threads, smem, stream>>>(args...);
+  return launch_status();
 }
 
 template <int POWER_MODE, int G, int HG>
@@ -1568,12 +1559,7 @@ static int launch_power(const Pow2Params& p, cudaStream_t stream) {
   auto kern = stft_pow2_power_kernel<POWER_MODE, G, HG, NW, false>;
   if constexpr (POWER_MODE != kComplexOut)
     if (p.kaldi) kern = stft_pow2_power_kernel<POWER_MODE, G, -1, NW, true>;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-    return B200A_ECUDA;
-  const int64_t grid = persistent_grid(p, NW);
-  if (grid < 0) return B200A_ECUDA;
-  kern<<<(unsigned)grid, NW * 32, smem, stream>>>(p);
-  return launch_status();
+  return launch_kernel(kern, persistent_grid(p.total_units, NW), NW * 32, smem, stream, p);
 }
 
 template <int POWER_MODE, int G, int HG>
@@ -1585,12 +1571,7 @@ static int launch_mel(const Pow2Params& p, cudaStream_t stream) {
   constexpr size_t smem = mel_smem_bytes<G>();
   static_assert(smem <= kSmemLimit, "16-warp mel kernel exceeds the shared-memory budget");
   auto kern = p.kaldi ? stft_pow2_mel_kernel<POWER_MODE, G, -1, true> : stft_pow2_mel_kernel<POWER_MODE, G, HG, false>;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess)
-    return B200A_ECUDA;
-  const int64_t grid = persistent_grid(p, kUniWarps);
-  if (grid < 0) return B200A_ECUDA;
-  kern<<<(unsigned)grid, kUniWarps * 32, smem, stream>>>(p);
-  return launch_status();
+  return launch_kernel(kern, persistent_grid(p.total_units, kUniWarps), kUniWarps * 32, smem, stream, p);
 }
 
 template <int POWER_MODE, int G>
@@ -1617,24 +1598,52 @@ static int launch_any(Pow2Params& p, int n_fft, bool mel, cudaStream_t stream) {
 
 template <int POWER_MODE>
 static int launch_eo(const Pow2Params& p, const float2* tw_eo, bool mel, cudaStream_t stream) {
-  const int64_t grid = persistent_grid(p);
-  if (grid < 0) return B200A_ECUDA;
+  const int64_t grid = persistent_grid(p.total_units, kWarps);
   const size_t tables = sizeof(float2) * (1024 + 1024 + 17 * 32 + kWarps * 32 * 33);
-  if (!mel) {
-    auto kern = stft2048_power_kernel<POWER_MODE>;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-      return B200A_ECUDA;
-    kern<<<(unsigned)grid, kWarps * 32, tables + sizeof(uint64_t) * kWarps, stream>>>(p, tw_eo);
-    return launch_status();
-  }
+  if (!mel)
+    return launch_kernel(stft2048_power_kernel<POWER_MODE>, grid, kWarps * 32, tables + sizeof(uint64_t) * kWarps, stream,
+                         p, tw_eo);
   const size_t smem = tables + sizeof(float) * kEoSlots * kEoPitch + sizeof(int64_t) * 2 * kEoSlots +
                       sizeof(uint64_t) * (kWarps + 2) + sizeof(MelPlan) + sizeof(float4) * 32 * kEoFragSteps;
-  if (smem > 227 * 1024) return B200A_EUNSUPPORTED;
-  auto kern = stft2048_mel_kernel<POWER_MODE>;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-    return B200A_ECUDA;
-  kern<<<(unsigned)grid, (kWarps + kMelWarps) * 32, smem, stream>>>(p, tw_eo);
-  return launch_status();
+  if (smem > kSmemLimit) return B200A_EUNSUPPORTED;
+  return launch_kernel(stft2048_mel_kernel<POWER_MODE>, grid, (kWarps + kMelWarps) * 32, smem, stream, p, tw_eo);
+}
+
+// floats of a warp's staging region: the mel kernel's region, or the float2 transpose tile of the Spectrogram and
+// gradient kernels
+static int stage_floats(int G, bool mel) {
+  if (mel) return G == 8 ? Geo<8>::kMelRegion : G == 16 ? Geo<16>::kMelRegion : Geo<32>::kMelRegion;
+  return 2 * (G == 8 ? Geo<8>::kTileF2 : G == 16 ? Geo<16>::kTileF2 : Geo<32>::kTileF2);
+}
+
+// The Pow2Params fields the forward and the gradient kernels fill alike: the waveform and its framing, the window,
+// twiddle and header tables of the workspace, and stage_ok: an edge unit's span fits the warp's staging region of
+// `staging` floats, and its gather can index with 32 bits.
+static Pow2Params pow2_geometry(const b200a_frontend_desc& d, const void* ws, const float* wave, int64_t rows,
+                                int64_t length, int64_t row_stride, int64_t frames, int staging) {
+  const WsLayout l = ws_layout(d);
+  const Pow2Extra e = pow2_layout(d, l.total);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const int G = d.n_fft == 2048 ? 32 : d.n_fft / 32;
+  const int frames_per_unit = 2 * (32 / G);
+  Pow2Params p{};
+  p.wave = wave;
+  p.length = length;
+  p.row_stride = row_stride;
+  p.frames = frames;
+  p.units_per_row = (frames + frames_per_unit - 1) / frames_per_unit;
+  p.total_units = rows * p.units_per_row;
+  p.window = reinterpret_cast<const float*>(base + l.window);
+  p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
+  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.hop = d.hop;
+  p.pad = d.pad;
+  p.center = d.center;
+  p.pad_mode = d.pad_mode;
+  p.power = d.power;
+  p.stage_ok = d.n_fft + (frames_per_unit - 1) * (int64_t)d.hop <= staging &&
+               length + 2 * (int64_t)d.pad + d.n_fft < (int64_t)1 << 31;
+  return p;
 }
 
 int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
@@ -1645,52 +1654,32 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   // Kaldi features with a 256 / 512 / 1024-point FFT; every other size takes the generic kernel
   if (kd != nullptr && d->n_fft > 1024) return B200A_EUNSUPPORTED;
   if (stage >= B200A_STAGE_MEL && mel_tiles(d->n_mels) > kMaxItems) return B200A_EUNSUPPORTED;  // > 512 filters
-  const WsLayout l = ws_layout(*d);
-  const Pow2Extra e = pow2_layout(*d, l.total);
+  const Pow2Extra e = pow2_layout(*d, ws_layout(*d).total);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   const bool eo = d->n_fft == 2048;
   const int G = eo ? 32 : d->n_fft / 32;
   const int frames_per_unit = 2 * (32 / G);
-  Pow2Params p{};
-  p.wave = wave;
-  p.length = length;
-  p.row_stride = row_stride;
-  p.frames = frames;
-  p.units_per_row = (frames + frames_per_unit - 1) / frames_per_unit;
-  p.total_units = rows * p.units_per_row;
+  const bool mel = stage >= B200A_STAGE_MEL;
+  const int staging = stage_floats(G, mel);
+  Pow2Params p = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, staging);
   p.out = out;
   p.group_max = group_max;
   p.rows_per_group = rows_per_group > 0 ? rows_per_group : 1;
-  p.window = reinterpret_cast<const float*>(base + l.window);
-  p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
   p.plan = reinterpret_cast<const MelPlan*>(base + e.plan);
   p.frags = reinterpret_cast<const float4*>(base + e.frags);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
-  p.hop = d->hop;
-  p.pad = d->pad;
-  p.center = d->center;
-  p.pad_mode = d->pad_mode;
   p.n_mels = d->n_mels;
   p.stage = stage;
   p.log_mels = d->log_mels;
-  p.power = d->power;
   p.db_mult = d->db_multiplier;
   p.db_amin = d->db_amin;
   p.db_offset = d->db_offset;
   // bulk staging needs 16-byte aligned sources and sizes (every unit starts at a multiple of
   // frames_per_unit*hop, minus half + pad) and the unit's span must fit the staging buffer: the warp's mel region,
   // or the Spectrogram kernel's float2 transpose tile
-  const bool mel = stage >= B200A_STAGE_MEL;
   const int half = d->center ? d->n_fft / 2 : 0;
-  const int stage_floats = !mel    ? 2 * (32 / G) * (32 * (G + 1) + (G == 8 ? 8 : 0))
-                           : G == 8  ? Geo<8>::kMelRegion
-                           : G == 16 ? Geo<16>::kMelRegion
-                                     : Geo<32>::kMelRegion;
   p.bulk_ok = d->hop % 4 == 0 && (half + d->pad) % 4 == 0 && row_stride % 4 == 0 &&
               (reinterpret_cast<uintptr_t>(wave) & 15) == 0 &&
-              d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= stage_floats;
-  p.stage_ok = d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= stage_floats &&  // edge units gather into it
-               length + 2 * (int64_t)d->pad + d->n_fft < (int64_t)1 << 31;           // with 32-bit indices
+              d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= staging;
   p.out_width = stage >= B200A_STAGE_MEL ? d->n_mels : d->n_fft / 2 + 1;
   p.out_col0 = 0;
   p.k_energy_col = -1;
@@ -1746,18 +1735,14 @@ int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float*
   p.window = reinterpret_cast<const float*>(base + l.window);
   p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
   p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
-  const int sms = num_sms();
-  if (sms < 0) return B200A_ECUDA;
-  const int64_t iters = (p.total_units + kIsWarps - 1) / kIsWarps;
-  const unsigned grid = (unsigned)(iters < sms ? (iters < 1 ? 1 : iters) : sms);
-  auto launch = [&](auto kern, size_t smem) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) return (int)B200A_ECUDA;
-    kern<<<grid, kIsWarps * 32, smem, stream>>>(p);
-    return launch_status();
+  const int64_t grid = persistent_grid(p.total_units, kIsWarps);
+  auto launch_g = [&](auto g) {
+    constexpr int GG = decltype(g)::value;
+    return launch_kernel(istft_pow2_kernel<GG>, grid, kIsWarps * 32, istft_smem<GG>(), stream, p);
   };
-  if (G == 32) return launch(istft_pow2_kernel<32>, sizeof(float2) * (32 * 32 + kIsWarps * Geo<32>::kTileF2) + 4 * 1024);
-  if (G == 16) return launch(istft_pow2_kernel<16>, sizeof(float2) * (32 * 16 + kIsWarps * Geo<16>::kTileF2) + 4 * 512);
-  return launch(istft_pow2_kernel<8>, sizeof(float2) * (32 * 8 + kIsWarps * Geo<8>::kTileF2) + 4 * 256);
+  if (G == 32) return launch_g(std::integral_constant<int, 32>{});
+  if (G == 16) return launch_g(std::integral_constant<int, 16>{});
+  return launch_g(std::integral_constant<int, 8>{});
 }
 
 // Shared memory of the fused gradient kernel, 0 when the descriptor / stage does not take it.
@@ -1779,33 +1764,14 @@ int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int sta
   const size_t smem = backward_smem(d, stage);
   if (smem == 0) return B200A_EUNSUPPORTED;
   const WsLayout l = ws_layout(*d);
-  const Pow2Extra e = pow2_layout(*d, l.total);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   const int G = d->n_fft / 32;
-  const int frames_per_unit = 2 * (32 / G);
   BwdParams bp{};
-  Pow2Params& p = bp.f;
-  p.wave = wave;
-  p.length = length;
-  p.row_stride = row_stride;
-  p.frames = frames;
-  p.units_per_row = (frames + frames_per_unit - 1) / frames_per_unit;
-  p.total_units = rows * p.units_per_row;
-  p.window = reinterpret_cast<const float*>(base + l.window);
-  p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
-  p.hop = d->hop;
-  p.pad = d->pad;
-  p.center = d->center;
-  p.pad_mode = d->pad_mode;
-  p.n_mels = stage == B200A_STAGE_MEL ? d->n_mels : 0;
-  p.stage = stage;
-  p.power = d->power;
-  p.bulk_ok = 0;  // the transpose tile doubles as the inverse passes' tile, so nothing is staged into it ahead
-  // edge units gather their span into the tile (the Spectrogram kernel's float2 transpose tile) with 32-bit indices
-  const int stage_floats = 2 * (32 / G) * (32 * (G + 1) + (G == 8 ? 8 : 0));
-  p.stage_ok = d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= stage_floats &&
-               length + 2 * (int64_t)d->pad + d->n_fft < (int64_t)1 << 31;
+  // edge units gather their span into the Spectrogram kernel's float2 transpose tile; bulk_ok stays 0: the tile doubles
+  // as the inverse transform's, so nothing is staged into it ahead
+  bp.f = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, stage_floats(G, false));
+  bp.f.n_mels = stage == B200A_STAGE_MEL ? d->n_mels : 0;
+  bp.f.stage = stage;
   bp.grad = grad;
   bp.gs_row = gs_row;
   bp.gs_frame = gs_frame;
@@ -1813,22 +1779,13 @@ int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int sta
   bp.frame_buf = frame_buf;
   bp.fb = reinterpret_cast<const float*>(base + l.fb);
   bp.bands = reinterpret_cast<const int2*>(base + l.bands);
-  bp.stage = stage;
-  const int sms = num_sms();
-  if (sms < 0) return B200A_ECUDA;
-  const int64_t iters = (p.total_units + kBwWarps - 1) / kBwWarps;
-  const unsigned grid = (unsigned)(iters < sms ? (iters < 1 ? 1 : iters) : sms);
-  auto launch = [&](auto kern) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess)
-      return (int)B200A_ECUDA;
-    kern<<<grid, kBwWarps * 32, smem, stream>>>(bp);
-    return launch_status();
-  };
+  const int64_t grid = persistent_grid(bp.f.total_units, kBwWarps);
   auto by_stage = [&](auto g) {
     constexpr int GG = decltype(g)::value;
-    if (stage == B200A_STAGE_COMPLEX) return launch(stft_pow2_backward_kernel<GG, B200A_STAGE_COMPLEX>);
-    if (stage == B200A_STAGE_POWER) return launch(stft_pow2_backward_kernel<GG, B200A_STAGE_POWER>);
-    return launch(stft_pow2_backward_kernel<GG, B200A_STAGE_MEL>);
+    auto kern = stage == B200A_STAGE_COMPLEX ? stft_pow2_backward_kernel<GG, B200A_STAGE_COMPLEX>
+                : stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<GG, B200A_STAGE_POWER>
+                                             : stft_pow2_backward_kernel<GG, B200A_STAGE_MEL>;
+    return launch_kernel(kern, grid, kBwWarps * 32, smem, stream, bp);
   };
   if (G == 32) return by_stage(std::integral_constant<int, 32>{});
   if (G == 16) return by_stage(std::integral_constant<int, 16>{});
