@@ -106,6 +106,11 @@ _SIGNATURES = {
         [POINTER(FrontendDesc), c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int64,
          c_int64, c_int64, c_void_p],
     ),
+    "b200a_istft_backward": (
+        ctypes.c_int,
+        [POINTER(FrontendDesc), c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p],
+    ),
+    "b200a_istft_backward_scratch_bytes": (c_size_t, [POINTER(FrontendDesc), c_int64, c_int64]),
     "b200a_griffinlim_update": (
         ctypes.c_int,
         [c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p, c_void_p, c_float, c_int32, c_void_p, c_int64, c_int64, c_int64,

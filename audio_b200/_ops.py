@@ -1,5 +1,6 @@
 """``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
-capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``mfcc_finish`` / ``resample_run``.
+capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
+``resample_run``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -30,6 +31,9 @@ _LIB.define(
 _LIB.define(
     "frontend_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int stage, int row_stride, "
     "Tensor grad_out) -> Tensor"
+)
+_LIB.define(
+    "istft_backward(Tensor grad, Tensor workspace, int[] desc_i, float[] desc_f, int start, int frames) -> Tensor"
 )
 _LIB.define(
     "mfcc_finish(Tensor feat, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? group_max, int rows_per_group, "
@@ -119,6 +123,30 @@ def _frontend_backward_meta(wave, workspace, desc_i, desc_f, stage, row_stride, 
     return wave.new_empty(wave.shape, dtype=torch.float32)
 
 
+# ---- istft_backward ----------------------------------------------------------------------------------------------
+def _istft_backward_cuda(grad, workspace, desc_i, desc_f, start, frames):
+    """(rows, L) upstream gradient -> (rows, frames, n_fft//2+1, 2) frame-major spectrogram gradient."""
+    d = _unpack_desc(desc_i, desc_f)
+    if grad.shape[0] > 0 and grad.shape[1] > 0 and grad.stride(1) != 1:
+        grad = grad.contiguous()
+    rows, g_len = grad.shape
+    dev = grad.device
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, d.n_fft // 2 + 1, 2), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_istft_backward_scratch_bytes(d, rows, frames)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
+        rc = lib.b200a_istft_backward(
+            d, workspace.data_ptr(), grad.data_ptr(), rows, grad.stride(0) if rows > 1 else g_len, start, g_len, frames,
+            None if scratch is None else scratch.data_ptr(), out.data_ptr(), _stream(dev))
+    _lib.check(rc, "istft_backward")
+    return out
+
+
+def _istft_backward_meta(grad, workspace, desc_i, desc_f, start, frames):
+    return grad.new_empty((grad.shape[0], frames, int(desc_i[_DESC_INTS.index("n_fft")]) // 2 + 1, 2))
+
+
 # ---- mfcc_finish -------------------------------------------------------------------------------------------------
 def _mfcc_finish_cuda(feat, workspace, desc_i, desc_f, group_max, rows_per_group, top_db):
     d = _unpack_desc(desc_i, desc_f)
@@ -156,6 +184,7 @@ def _resample_run_meta(wave, workspace, kernel, orig_r, new_r, width, row_stride
 
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
+                            ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
                             ("mfcc_finish", _mfcc_finish_cuda, _mfcc_finish_meta),
                             ("resample_run", _resample_run_cuda, _resample_run_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
@@ -163,5 +192,6 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
 
 frontend_run = torch.ops.b200audio.frontend_run
 frontend_backward = torch.ops.b200audio.frontend_backward
+istft_backward = torch.ops.b200audio.istft_backward
 mfcc_finish = torch.ops.b200audio.mfcc_finish
 resample_run = torch.ops.b200audio.resample_run

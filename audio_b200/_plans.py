@@ -37,20 +37,28 @@ def is_differentiable() -> bool:
     return getattr(_GRAD_STATE, "on", False)
 
 
-def set_differentiable(mode: bool) -> None:
-    """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode)."""
+def is_inverse_differentiable() -> bool:
+    """Whether InverseSpectrogram and F.inverse_spectrogram accept spectrograms that require grad (in this thread)."""
+    return getattr(_GRAD_STATE, "inverse", False)
+
+
+def set_differentiable(mode: bool, *, inverse: bool = False) -> None:
+    """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
+    ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT; it is a separate
+    switch so that vocoder inference and augmentation code does not build graphs when loss gradients are on."""
     _GRAD_STATE.on = bool(mode)
+    _GRAD_STATE.inverse = bool(mode) and bool(inverse)
 
 
 @contextlib.contextmanager
-def differentiable(mode: bool = True):
-    """Context manager form of :func:`set_differentiable`; restores the previous setting on exit."""
-    prev = is_differentiable()
-    set_differentiable(mode)
+def differentiable(mode: bool = True, *, inverse: bool = False):
+    """Context manager form of :func:`set_differentiable`; restores the previous settings on exit."""
+    prev = is_differentiable(), is_inverse_differentiable()
+    set_differentiable(mode, inverse=inverse)
     try:
         yield
     finally:
-        set_differentiable(prev)
+        set_differentiable(prev[0], inverse=prev[1])
 
 
 def _no_autograd(t: torch.Tensor) -> None:
@@ -58,19 +66,20 @@ def _no_autograd(t: torch.Tensor) -> None:
         raise RuntimeError(
             "audio_b200 kernels are forward-only: the input requires grad. Call under torch.no_grad() / "
             "torch.inference_mode(), or detach() the input. (Spectrogram, MelSpectrogram and F.spectrogram compute "
-            "waveform gradients inside audio_b200.differentiable().)"
+            "waveform gradients inside audio_b200.differentiable(); InverseSpectrogram and F.inverse_spectrogram "
+            "compute spectrogram gradients inside audio_b200.differentiable(inverse=True).)"
         )
 
 
-def _wants_grad(waveform: torch.Tensor, constants) -> bool:
-    """True when the frontend output must carry a waveform gradient; raises for constant buffers that require grad,
-    whose gradients are not computed."""
-    if not (is_differentiable() and torch.is_grad_enabled()):
+def _wants_grad(waveform: torch.Tensor, constants, switch=is_differentiable, input_name: str = "waveform") -> bool:
+    """True when the output must carry a gradient of the input ``waveform`` and ``switch()`` is on; raises for
+    constant buffers that require grad, whose gradients are not computed."""
+    if not (switch() and torch.is_grad_enabled()):
         return False
     for name, t in constants:
         if t is not None and t.requires_grad:
             raise RuntimeError(
-                f"audio_b200: {name} requires grad, but only the waveform gradient is implemented; detach() it "
+                f"audio_b200: {name} requires grad, but only the {input_name} gradient is implemented; detach() it "
                 "or register it as a buffer"
             )
     return waveform.requires_grad

@@ -16,6 +16,9 @@ int griffinlim_update_impl(const float*, int64_t, int64_t, int64_t, float, const
 int istft_run_impl(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t, float*,
                    float*, int64_t, int64_t, int64_t, cudaStream_t);
 size_t frontend_backward_scratch(const b200a_frontend_desc*, int, int64_t, int64_t);
+size_t istft_backward_scratch(const b200a_frontend_desc*, int64_t, int64_t);
+int istft_backward_impl(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t,
+                        void*, float*, cudaStream_t);
 int frontend_backward_impl(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
                            const float*, int64_t, int64_t, int64_t, void*, float*, int64_t, cudaStream_t);
 int frontend_run_pow2(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
@@ -237,6 +240,25 @@ int b200a_istft_run(const b200a_frontend_desc* desc, const void* workspace, cons
   if (workspace == nullptr || spec == nullptr || frame_buf == nullptr || out == nullptr) return B200A_EINVAL;
   return istft_run_impl(desc, workspace, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, out,
                         out_row_stride, start, out_len, static_cast<cudaStream_t>(stream));
+}
+
+size_t b200a_istft_backward_scratch_bytes(const b200a_frontend_desc* desc, int64_t rows, int64_t frames) {
+  if (validate_desc(desc) != B200A_OK || !desc->onesided || rows < 0 || frames < 1) return 0;
+  return istft_backward_scratch(desc, rows, frames);
+}
+
+int b200a_istft_backward(const b200a_frontend_desc* desc, const void* workspace, const float* grad, int64_t rows,
+                         int64_t g_row_stride, int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec,
+                         b200a_stream stream) {
+  int rc = validate_desc(desc);
+  if (rc != B200A_OK) return rc;
+  if (!desc->onesided) return B200A_EUNSUPPORTED;
+  if (rows < 0 || frames < 1 || g_row_stride < 0 || start < 0 || g_len < 0) return B200A_EINVAL;
+  if (rows == 0) return B200A_OK;  // empty batch: nothing to enqueue (pointers may be null)
+  if (workspace == nullptr || grad == nullptr || grad_spec == nullptr) return B200A_EINVAL;
+  if (scratch == nullptr && istft_backward_scratch(desc, rows, frames) > 0) return B200A_EINVAL;
+  return istft_backward_impl(desc, workspace, grad, rows, g_row_stride, start, g_len, frames, scratch, grad_spec,
+                             static_cast<cudaStream_t>(stream));
 }
 
 int b200a_griffinlim_update(const float* mag, int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float inv_power,

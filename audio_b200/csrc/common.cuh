@@ -94,6 +94,20 @@ __device__ __forceinline__ float2 power_vjp(float re, float im, float p, float s
   return make_float2(re * c, im * c);
 }
 
+// The overlap-added squared window at sample s of an iSTFT of `frames` frames, formed exactly as istft_ola_kernel forms
+// it (float, fmaf, frames in ascending order); 0 where no frame covers s.
+__device__ __forceinline__ float istft_envelope(const float* window, int n_fft, int hop, int64_t frames, int64_t s) {
+  const int64_t t_lo = s - n_fft + 1 <= 0 ? 0 : (s - n_fft + hop) / hop;  // ceil((s - n_fft + 1) / hop)
+  int64_t t_hi = s / hop;
+  if (t_hi > frames - 1) t_hi = frames - 1;
+  float env = 0.f;
+  for (int64_t t = t_lo; t <= t_hi; ++t) {
+    const float w = window[s - t * hop];
+    env = fmaf(w, w, env);
+  }
+  return env;
+}
+
 // The filters [x, y) with a non-zero weight at bin k, from each filter's non-zero bin range bands[m] = [x, y); (0, 0)
 // when none is.
 __device__ __forceinline__ int2 filter_range(const int2* bands, int n_mels, int k) {

@@ -1081,6 +1081,83 @@ int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int sta
   return launch_status();
 }
 
+// ------------------------------------------------------------------------------------------
+// spectrogram gradient of the inverse STFT (b200a_istft_backward)
+//   g_hat[s] = g[s - start] / env[s] on the returned samples (0 elsewhere); the adjoint of the C2R frame stage and the
+//   overlap-add is grad_Z[t][k] = c_k / (N scale) * DFT(w * g_hat[t hop ..])[k], c_k = 2 but c_0 = c_{N/2} = 1.
+//   n_fft 256 / 512 / 1024: one kernel (frontend_pow2.cu).  Every other size: g_hat into scratch, the forward COMPLEX
+//   kernel with center = pad = 0 (which gives scale * DFT(w * frame)), then c_k / (N scale^2) per bin.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) istft_grad_prescale_kernel(const float* __restrict__ grad, int64_t g_row_stride,
+                                                                  int64_t start, int64_t g_len, const float* __restrict__ window,
+                                                                  int n_fft, int hop, int64_t frames, int64_t expected,
+                                                                  int64_t blocks_per_row, float* __restrict__ g_hat) {
+  const int64_t row = blockIdx.x / blocks_per_row;
+  const int64_t s = (blockIdx.x - row * blocks_per_row) * (int64_t)blockDim.x + threadIdx.x;
+  if (s >= expected) return;
+  const int64_t i = s - start;
+  float v = 0.f;
+  if (i >= 0 && i < g_len) {
+    const float env = istft_envelope(window, n_fft, hop, frames, s);
+    v = env > 0.f ? grad[row * g_row_stride + i] / env : 0.f;
+  }
+  g_hat[row * expected + s] = v;
+}
+
+__global__ void __launch_bounds__(256) istft_grad_scale_kernel(float2* __restrict__ spec, int64_t n, int n_fft, int n_bins,
+                                                               const WsHeader* __restrict__ hdr) {
+  const float scale = hdr->scale;
+  const float base = 1.f / ((float)n_fft * scale * scale);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int k = (int)(i % n_bins);
+    const float2 v = spec[i];
+    spec[i] = k == 0 || 2 * k == n_fft ? make_float2(base * v.x, 0.f) : make_float2(2.f * base * v.x, 2.f * base * v.y);
+  }
+}
+
+bool istft_backward_fused_applicable(const b200a_frontend_desc* d, int64_t frames);  // frontend_pow2.cu
+int istft_backward_pow2(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t,
+                        float*, cudaStream_t);
+
+size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames) {
+  if (istft_backward_fused_applicable(d, frames)) return 0;
+  return align_up(sizeof(float) * (size_t)rows * (size_t)(d->n_fft + (int64_t)d->hop * (frames - 1)), 256);
+}
+
+int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
+                        int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream) {
+  const int rc = istft_backward_pow2(d, ws, grad, rows, g_row_stride, start, g_len, frames, grad_spec, stream);
+  if (rc != B200A_EUNSUPPORTED) return rc;
+  const WsLayout l = ws_layout(*d);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const int64_t expected = d->n_fft + (int64_t)d->hop * (frames - 1);
+  float* g_hat = static_cast<float*>(scratch);
+  const int64_t bpr = (expected + 255) / 256;
+  if (rows * bpr > 0x7fffffffLL) return B200A_EUNSUPPORTED;
+  istft_grad_prescale_kernel<<<(unsigned)(rows * bpr), 256, 0, stream>>>(
+      grad, g_row_stride, start, g_len, reinterpret_cast<const float*>(base + l.window), d->n_fft, d->hop, frames, expected,
+      bpr, g_hat);
+  int r = launch_status();
+  if (r != B200A_OK) return r;
+  b200a_frontend_desc plain = *d;  // frames of g_hat from sample 0: no centre or constant padding
+  plain.center = 0;
+  plain.pad = 0;
+  r = frontend_run_pow2(&plain, ws, B200A_STAGE_COMPLEX, g_hat, rows, expected, expected, frames, grad_spec, nullptr, 1, stream,
+                        nullptr);
+  if (r == B200A_EUNSUPPORTED)
+    r = frontend_run_generic(&plain, ws, B200A_STAGE_COMPLEX, g_hat, rows, expected, expected, frames, grad_spec, nullptr, 1,
+                             stream, nullptr);
+  if (r != B200A_OK) return r;
+  const int n_bins = d->n_fft / 2 + 1;
+  const int64_t n = rows * frames * n_bins;
+  const int sms = device_sm_count();
+  if (sms < 0) return B200A_ECUDA;
+  const int64_t want = (n + 255) / 256;
+  istft_grad_scale_kernel<<<(unsigned)(want < 8 * (int64_t)sms ? want : 8 * (int64_t)sms), 256, 0, stream>>>(
+      reinterpret_cast<float2*>(grad_spec), n, d->n_fft, n_bins, reinterpret_cast<const WsHeader*>(base + l.header));
+  return launch_status();
+}
+
 int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* feat, int64_t rows,
                      int64_t frames, const float* group_max, int64_t rows_per_group, float top_db,
                      float* out, cudaStream_t stream) {

@@ -214,6 +214,8 @@ struct Pow2Params {
   int kaldi, k_off, k_win, k_dc, k_energy_mode, k_energy_col, k_log;
   float k_preemph, k_energy_floor;
   float power, db_mult, db_amin, db_offset;
+  // iSTFT adjoint (kIstftGrad): frames [env_t_lo, env_t_hi] have the full window envelope at every sample
+  int64_t env_t_lo, env_t_hi;
 };
 
 // samples before t * hop where frame t starts: n_fft/2 (torch.stft center), 0, or Kaldi's win/2 - shift/2
@@ -223,6 +225,9 @@ __device__ __forceinline__ int frame_lead(const Pow2Params& p, int n_fft) {
 
 constexpr int kComplexOut = 3;  // POWER_MODE of the complex (power = None) Spectrogram kernel
 constexpr int kSpectra = 4;     // POWER_MODE of the gradient kernel: transform_unit returns the two complex spectra
+// POWER_MODE of the iSTFT adjoint (b200a_istft_backward): the COMPLEX Spectrogram kernel over the upstream gradient g,
+// staged as g / env (env: the overlap-added squared window), with c_k / (N scale) in place of scale
+constexpr int kIstftGrad = 5;
 
 template <int POWER_MODE>  // 2: |.|^2, 0: general exponent (1 handled inside)
 __device__ __forceinline__ float pow_of(float re, float im, float power) {
@@ -298,12 +303,15 @@ struct UnitCursor {
   }
 };
 
-// a unit can be staged by one bulk copy iff all its frames exist and lie inside the row un-padded
-template <int G>
+// a unit can be staged by one bulk copy iff all its frames exist and lie inside the row un-padded (ADJ: and have the
+// full window envelope, so that the staged samples need no division)
+template <int G, bool ADJ = false>
 __device__ __forceinline__ bool bulk_eligible(const Pow2Params& p, int half, int64_t u, int64_t ub) {
   using Ge = Geo<G>;
   if (!p.bulk_ok || u >= p.total_units) return false;
   const int64_t t0 = ub * Ge::kFrames;
+  if constexpr (ADJ)
+    if (t0 < p.env_t_lo || t0 + Ge::kFrames - 1 > p.env_t_hi) return false;
   const int64_t s0 = t0 * p.hop - half - p.pad;
   return t0 + Ge::kFrames <= p.frames && s0 >= 0 && s0 + (int64_t)(Ge::kFrames - 1) * p.hop + Ge::kNfft <= p.length;
 }
@@ -425,6 +433,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
                                                const UnitCursor& cur, int half, int lane, PT (&pa)[17],
                                                PT (&pb)[17]) {
   using Ge = Geo<G>;
+  constexpr bool ADJ = POWER_MODE == kIstftGrad;
   float* stage = reinterpret_cast<float*>(tile);
   const int gi = lane / G, l = lane % G;
   const int64_t row = cur.row, t0 = cur.ub * Ge::kFrames;
@@ -433,10 +442,15 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
   const float* __restrict__ x = p.wave + row * p.row_stride;
   const int64_t s0 = t0 * p.hop - half - p.pad;  // first raw sample of the unit
   const int64_t sa = s0 + (int64_t)2 * gi * p.hop, sb = sa + p.hop;
-  const bool next_staged = bulk_eligible<G>(p, half, cur.u + cur.stride, cur.nub);
+  const bool next_staged = bulk_eligible<G, ADJ>(p, half, cur.u + cur.stride, cur.nub);
   // every frame of the unit inside the signal: plain loads; otherwise the padding-aware gather
   const int64_t last = p.frames - t0 < Ge::kFrames ? p.frames - t0 : Ge::kFrames;  // frames present
   const bool interior = s0 >= 0 && s0 + (last - 1) * p.hop + Ge::kNfft <= p.length;
+  // ADJ: a unit that is gathered (a sample short of the full window envelope, or outside g) divides by env in the
+  // gather and takes the plain window table; every other unit takes the table with 1/env folded in (s_win + n_fft)
+  bool env_edge = false;
+  if constexpr (ADJ) env_edge = t0 < p.env_t_lo || t0 + last - 1 > p.env_t_hi;
+  const float* win = ADJ && interior && !env_edge ? s_win + Ge::kNfft : s_win;
 
   float2 a[32];
   float* grp_f = stage + gi * (SPLIT ? Ge::kRegionF : 2 * Ge::kRegion);  // the lane group's region as floats
@@ -444,7 +458,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
   if (staged) {
     mbar_wait(bar, parity);
     parity ^= 1;
-  } else if ((!interior || KALDI) && p.stage_ok) {
+  } else if ((!interior || KALDI || env_edge) && p.stage_ok) {
     // edge unit (padding / reflection / ragged end): the lanes gather the unit's whole span into the (idle)
     // staging buffer with 4-byte asynchronous copies -- every sample once, all copies in flight together --
     // and the unit then takes the same register-load path as a bulk-staged one
@@ -452,6 +466,18 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
     // 32-bit index arithmetic (the launch guarantees length + 2 pad + n_fft < 2^31): j indexes the constant
     // pre-padded signal of `ext` samples, exactly as source_index() does in 64 bits
     const int len = (int)p.length, ext = len + 2 * p.pad, j0 = (int)(t0 * p.hop) - half, mode = p.pad_mode;
+    if constexpr (ADJ) {  // constant padding, half = 0: sample n of the span is output sample s = j0 + n of the iSTFT
+#pragma unroll 4
+      for (int n = lane; n < span; n += 32) {
+        const int src = j0 + n - p.pad;
+        float v = 0.f;
+        if ((unsigned)src < (unsigned)len) {
+          const float env = istft_envelope(p.window, Ge::kNfft, p.hop, p.frames, j0 + n);
+          v = env > 0.f ? __fdividef(__ldg(x + src), env) : 0.f;  // no IEEE-division slow path: 2 ulp
+        }
+        stage[n] = v;
+      }
+    } else {
 #pragma unroll 4
     for (int n = lane; n < span; n += 32) {
       int j = j0 + n;
@@ -475,6 +501,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
         stage[n] = 0.f;
     }
     cp_async_wait_all();
+    }
     __syncwarp();
     from_stage = true;
   }
@@ -549,7 +576,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       });
       static_for<32>([&](auto ji) {
         constexpr int j = decltype(ji)::value;
-        const float w = s_win[lane + 32 * j];
+        const float w = win[lane + 32 * j];
         a[brev5(j)] = make_float2(v[j] * w, v[j + (HG >= 0 ? HG : 0)] * w);
       });
     } else {
@@ -557,7 +584,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       const float* pb_ptr = pa_ptr + p.hop;
       static_for<32>([&](auto ji) {
         constexpr int j = decltype(ji)::value;
-        a[brev5(j)] = scale2(s_win[l + G * j], make_float2(pa_ptr[G * j], pb_ptr[G * j]));
+        a[brev5(j)] = scale2(win[l + G * j], make_float2(pa_ptr[G * j], pb_ptr[G * j]));
       });
     }
     __syncwarp();  // every lane has consumed the staging buffer
@@ -566,9 +593,9 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       constexpr int j = decltype(ji)::value;
       const float va = has_a ? __ldg(x + sa + l + G * j) : 0.f;
       const float vb = has_b ? __ldg(x + sb + l + G * j) : 0.f;
-      a[brev5(j)] = scale2(s_win[l + G * j], make_float2(va, vb));
+      a[brev5(j)] = scale2(win[l + G * j], make_float2(va, vb));
     });
-  } else {
+  } else if constexpr (!ADJ) {  // (the adjoint launches only with stage_ok)
     // edge unit whose span does not fit the staging buffer: gather frame a, then frame b, through the group's region
     // (n_fft floats) with a rolled loop so the index arithmetic is not replicated 64 times in the instruction stream
 #pragma unroll
@@ -625,6 +652,11 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       float2* oc = reinterpret_cast<float2*>(p.out) + (row * p.frames + ta) * Ge::kBins + l + G * m;
       if (has_a) oc[0] = make_float2(sx.x, sy.x);
       if (has_b) oc[Ge::kBins] = make_float2(sy.y, -sx.y);
+    } else if constexpr (ADJ) {  // c_k = 2 at bins 1 .. N/2 - 1 (the window table carries the 1/2 of c_0 = 1)
+      const float c = m == 0 && l == 0 ? 1.f : 2.f;
+      float2* oc = reinterpret_cast<float2*>(p.out) + (row * p.frames + ta) * Ge::kBins + l + G * m;
+      if (has_a) oc[0] = make_float2(c * sx.x, c * sy.x);
+      if (has_b) oc[Ge::kBins] = make_float2(c * sy.y, -c * sx.y);
     } else if constexpr (POWER_MODE == kSpectra) {
       pa[m] = make_float2(sx.x, sy.x);
       pb[m] = make_float2(sy.y, -sx.y);
@@ -639,7 +671,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
   });
   // bin N/2 (l == 0, m = 16) is its own mirror: A = Re, B = Im  (x2 because wreg carries the 1/2)
   constexpr int slot16 = (16 % NG) * G + 16 / NG;
-  if constexpr (POWER_MODE == kComplexOut) {
+  if constexpr (POWER_MODE == kComplexOut || ADJ) {  // ADJ: c_{N/2} = 1
     if (l == 0) {
       float2* oc = reinterpret_cast<float2*>(p.out) + (row * p.frames + ta) * Ge::kBins + Ge::kNfft / 2;
       if (has_a) oc[0] = make_float2(2.f * a[slot16].x, 0.f);
@@ -662,15 +694,28 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   using Ge = Geo<G>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float2* s_tw = reinterpret_cast<float2*>(smem_raw);                                    // [32][G]
-  float* s_win = reinterpret_cast<float*>(s_tw + 32 * 32);                               // [n_fft]
-  float2* s_tile_all = reinterpret_cast<float2*>(s_win + Ge::kNfft);                     // [NW][kTileF2] (also staging)
+  constexpr bool ADJ = POWER_MODE == kIstftGrad;
+  float* s_win = reinterpret_cast<float*>(s_tw + 32 * 32);                               // [n_fft] (ADJ: [2][n_fft])
+  float2* s_tile_all = reinterpret_cast<float2*>(s_win + (ADJ ? 2 : 1) * Ge::kNfft);     // [NW][kTileF2] (also staging)
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_tile_all + NW * Ge::kTileF2);          // [NW]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // the tables of load_fft_tables, written out: through the helper the n_fft = 1024 general-power variant spills more
   for (int i = tid; i < 32 * G; i += blockDim.x) s_tw[i] = p.tw2d[i];
-  const float hs = 0.5f * p.hdr->scale;  // the window x 1/2 (un-packing) x scale
-  for (int i = tid; i < Ge::kNfft; i += blockDim.x) s_win[i] = p.window[i] * hs;
+  if constexpr (ADJ) {
+    // the window x 1/2 / (N scale), and the same over the full envelope at sample i (period hop), 0 where that is 0
+    const float hs = 0.5f / ((float)Ge::kNfft * p.hdr->scale);
+    for (int i = tid; i < Ge::kNfft; i += blockDim.x) {
+      const float w = p.window[i] * hs;
+      const int r = i % p.hop;
+      const float env = istft_envelope(p.window, Ge::kNfft, p.hop, p.frames, r + (Ge::kNfft - 1 - r) / p.hop * p.hop);
+      s_win[i] = w;
+      s_win[Ge::kNfft + i] = env > 0.f ? __fdividef(w, env) : 0.f;
+    }
+  } else {
+    const float hs = 0.5f * p.hdr->scale;  // the window x 1/2 (un-packing) x scale
+    for (int i = tid; i < Ge::kNfft; i += blockDim.x) s_win[i] = p.window[i] * hs;
+  }
   if (tid < NW) mbar_init(s_bar + tid, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   __syncthreads();
@@ -684,14 +729,14 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
   bool staged = false;
   UnitCursor cur;
   cur.init((int64_t)blockIdx.x * NW + warp, (int64_t)gridDim.x * NW, p.units_per_row);
-  if (bulk_eligible<G>(p, half, cur.u, cur.ub)) {
+  if (bulk_eligible<G, ADJ>(p, half, cur.u, cur.ub)) {
     if (lane == 0) issue_bulk<G>(p, half, cur.row, cur.ub, stage, bar);
     staged = true;
   }
   for (; cur.u < p.total_units; cur.advance()) {
     float pa[17], pb[17];
     transform_unit<POWER_MODE, G, HG, KALDI, false>(p, s_win, s_tw, tile, bar, parity, staged, cur, half, lane, pa, pb);
-    if constexpr (POWER_MODE == kComplexOut) continue;  // transform_unit has written the complex spectra
+    if constexpr (POWER_MODE == kComplexOut || ADJ) continue;  // transform_unit has written the complex spectra
     const int64_t ta = cur.ub * Ge::kFrames + 2 * gi;
     const bool has_a = ta < p.frames, has_b = ta + 1 < p.frames;
     float* oa = p.out + (cur.row * p.frames + ta) * p.out_width + p.out_col0;
@@ -1555,9 +1600,10 @@ static int launch_power(const Pow2Params& p, cudaStream_t stream) {
   // the transform is latency bound: as many warps as shared memory (one tile each, also the staging buffer) and the
   // register file (168 registers at 12 warps, no spills) allow
   constexpr int NW = 16;
-  const size_t smem = sizeof(float2) * (32 * 32 + NW * Ge::kTileF2) + sizeof(float) * Ge::kNfft + sizeof(uint64_t) * NW;
+  const size_t smem = sizeof(float2) * (32 * 32 + NW * Ge::kTileF2) +
+                      sizeof(float) * Ge::kNfft * (POWER_MODE == kIstftGrad ? 2 : 1) + sizeof(uint64_t) * NW;
   auto kern = stft_pow2_power_kernel<POWER_MODE, G, HG, NW, false>;
-  if constexpr (POWER_MODE != kComplexOut)
+  if constexpr (POWER_MODE != kComplexOut && POWER_MODE != kIstftGrad)
     if (p.kaldi) kern = stft_pow2_power_kernel<POWER_MODE, G, -1, NW, true>;
   return launch_kernel(kern, persistent_grid(p.total_units, NW), NW * 32, smem, stream, p);
 }
@@ -1576,7 +1622,7 @@ static int launch_mel(const Pow2Params& p, cudaStream_t stream) {
 
 template <int POWER_MODE, int G>
 static int launch_g(const Pow2Params& p, bool mel, cudaStream_t stream) {
-  if constexpr (POWER_MODE == kComplexOut) {  // complex spectra: only the Spectrogram kernel
+  if constexpr (POWER_MODE == kComplexOut || POWER_MODE == kIstftGrad) {  // complex spectra: only the Spectrogram kernel
     if constexpr (G == 32)
       if (p.bulk_ok && p.hop == 256) return launch_power<POWER_MODE, 32, 8>(p, stream);
     return launch_power<POWER_MODE, G, -1>(p, stream);
@@ -1790,6 +1836,43 @@ int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int sta
   if (G == 32) return by_stage(std::integral_constant<int, 32>{});
   if (G == 16) return by_stage(std::integral_constant<int, 16>{});
   return by_stage(std::integral_constant<int, 8>{});
+}
+
+// The iSTFT adjoint runs on the register FFT when n_fft is 256 / 512 / 1024 (one-sided), an edge unit's span fits the
+// Spectrogram kernel's staging tile (hop <= ~n_fft) and the frames' samples index with 32 bits.
+bool istft_backward_fused_applicable(const b200a_frontend_desc* d, int64_t frames) {
+  if (!pow2_applicable(*d) || d->n_fft > 1024) return false;
+  const int G = d->n_fft / 32;
+  const int64_t span = d->n_fft + (2 * (32 / G) - 1) * (int64_t)d->hop;
+  return span <= stage_floats(G, false) && d->n_fft + (int64_t)d->hop * (frames - 1) + 2 * d->n_fft < (int64_t)1 << 31;
+}
+
+// b200a_istft_backward for n_fft = 256 / 512 / 1024: the COMPLEX Spectrogram kernel in its kIstftGrad variant over g,
+// framed with a lead of `start` samples and constant padding, straight into grad_spec.
+int istft_backward_pow2(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
+                        int64_t start, int64_t g_len, int64_t frames, float* grad_spec, cudaStream_t stream) {
+  if (!istft_backward_fused_applicable(d, frames)) return B200A_EUNSUPPORTED;
+  const int G = d->n_fft / 32;
+  const int frames_per_unit = 2 * (32 / G);
+  const int staging = stage_floats(G, false);
+  // samples at or past expected = n_fft + hop (frames - 1) get no gradient: clamp so that every index fits 32 bits
+  const int64_t expected = d->n_fft + (int64_t)d->hop * (frames - 1);
+  const int64_t lead = start < expected ? start : expected;
+  const int64_t len = g_len < expected - lead ? g_len : expected - lead;
+  Pow2Params p = pow2_geometry(*d, ws, grad, rows, len, g_row_stride, frames, staging);
+  p.center = 0;
+  p.pad = (int)lead;
+  p.pad_mode = B200A_PAD_CONSTANT;
+  p.stage_ok = 1;
+  p.out = grad_spec;
+  p.bulk_ok = d->hop % 4 == 0 && lead % 4 == 0 && g_row_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(grad) & 15) == 0 &&
+              d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= staging;
+  const int64_t cover = (d->n_fft + d->hop - 1) / d->hop;  // frames overlapping one sample, at most
+  p.env_t_lo = cover - 1;
+  p.env_t_hi = frames - cover;
+  if (G == 32) return launch_g<kIstftGrad, 32>(p, false, stream);
+  if (G == 16) return launch_g<kIstftGrad, 16>(p, false, stream);
+  return launch_g<kIstftGrad, 8>(p, false, stream);
 }
 
 }  // namespace b200a

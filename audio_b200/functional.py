@@ -8,7 +8,8 @@ private helpers ``transforms`` imports (``_get_sinc_resample_kernel`` 1305-1402,
 ``_apply_sinc_resample_kernel`` 1405-1432).
 
 Differences, all explicit (never a silent fallback): CUDA float32 tensors only, forward only except the waveform
-gradient of ``spectrogram`` (and of the MelSpectrogram path) inside ``audio_b200.differentiable()``.
+gradient of ``spectrogram`` (and of the MelSpectrogram path) inside ``audio_b200.differentiable()`` and the spectrogram
+gradient of ``inverse_spectrogram`` inside ``audio_b200.differentiable(inverse=True)``.
 """
 from __future__ import annotations
 
@@ -20,10 +21,13 @@ from typing import Optional, Union
 import torch
 from torch import Tensor
 
-from . import _lib
+from torch.autograd.function import once_differentiable
+
+from . import _lib, _ops
 from ._bookkeeping import resample_ratio
 from ._constants import create_dct, linear_fbanks, melscale_fbanks, sinc_resample_kernel
-from ._plans import FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, new_group_max
+from ._plans import (FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad,
+                     is_inverse_differentiable, new_group_max)
 
 __all__ = [
     "spectrogram",
@@ -167,13 +171,14 @@ def inverse_spectrogram(
         raise TypeError(f"audio_b200: spectrogram must be complex64 (got {spectrogram.dtype})")
     if not onesided:
         raise NotImplementedError("audio_b200: inverse_spectrogram(onesided=False) is not implemented")
-    _no_autograd(spectrogram)
+    grad = _wants_grad(spectrogram, (("window", window),), is_inverse_differentiable, "spectrogram")
+    if not grad:
+        _no_autograd(spectrogram)
     shape = spectrogram.size()
     n_bins, frames = shape[-2], shape[-1]
     if n_bins != n_fft // 2 + 1:
         raise RuntimeError(f"istft: expected {n_fft // 2 + 1} frequency bins for n_fft={n_fft}, got {n_bins}")
     spec3 = spectrogram.reshape(-1, n_bins, frames)
-    rows = spec3.shape[0]
     desc = FrontendPlan.make_desc(n_fft, win_length, hop_length, 0, center, "reflect", True, fl_norm, win_norm, 2.0)
     plan = _plan_for(desc, spectrogram.device)
     ws = plan.workspace(window, None, None)
@@ -189,19 +194,46 @@ def inverse_spectrogram(
     if start + out_len > expected:
         warnings.warn("The length of signal is shorter than the length parameter. Result is being padded with zeros in "
                       "the tail. Please check your center and hop_length settings.")
-    dev = spectrogram.device
+    cut = pad if length is not None and pad > 0 else 0
+    if grad:
+        out = _IstftFunction.apply(spec3, ws, desc, start, out_len, cut)
+    else:
+        out = _istft_run(spec3, ws, desc, start, out_len, cut)
+    return out.reshape(shape[:-2] + out.shape[-1:])
+
+
+def _istft_run(spec3: Tensor, ws: Tensor, desc, start: int, out_len: int, cut: int) -> Tensor:
+    """b200a_istft_run on the packed (rows, bins, frames) spectrogram: samples [start, start + out_len) of the
+    overlap-added signal, less ``cut`` samples at each end."""
+    rows, _, frames = spec3.shape
+    dev = spec3.device
     real = torch.view_as_real(spec3)  # (rows, bins, frames, 2) float32 view, same storage
     with torch.cuda.device(dev):
-        frame_buf = torch.empty((rows, frames, n_fft), dtype=torch.float32, device=dev)
+        frame_buf = torch.empty((rows, frames, desc.n_fft), dtype=torch.float32, device=dev)
         out = torch.empty((rows, out_len), dtype=torch.float32, device=dev)
         rc = _lib.lib().b200a_istft_run(
             desc, ws.data_ptr(), real.data_ptr(), rows, frames, spec3.stride(0), spec3.stride(1), spec3.stride(2),
             frame_buf.data_ptr(), out.data_ptr(), out_len, start, out_len, _stream_ptr(dev),
         )
     _lib.check(rc, "istft_run")
-    if length is not None and pad > 0:
-        out = out[:, pad:-pad]
-    return out.reshape(shape[:-2] + out.shape[-1:])
+    return out[:, cut:-cut] if cut > 0 else out
+
+
+class _IstftFunction(torch.autograd.Function):
+    """_istft_run with b200audio::istft_backward as its backward.  The map is linear, so nothing is saved but the
+    forward's workspace: a window edited before backward does not change the gradient.  The ``cut`` slice happens
+    inside, so autograd adds no slice_backward fill of the full-length gradient."""
+
+    @staticmethod
+    def forward(ctx, spec3, ws, desc, start, out_len, cut):
+        ctx.ws, ctx.desc_lists, ctx.start, ctx.frames = ws, _ops.pack_desc(desc), start + cut, spec3.shape[2]
+        return _istft_run(spec3, ws, desc, start, out_len, cut)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        gz = _ops.istft_backward(g, ctx.ws, *ctx.desc_lists, ctx.start, ctx.frames)  # (rows, frames, bins, 2)
+        return torch.view_as_complex(gz).transpose(1, 2), None, None, None, None, None
 
 
 def griffinlim(

@@ -216,6 +216,28 @@ int b200a_istft_run(const b200a_frontend_desc* desc, const void* workspace, cons
                     b200a_stream stream);
 
 /*
+ * Spectrogram gradient of b200a_istft_run (the backward of torch.istft as F.inverse_spectrogram calls it), with the
+ * workspace the forward ran with.  With X = scale * DFT(w * frame) the forward normalisation, N = n_fft,
+ * env[s] = sum_t w^2[s - t hop] and g the upstream gradient of the returned samples:
+ *   g_hat[s] = g[s - start] / env[s] for start <= s < start + g_len and s < N + hop (frames - 1), else 0;
+ *   grad_spec[t][k] = c_k / (N scale) * sum_n w[n] g_hat[t hop + n] e^(-2 pi i k n / N),
+ *   c_0 = 1, c_{N/2} = 1 (even N), c_k = 2 otherwise: the imaginary parts at bins 0 and N/2 are exactly 0
+ * (torch's complex-gradient convention dL/dRe + i dL/dIm).  `start` counts the returned signal's offset in the
+ * overlap-added one: n_fft/2 when centred, plus the `pad` F.inverse_spectrogram slices off.
+ *   grad      : [rows] rows of g_len floats, row r at grad + r * g_row_stride (0 allowed: expanded gradients)
+ *   scratch   : caller-owned device memory of b200a_istft_backward_scratch_bytes(desc, rows, frames) bytes (NULL when 0)
+ *   grad_spec : complex64, frame-major [rows][frames][n_fft/2+1] (every element written)
+ * Deterministic: no atomics, every row independent of the others.  onesided descriptors only; any n_fft (one kernel for
+ * 256 / 512 / 1024 with hop <= ~n_fft, three for every other size).
+ */
+int b200a_istft_backward(const b200a_frontend_desc* desc, const void* workspace, const float* grad, int64_t rows,
+                         int64_t g_row_stride, int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec,
+                         b200a_stream stream);
+/* Bytes of scratch b200a_istft_backward needs: 0 on the register-FFT path, rows * (N + hop (frames - 1)) floats of g_hat
+ * otherwise; also 0 for an invalid request (which b200a_istft_backward then rejects). */
+size_t b200a_istft_backward_scratch_bytes(const b200a_frontend_desc* desc, int64_t rows, int64_t frames);
+
+/*
  * One phase step of F.griffinlim (functional/functional.py:330-341):
  *   proj = mag^inv_power * angles,  angles = d / (|d| + 1e-16),  d = rebuilt - momentum * tprev
  * with angles = 1 when rebuilt is NULL (the first inversion, rand_init = False), d = rebuilt when tprev is NULL, and

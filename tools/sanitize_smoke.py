@@ -25,6 +25,10 @@ with audio_b200.differentiable():  # waveform gradients: the fused path (512 / 1
                 T.Spectrogram(n_fft=400, power=None, onesided=False)):
         xg = x.clone().requires_grad_()
         mod.cuda()(xg).abs().sum().backward()
+with audio_b200.differentiable(inverse=True):  # spectrogram gradients: fused (256 / 1024), composition (400 / 2048)
+    for n_fft, pad in ((256, 0), (1024, 5), (400, 3), (2048, 0)):
+        spec = T.Spectrogram(n_fft=n_fft, hop_length=n_fft // 4, power=None).cuda()(x).requires_grad_()
+        T.InverseSpectrogram(n_fft=n_fft, hop_length=n_fft // 4, pad=pad).cuda()(spec, 11000).sum().backward()
 T.MFCC(16000, n_mfcc=13, melkwargs=dict(n_fft=512, hop_length=160, n_mels=40)).cuda()(x)
 T.MFCC(16000, n_mfcc=40, melkwargs=dict(n_fft=1024, hop_length=256, n_mels=80)).cuda()(x.reshape(1, 3, -1))
 for kw in (dict(num_mel_bins=40, snip_edges=False, use_energy=True), dict(num_mel_bins=23), dict(frame_length=20.0, round_to_power_of_two=False)):
