@@ -3,42 +3,6 @@
 
 #include "common.cuh"
 
-namespace b200a {
-int validate_desc(const b200a_frontend_desc* d);
-int frontend_prepare_impl(const b200a_frontend_desc*, const float*, const float*, const float*, void*, size_t, cudaStream_t);
-int frontend_run_generic(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
-                         float*, float*, int64_t, cudaStream_t, const b200a_kaldi_desc* = nullptr);
-int subtract_column_mean_impl(float*, int64_t, int64_t, int64_t, cudaStream_t);
-int phase_vocoder_impl(const float*, int64_t, int64_t, int64_t, int64_t, int64_t, int64_t, double, const float*, float*, int64_t,
-                       cudaStream_t);
-int griffinlim_update_impl(const float*, int64_t, int64_t, int64_t, float, const float*, const float*, float, int, float*,
-                           int64_t, int64_t, int64_t, cudaStream_t);
-int istft_run_impl(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t, float*,
-                   float*, int64_t, int64_t, int64_t, cudaStream_t);
-size_t frontend_backward_scratch(const b200a_frontend_desc*, int, int64_t, int64_t);
-size_t istft_backward_scratch(const b200a_frontend_desc*, int64_t, int64_t);
-int istft_backward_impl(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t,
-                        void*, float*, cudaStream_t);
-int frontend_backward_impl(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
-                           const float*, int64_t, int64_t, int64_t, void*, float*, int64_t, cudaStream_t);
-int frontend_run_pow2(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
-                      float*, float*, int64_t, cudaStream_t,
-                      const b200a_kaldi_desc* = nullptr);  // returns B200A_EUNSUPPORTED when not applicable
-size_t pow2_workspace_extra(const b200a_frontend_desc*);
-int pow2_prepare(const b200a_frontend_desc*, void*, size_t, cudaStream_t);
-int mfcc_finish_impl(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, const float*, int64_t, float,
-                     float*, cudaStream_t);
-int fill_impl(float*, int64_t, float, cudaStream_t);
-int ratio_impl(const float*, int64_t, float*, cudaStream_t);
-int apply_fbank_impl(const float*, int64_t, int64_t, int64_t, int64_t, int64_t, int64_t, const float*, int, float*,
-                     cudaStream_t);
-int amplitude_to_db_impl(const float*, int64_t, int64_t, float, float, float, float, float*, float*, cudaStream_t);
-size_t resample_workspace_bytes_impl(int, int);
-int resample_prepare_impl(const float*, int, int, int, void*, size_t, cudaStream_t);
-int resample_run_impl(const void*, const float*, int, int, int, const float*, int64_t, int64_t, int64_t, float*, int64_t,
-                      int64_t, cudaStream_t);
-}  // namespace b200a
-
 using namespace b200a;
 
 #pragma GCC visibility push(default)
@@ -130,17 +94,13 @@ int b200a_frontend_prepare(const b200a_frontend_desc* desc, const float* window,
   return pow2_prepare(desc, workspace, workspace_bytes, s);
 }
 
-int b200a_frontend_run(const b200a_frontend_desc* desc, const void* workspace, int32_t stage, const float* wave,
-                       int64_t rows, int64_t length, int64_t row_stride, float* out, float* group_max,
-                       int64_t rows_per_group, b200a_stream stream) {
-  int rc = validate_desc(desc);
-  if (rc != B200A_OK) return rc;
-  if (rows == 0) return B200A_OK;  // empty batch: nothing to enqueue (pointers may be null)
-  if (workspace == nullptr || wave == nullptr || out == nullptr) return B200A_EINVAL;
-  if (rows < 0 || length < 0 || row_stride < length) return B200A_EINVAL;
+// Checks of a forward or backward call on a valid descriptor that read no pointer: stage, power, rows, length and the
+// padding torch accepts.  The frame count on success, else a negative status.
+static int64_t frontend_frames(const b200a_frontend_desc* desc, int32_t stage, int64_t rows, int64_t length) {
   if (stage < B200A_STAGE_COMPLEX || stage > B200A_STAGE_FEAT) return B200A_EINVAL;
   if (stage >= B200A_STAGE_MEL && desc->n_mels <= 0) return B200A_EINVAL;
   if (stage != B200A_STAGE_COMPLEX && !(desc->power > 0.f)) return B200A_EINVAL;
+  if (rows < 0 || length < 0) return B200A_EINVAL;
   const int64_t ext = length + 2 * (int64_t)desc->pad;
   if (desc->center && (desc->pad_mode == B200A_PAD_REFLECT || desc->pad_mode == B200A_PAD_CIRCULAR)) {
     // torch: "Padding size should be less than the corresponding input dimension" (reflect needs
@@ -149,36 +109,24 @@ int b200a_frontend_run(const b200a_frontend_desc* desc, const void* workspace, i
     if (desc->pad_mode == B200A_PAD_REFLECT ? half >= ext : half > ext) return B200A_ESHORT;
   }
   const int64_t frames = b200a_num_frames(length, desc->n_fft, desc->hop, desc->center, desc->pad);
-  if (frames < 1) return B200A_ESHORT;
-  if (rows == 0) return B200A_OK;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  rc = frontend_run_pow2(desc, workspace, stage, wave, rows, length, row_stride, frames, out, group_max,
-                         rows_per_group, s);
-  if (rc != B200A_EUNSUPPORTED) return rc;
-  return frontend_run_generic(desc, workspace, stage, wave, rows, length, row_stride, frames, out, group_max,
-                              rows_per_group, s);
-}
-
-// Shared checks of the backward entry points; the frame count on success, else a negative status.
-static int64_t backward_frames(const b200a_frontend_desc* desc, int32_t stage, int64_t rows, int64_t length) {
-  int rc = validate_desc(desc);
-  if (rc != B200A_OK) return rc;
-  if (stage < B200A_STAGE_COMPLEX || stage > B200A_STAGE_FEAT) return B200A_EINVAL;
-  if (stage == B200A_STAGE_FEAT) return B200A_EUNSUPPORTED;
-  if (stage == B200A_STAGE_MEL && desc->n_mels <= 0) return B200A_EINVAL;
-  if (stage != B200A_STAGE_COMPLEX && !(desc->power > 0.f)) return B200A_EINVAL;
-  if (rows < 0 || length < 0) return B200A_EINVAL;
-  const int64_t ext = length + 2 * (int64_t)desc->pad;
-  if (desc->center && (desc->pad_mode == B200A_PAD_REFLECT || desc->pad_mode == B200A_PAD_CIRCULAR)) {
-    const int64_t half = desc->n_fft / 2;
-    if (desc->pad_mode == B200A_PAD_REFLECT ? half >= ext : half > ext) return B200A_ESHORT;
-  }
-  const int64_t frames = b200a_num_frames(length, desc->n_fft, desc->hop, desc->center, desc->pad);
   return frames < 1 ? (int64_t)B200A_ESHORT : frames;
 }
 
+int b200a_frontend_run(const b200a_frontend_desc* desc, const void* workspace, int32_t stage, const float* wave,
+                       int64_t rows, int64_t length, int64_t row_stride, float* out, float* group_max,
+                       int64_t rows_per_group, b200a_stream stream) {
+  const int rc = validate_desc(desc);
+  if (rc != B200A_OK || rows == 0) return rc;  // empty batch: nothing to enqueue (pointers may be null)
+  if (workspace == nullptr || wave == nullptr || out == nullptr || row_stride < length) return B200A_EINVAL;
+  const int64_t frames = frontend_frames(desc, stage, rows, length);
+  if (frames < 1) return (int)frames;
+  return frontend_run_impl(desc, workspace, stage, wave, rows, length, row_stride, frames, out, group_max, rows_per_group,
+                           static_cast<cudaStream_t>(stream), nullptr);
+}
+
 size_t b200a_frontend_backward_scratch_bytes(const b200a_frontend_desc* desc, int32_t stage, int64_t rows, int64_t length) {
-  const int64_t frames = backward_frames(desc, stage, rows, length);
+  if (validate_desc(desc) != B200A_OK || stage == B200A_STAGE_FEAT) return 0;
+  const int64_t frames = frontend_frames(desc, stage, rows, length);
   if (frames < 1) return 0;
   return frontend_backward_scratch(desc, stage, rows, frames);
 }
@@ -194,8 +142,8 @@ int b200a_frontend_backward(const b200a_frontend_desc* desc, const void* workspa
   if (rows == 0) return B200A_OK;  // empty batch: nothing to enqueue (pointers may be null)
   if (workspace == nullptr || wave == nullptr || grad_out == nullptr || scratch == nullptr || grad_wave == nullptr)
     return B200A_EINVAL;
-  if (rows < 0 || length < 0 || row_stride < length || grad_row_stride < length) return B200A_EINVAL;
-  const int64_t frames = backward_frames(desc, stage, rows, length);
+  if (row_stride < length || grad_row_stride < length) return B200A_EINVAL;
+  const int64_t frames = frontend_frames(desc, stage, rows, length);
   if (frames < 1) return (int)frames;
   return frontend_backward_impl(desc, workspace, stage, wave, rows, length, row_stride, frames, grad_out, g_stride_row,
                                 g_stride_frame, g_stride_col, scratch, grad_wave, grad_row_stride,
@@ -313,10 +261,8 @@ int b200a_kaldi_run(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* de
   if (length < kaldi->window_size) return B200A_ESHORT;  // kaldi.py:142-144
   const int64_t frames = b200a_kaldi_num_frames(length, kaldi->window_size, kaldi->window_shift, kaldi->snip_edges);
   if (frames < 1) return B200A_ESHORT;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  rc = frontend_run_pow2(desc, workspace, stage, wave, rows, length, row_stride, frames, out, nullptr, 1, s, kaldi);
-  if (rc != B200A_EUNSUPPORTED) return rc;
-  return frontend_run_generic(desc, workspace, stage, wave, rows, length, row_stride, frames, out, nullptr, 1, s, kaldi);
+  return frontend_run_impl(desc, workspace, stage, wave, rows, length, row_stride, frames, out, nullptr, 1,
+                           static_cast<cudaStream_t>(stream), kaldi);
 }
 
 int b200a_subtract_column_mean(float* x, int64_t rows, int64_t frames, int64_t width, b200a_stream stream) {

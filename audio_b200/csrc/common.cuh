@@ -52,16 +52,105 @@ inline WsLayout ws_layout(const b200a_frontend_desc& d) {
   return l;
 }
 
-// SMs of the current device (persistent grids are sized to one wave of it); -1 if the query fails
-inline int device_sm_count() {
-  int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-      n <= 0)
+constexpr int kSmemLimit = 227 * 1024;  // dynamic shared memory per CTA on sm_90
+
+// Returned by a register-FFT entry point whose path does not take the call: its dispatcher runs the shared-memory
+// Stockham path instead.  Never leaves the library (every public status is <= 0).
+constexpr int kPathDeclined = 1;
+
+// min(blocks, per_sm * SMs of the current device), the grid of a kernel that grid-strides over `blocks` CTAs' worth of
+// work; -1 if the SM count cannot be read
+inline int64_t sm_capped_grid(int64_t blocks, int per_sm) {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      sms <= 0)
     return -1;
-  return n;
+  return blocks < (int64_t)per_sm * sms ? blocks : (int64_t)per_sm * sms;
+}
+
+// persistent: one resident CTA per SM, units dealt round-robin (every CTA gets the same count +-1); -1 when the SM
+// count cannot be read
+inline int64_t persistent_grid(int64_t total_units, int warps) {
+  const int64_t grid = sm_capped_grid((total_units + warps - 1) / warps, 1);
+  return grid == 0 ? 1 : grid;
 }
 
 inline int launch_status() { return cudaGetLastError() == cudaSuccess ? B200A_OK : B200A_ECUDA; }
+
+// Raises the kernel's dynamic shared-memory limit to kSmemLimit and launches it on `grid` CTAs (grid < 0: the
+// sm_capped_grid error).  The limit is a cap, not a carve-out: the launch still reserves only `smem`.
+template <typename Kernel, typename... Args>
+int launch_kernel(Kernel kern, int64_t grid, int threads, size_t smem, cudaStream_t stream, const Args&... args) {
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess || grid < 0)
+    return B200A_ECUDA;
+  kern<<<(unsigned)grid, threads, smem, stream>>>(args...);
+  return launch_status();
+}
+
+// ---- host functions shared across csrc/ -----------------------------------------------------
+// frontend_generic.cu
+int validate_desc(const b200a_frontend_desc* d);
+int frontend_prepare_impl(const b200a_frontend_desc* d, const float* window, const float* fb, const float* dct, void* ws,
+                          size_t ws_bytes, cudaStream_t stream);
+// The forward front end: the register-FFT kernels when they take the call, the Stockham kernel otherwise.  kd: Kaldi
+// framing and conditioning, or null.
+int frontend_run_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                      int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
+                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd);
+int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
+                   int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, float* out,
+                   int64_t out_row_stride, int64_t start, int64_t out_len, cudaStream_t stream);
+size_t frontend_backward_scratch(const b200a_frontend_desc* d, int stage, int64_t rows, int64_t frames);
+int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                           int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
+                           int64_t gs_frame, int64_t gs_col, void* scratch, float* grad_wave, int64_t grad_row_stride,
+                           cudaStream_t stream);
+size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
+int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
+                        int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);
+int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* feat, int64_t rows, int64_t frames,
+                     const float* group_max, int64_t rows_per_group, float top_db, float* out, cudaStream_t stream);
+
+// frontend_pow2.cu: the register-FFT path.  frontend_run_pow2, istft_frames_pow2 and istft_backward_pow2 return
+// kPathDeclined when it does not take the call.
+size_t pow2_workspace_extra(const b200a_frontend_desc* d);
+int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaStream_t stream);
+int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                      int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
+                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd);
+int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
+                      int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, cudaStream_t stream);
+bool backward_fused_applicable(const b200a_frontend_desc* d, int stage);
+int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                           int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
+                           int64_t gs_frame, int64_t gs_col, float* frame_buf, cudaStream_t stream);
+bool istft_backward_fused_applicable(const b200a_frontend_desc* d, int64_t frames);
+int istft_backward_pow2(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
+                        int64_t start, int64_t g_len, int64_t frames, float* grad_spec, cudaStream_t stream);
+
+// standalone.cu
+int fill_impl(float* dst, int64_t n, float v, cudaStream_t stream);
+int ratio_impl(const float* pairs, int64_t n, float* out, cudaStream_t stream);
+int apply_fbank_impl(const float* spec, int64_t rows, int64_t n_bins, int64_t frames, int64_t stride_row,
+                     int64_t stride_bin, int64_t stride_frame, const float* fb, int n_filters, float* out,
+                     cudaStream_t stream);
+int amplitude_to_db_impl(const float* x, int64_t groups, int64_t group_elems, float mult, float amin, float offset,
+                         float top_db, float* scratch, float* out, cudaStream_t stream);
+int subtract_column_mean_impl(float* x, int64_t rows, int64_t frames, int64_t width, cudaStream_t stream);
+int griffinlim_update_impl(const float* mag, int64_t ms_row, int64_t ms_bin, int64_t ms_frame, float inv_power,
+                           const float* rebuilt, const float* tprev, float momentum, int normalize, float* proj,
+                           int64_t rows, int64_t bins, int64_t frames, cudaStream_t stream);
+int phase_vocoder_impl(const float* spec, int64_t s_row, int64_t s_bin, int64_t s_frame, int64_t rows, int64_t bins,
+                       int64_t frames_in, double rate, const float* phase_advance, float* out, int64_t frames_out,
+                       cudaStream_t stream);
+
+// resample.cu
+size_t resample_workspace_bytes_impl(int new_r, int taps);
+int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width, void* ws, size_t ws_bytes,
+                          cudaStream_t stream);
+int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r, int width, const float* wave,
+                      int64_t rows, int64_t length, int64_t row_stride, float* out, int64_t out_row_stride,
+                      int64_t out_len, cudaStream_t stream);
 
 // ---- device helpers -----------------------------------------------------------------------
 // Index into the raw waveform row for sample i of the (constant `pad`-extended, then centre

@@ -670,10 +670,26 @@ int frontend_prepare_impl(const b200a_frontend_desc* d, const float* window, con
   return launch_status();
 }
 
-int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave,
-                         int64_t rows, int64_t length, int64_t row_stride, int64_t frames, float* out,
-                         float* group_max, int64_t rows_per_group, cudaStream_t stream,
-                         const b200a_kaldi_desc* kd) {
+// Launches a Stockham kernel (stft_generic_kernel or istft_frames_kernel) over `frames` frames of each of `rows` rows:
+// 2 * pairs frames per CTA, enough work for 256 threads with at most ~48 KB of ping-pong buffers.
+template <typename Params>
+static int launch_stockham(void (*kern)(Params), Params p, int64_t rows, int64_t frames, cudaStream_t stream) {
+  int pairs = (int)(49152 / (16 * (size_t)p.n_fft));
+  if (pairs < 1) pairs = 1;
+  if (pairs > 8) pairs = 8;
+  while (pairs > 1 && (int64_t)2 * (pairs - 1) >= frames) --pairs;
+  p.pairs = pairs;
+  p.tiles_per_row = (frames + 2 * pairs - 1) / (2 * pairs);
+  const size_t smem = sizeof(float2) * (size_t)p.n_fft * (2 * pairs + 1);
+  static_assert(kMaxFft * 8 * 3 <= kSmemLimit, "largest FFT must fit in shared memory");
+  const int64_t grid = rows * p.tiles_per_row;
+  if (grid <= 0 || grid > 0x7fffffffLL) return B200A_EUNSUPPORTED;
+  return launch_kernel(kern, grid, 256, smem, stream, p);
+}
+
+static int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                                int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
+                                int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd) {
   const WsLayout l = ws_layout(*d);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   GenericParams p{};
@@ -685,7 +701,7 @@ int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, int stage
   p.frames = frames;
   p.out = out;
   p.group_max = group_max;
-  p.rows_per_group = rows_per_group > 0 ? rows_per_group : 1;
+  p.rows_per_group = rows_per_group;
   p.window = reinterpret_cast<const float*>(base + l.window);
   p.twiddle = reinterpret_cast<const float2*>(base + l.twiddle);
   p.bands = reinterpret_cast<const int2*>(base + l.bands);
@@ -720,21 +736,18 @@ int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, int stage
     p.out_width = kd->out_width;
     p.out_col0 = kd->out_col0;
   }
-  // frames per CTA: enough work for 256 threads, at most ~48 KB of ping-pong buffers
-  int pairs = (int)(49152 / (16 * (size_t)d->n_fft));
-  if (pairs < 1) pairs = 1;
-  if (pairs > 8) pairs = 8;
-  while (pairs > 1 && (int64_t)2 * (pairs - 1) >= frames) --pairs;
-  p.pairs = pairs;
-  p.tiles_per_row = (frames + 2 * pairs - 1) / (2 * pairs);
-  const size_t smem = sizeof(float2) * (size_t)d->n_fft * (2 * pairs + 1);
-  static_assert(kMaxFft * 8 * 3 <= 227 * 1024, "largest FFT must fit in shared memory");
-  if (cudaFuncSetAttribute(stft_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-    return B200A_ECUDA;
-  const int64_t grid = rows * p.tiles_per_row;
-  if (grid <= 0 || grid > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  stft_generic_kernel<<<(unsigned)grid, 256, smem, stream>>>(p);
-  return launch_status();
+  return launch_stockham(stft_generic_kernel, p, rows, frames, stream);
+}
+
+int frontend_run_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                      int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
+                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd) {
+  if (rows_per_group < 1) rows_per_group = 1;
+  const int rc = frontend_run_pow2(d, ws, stage, wave, rows, length, row_stride, frames, out, group_max, rows_per_group,
+                                   stream, kd);
+  if (rc != kPathDeclined) return rc;
+  return frontend_run_generic(d, ws, stage, wave, rows, length, row_stride, frames, out, group_max, rows_per_group, stream,
+                              kd);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -819,9 +832,6 @@ __global__ void __launch_bounds__(256) istft_ola_kernel(const float* __restrict_
   out[row * out_row_stride + sp] = t_hi >= t_lo ? acc / env : 0.f;
 }
 
-int istft_frames_pow2(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t, float*,
-                      cudaStream_t);  // frontend_pow2.cu; B200A_EUNSUPPORTED when the size is not 256 / 512 / 1024
-
 // First half of b200a_istft_run: the windowed time frames w * irfft(spec) / scale of every frame into frame_buf, on the
 // register FFT for n_fft = 256 / 512 / 1024 (onesided descriptors) and the shared-memory Stockham FFT otherwise.  Any
 // n_fft works, odd ones included (bins (N+1)/2 .. N-1 are the Hermitian mirror of 1 .. (N-1)/2): torch.istft's
@@ -830,7 +840,7 @@ static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const
                              int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf,
                              cudaStream_t stream) {
   const int rc = istft_frames_pow2(d, ws, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, stream);
-  if (rc != B200A_EUNSUPPORTED) return rc;
+  if (rc != kPathDeclined) return rc;
   // any other size: shared-memory Stockham
   const WsLayout l = ws_layout(*d);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
@@ -847,19 +857,7 @@ static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const
   p.twiddle = reinterpret_cast<const float2*>(base + l.twiddle);
   p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
   p.n_fft = d->n_fft;
-  int pairs = (int)(49152 / (16 * (size_t)d->n_fft));
-  if (pairs < 1) pairs = 1;
-  if (pairs > 8) pairs = 8;
-  while (pairs > 1 && (int64_t)2 * (pairs - 1) >= frames) --pairs;
-  p.pairs = pairs;
-  p.tiles_per_row = (frames + 2 * pairs - 1) / (2 * pairs);
-  const size_t smem = sizeof(float2) * (size_t)d->n_fft * (2 * pairs + 1);
-  if (cudaFuncSetAttribute(istft_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-    return B200A_ECUDA;
-  const int64_t grid = rows * p.tiles_per_row;
-  if (grid <= 0 || grid > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  istft_frames_kernel<<<(unsigned)grid, 256, smem, stream>>>(p);
-  return launch_status();
+  return launch_stockham(istft_frames_kernel, p, rows, frames, stream);
 }
 
 int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
@@ -998,13 +996,6 @@ __global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict
   grad[row * grad_row_stride + s] = acc;
 }
 
-// frontend_pow2.cu
-int frontend_run_pow2(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t, float*,
-                      float*, int64_t, cudaStream_t, const b200a_kaldi_desc*);
-bool backward_fused_applicable(const b200a_frontend_desc* d, int stage);
-int frontend_backward_pow2(const b200a_frontend_desc*, const void*, int, const float*, int64_t, int64_t, int64_t, int64_t,
-                           const float*, int64_t, int64_t, int64_t, float*, cudaStream_t);
-
 size_t frontend_backward_scratch(const b200a_frontend_desc* d, int stage, int64_t rows, int64_t frames) {
   const size_t n = (size_t)rows * (size_t)frames;
   const size_t frame_bytes = align_up(sizeof(float) * n * d->n_fft, 256);
@@ -1035,11 +1026,8 @@ int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int sta
     frame_buf = reinterpret_cast<float*>(sc + align_up(sizeof(float2) * (size_t)n * n_bins, 256));
     bad = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(frame_buf) + align_up(sizeof(float) * (size_t)n * d->n_fft, 256));
     float* spec_f = reinterpret_cast<float*>(spec);
-    rc = frontend_run_pow2(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames, spec_f, nullptr, 1, stream,
+    rc = frontend_run_impl(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames, spec_f, nullptr, 1, stream,
                            nullptr);
-    if (rc == B200A_EUNSUPPORTED)
-      rc = frontend_run_generic(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames, spec_f, nullptr, 1, stream,
-                                nullptr);
     if (rc != B200A_OK) return rc;
     SpecVjpParams p{};
     p.spec = spec;
@@ -1058,16 +1046,8 @@ int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int sta
     p.n_mels = d->n_mels;
     p.stage = stage;
     p.power = d->power;
-    const int sms = device_sm_count();
-    if (sms < 0) return B200A_ECUDA;
-    const int64_t want = (n + 7) / 8;
-    const unsigned grid = (unsigned)(want < 8 * (int64_t)sms ? want : 8 * (int64_t)sms);
     const size_t smem = stage == B200A_STAGE_MEL ? sizeof(int2) * n_bins : 0;
-    if (smem > 48 * 1024 &&
-        cudaFuncSetAttribute(spec_vjp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-      return B200A_ECUDA;
-    spec_vjp_kernel<<<grid, 256, smem, stream>>>(p);
-    rc = launch_status();
+    rc = launch_kernel(spec_vjp_kernel, sm_capped_grid((n + 7) / 8, 8), 256, smem, stream, p);
     if (rc != B200A_OK) return rc;
     rc = istft_frames_impl(d, ws, spec_f, rows, frames, frames * n_bins, 1, n_bins, frame_buf, stream);
   }
@@ -1115,10 +1095,6 @@ __global__ void __launch_bounds__(256) istft_grad_scale_kernel(float2* __restric
   }
 }
 
-bool istft_backward_fused_applicable(const b200a_frontend_desc* d, int64_t frames);  // frontend_pow2.cu
-int istft_backward_pow2(const b200a_frontend_desc*, const void*, const float*, int64_t, int64_t, int64_t, int64_t, int64_t,
-                        float*, cudaStream_t);
-
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames) {
   if (istft_backward_fused_applicable(d, frames)) return 0;
   return align_up(sizeof(float) * (size_t)rows * (size_t)(d->n_fft + (int64_t)d->hop * (frames - 1)), 256);
@@ -1127,7 +1103,7 @@ size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream) {
   const int rc = istft_backward_pow2(d, ws, grad, rows, g_row_stride, start, g_len, frames, grad_spec, stream);
-  if (rc != B200A_EUNSUPPORTED) return rc;
+  if (rc != kPathDeclined) return rc;
   const WsLayout l = ws_layout(*d);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   const int64_t expected = d->n_fft + (int64_t)d->hop * (frames - 1);
@@ -1142,18 +1118,14 @@ int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const floa
   b200a_frontend_desc plain = *d;  // frames of g_hat from sample 0: no centre or constant padding
   plain.center = 0;
   plain.pad = 0;
-  r = frontend_run_pow2(&plain, ws, B200A_STAGE_COMPLEX, g_hat, rows, expected, expected, frames, grad_spec, nullptr, 1, stream,
+  r = frontend_run_impl(&plain, ws, B200A_STAGE_COMPLEX, g_hat, rows, expected, expected, frames, grad_spec, nullptr, 1, stream,
                         nullptr);
-  if (r == B200A_EUNSUPPORTED)
-    r = frontend_run_generic(&plain, ws, B200A_STAGE_COMPLEX, g_hat, rows, expected, expected, frames, grad_spec, nullptr, 1,
-                             stream, nullptr);
   if (r != B200A_OK) return r;
   const int n_bins = d->n_fft / 2 + 1;
   const int64_t n = rows * frames * n_bins;
-  const int sms = device_sm_count();
-  if (sms < 0) return B200A_ECUDA;
-  const int64_t want = (n + 255) / 256;
-  istft_grad_scale_kernel<<<(unsigned)(want < 8 * (int64_t)sms ? want : 8 * (int64_t)sms), 256, 0, stream>>>(
+  const int64_t grid = sm_capped_grid((n + 255) / 256, 8);
+  if (grid < 0) return B200A_ECUDA;
+  istft_grad_scale_kernel<<<(unsigned)grid, 256, 0, stream>>>(
       reinterpret_cast<float2*>(grad_spec), n, d->n_fft, n_bins, reinterpret_cast<const WsHeader*>(base + l.header));
   return launch_status();
 }
@@ -1165,20 +1137,15 @@ int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* 
   const float* dct = reinterpret_cast<const float*>(static_cast<const unsigned char*>(ws) + l.dct);
   const int64_t total = rows * frames;
   if (total == 0) return B200A_OK;
+  if (rows_per_group < 1) rows_per_group = 1;
   if (d->n_mfcc <= 64 && group_max != nullptr && top_db >= 0.f) {  // dB path: tensor-pipe kernel
     const int ksteps = (d->n_mels + 7) / 8, ntiles = (d->n_mfcc + 7) / 8;
     const size_t msmem = sizeof(float4) * (size_t)ksteps * ntiles * 32 + sizeof(float) * ((size_t)kMmaFinRows * (8 * ksteps + 4) + kMmaFinRows);
     if (msmem <= 200 * 1024) {
-      if (cudaFuncSetAttribute(mfcc_finish_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
-        return B200A_ECUDA;
       const int64_t tiles = (total + kMmaFinRows - 1) / kMmaFinRows;
       const int per_sm = msmem <= 72 * 1024 ? 3 : (msmem <= 110 * 1024 ? 2 : 1);
-      const int sms = device_sm_count();
-      if (sms < 0) return B200A_ECUDA;
-      const int64_t grid = tiles < (int64_t)sms * per_sm ? tiles : (int64_t)sms * per_sm;
-      mfcc_finish_mma_kernel<<<(unsigned)grid, 256, msmem, stream>>>(feat, total, frames, d->n_mels, d->n_mfcc, dct, group_max,
-                                                                   rows_per_group > 0 ? rows_per_group : 1, top_db, out);
-      return launch_status();
+      return launch_kernel(mfcc_finish_mma_kernel, sm_capped_grid(tiles, per_sm), 256, msmem, stream, feat, total, frames,
+                           d->n_mels, d->n_mfcc, dct, group_max, rows_per_group, top_db, out);
     }
   }
   if (d->n_mfcc <= 64) {  // register-tiled persistent kernel
@@ -1186,26 +1153,17 @@ int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* 
     const size_t tsmem = sizeof(float) * ((size_t)d->n_mels * 8 * cpt + (size_t)kFinRows * (d->n_mels + 2));
     if (tsmem <= 200 * 1024) {
       auto kern = cpt == 5 ? mfcc_finish_tiled_kernel<5> : mfcc_finish_tiled_kernel<8>;
-      if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
-        return B200A_ECUDA;
       const int64_t tiles = (total + kFinRows - 1) / kFinRows;
-      const int sms = device_sm_count();
-      if (sms < 0) return B200A_ECUDA;
-      const int64_t grid = tiles < (int64_t)sms * 4 ? tiles : (int64_t)sms * 4;
-      kern<<<(unsigned)grid, 256, tsmem, stream>>>(feat, total, frames, d->n_mels, d->n_mfcc, dct, group_max,
-                                                   rows_per_group > 0 ? rows_per_group : 1, top_db, out);
-      return launch_status();
+      return launch_kernel(kern, sm_capped_grid(tiles, 4), 256, tsmem, stream, feat, total, frames, d->n_mels, d->n_mfcc, dct,
+                           group_max, rows_per_group, top_db, out);
     }
   }
   const size_t smem = sizeof(float) * ((size_t)d->n_mels * d->n_mfcc + (size_t)kDctRowsPerBlock * (d->n_mels + 1));
   if (smem > 200 * 1024) return B200A_EUNSUPPORTED;
-  if (cudaFuncSetAttribute(mfcc_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
-    return B200A_ECUDA;
   const int64_t grid = (total + kDctRowsPerBlock - 1) / kDctRowsPerBlock;
   if (grid > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  mfcc_finish_kernel<<<(unsigned)grid, 256, smem, stream>>>(feat, total, frames, d->n_mels, d->n_mfcc, dct, group_max,
-                                                            rows_per_group > 0 ? rows_per_group : 1, top_db, out);
-  return launch_status();
+  return launch_kernel(mfcc_finish_kernel, grid, 256, smem, stream, feat, total, frames, d->n_mels, d->n_mfcc, dct, group_max,
+                       rows_per_group, top_db, out);
 }
 
 }  // namespace b200a

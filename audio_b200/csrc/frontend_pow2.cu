@@ -43,7 +43,6 @@ constexpr int kMaxItemsPerWarp = 32;
 constexpr int kMaxMTiles = 8;  // 16-frame MMA tiles per iteration of the 16-warp mel kernel (n_fft = 256: 128 frames)
 constexpr int kFragSmemSteps = 112;  // filterbank fragments kept in shared memory (x 512 B)
 constexpr int kMaxSlots = 128;
-constexpr int kSmemLimit = 227 * 1024;  // dynamic shared memory per CTA on sm_90
 
 // Geometry of one transform size: G lanes per frame pair.
 template <int G>
@@ -1549,6 +1548,28 @@ static_assert(kMaxItemsPerWarp * kMelWarps >= kMaxItems,
 
 }  // namespace
 
+// The register FFT's lanes per frame pair G (n_fft = 2048 runs on the 1024-point complex core) and frames per unit,
+// Geo<G>::kFrames.
+static int fft_g(int n_fft) { return n_fft == 2048 ? 32 : n_fft / 32; }
+static int unit_frames(int n_fft) { return 2 * (32 / fft_g(n_fft)); }
+
+// f(std::integral_constant<int, G>{}) with the G of n_fft
+template <typename F>
+static auto with_g(int n_fft, F&& f) {
+  switch (fft_g(n_fft)) {
+    case 8: return f(std::integral_constant<int, 8>{});
+    case 16: return f(std::integral_constant<int, 16>{});
+    default: return f(std::integral_constant<int, 32>{});
+  }
+}
+
+// The bulk copies stage 16-byte aligned spans of whole 16-byte words: the source, its row stride, the hop and the lead
+// (samples a row's first frame starts before sample 0; every unit starts at a multiple of frames-per-unit * hop minus
+// the lead) are multiples of 4 floats.
+static bool bulk_aligned(int hop, int64_t lead, int64_t row_stride, const float* src) {
+  return hop % 4 == 0 && lead % 4 == 0 && row_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
+}
+
 size_t pow2_workspace_extra(const b200a_frontend_desc* d) {
   if (!pow2_applicable(*d)) return 0;
   const size_t base = ws_layout(*d).total;
@@ -1561,11 +1582,11 @@ int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaSt
   const Pow2Extra e = pow2_layout(*d, l.total);
   if (ws_bytes < e.total) return B200A_EWORKSPACE;
   unsigned char* base = static_cast<unsigned char*>(ws);
-  const int G = d->n_fft == 2048 ? 32 : d->n_fft / 32;  // 2048 runs on the 1024-point complex core
+  const int G = fft_g(d->n_fft);
   prepare_tw2d_kernel<<<(32 * G + 255) / 256, 256, 0, stream>>>(reinterpret_cast<float2*>(base + e.tw2d), G);
   if (d->n_fft == 2048) prepare_tw_eo_kernel<<<3, 256, 0, stream>>>(reinterpret_cast<float2*>(base + e.tw_eo));
   if (d->n_mels > 0 && mel_tiles(d->n_mels) <= kMaxItems) {
-    const int n_mtiles = d->n_fft == 2048 ? 0 : kUniWarps * 2 * (32 / G) / 16;  // Geo<G>::kMTiles
+    const int n_mtiles = d->n_fft == 2048 ? 0 : kUniWarps * unit_frames(d->n_fft) / 16;  // Geo<G>::kMTiles
     prepare_mma_kernel<<<1, 256, 0, stream>>>(reinterpret_cast<const float*>(base + l.fb),
                                               reinterpret_cast<const int2*>(base + l.bands), d->n_fft / 2 + 1, d->n_mels,
                                               mel_tiles(d->n_mels), n_mtiles, reinterpret_cast<MelPlan*>(base + e.plan),
@@ -1574,31 +1595,11 @@ int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaSt
   return launch_status();
 }
 
-// persistent: one resident CTA per SM, units dealt round-robin (every CTA gets the same count +-1); -1 when the SM
-// count cannot be read
-static int64_t persistent_grid(int64_t total_units, int warps) {
-  const int sms = device_sm_count();
-  if (sms < 0) return -1;
-  const int64_t iters = (total_units + warps - 1) / warps;
-  const int64_t grid = iters < sms ? iters : sms;
-  return grid < 1 ? 1 : grid;
-}
-
-// Raises the kernel's dynamic shared-memory limit to kSmemLimit and launches it on `grid` CTAs (grid < 0: the
-// persistent_grid error).
-template <typename Kernel, typename... Args>
-static int launch_kernel(Kernel kern, int64_t grid, int threads, size_t smem, cudaStream_t stream, const Args&... args) {
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess || grid < 0)
-    return B200A_ECUDA;
-  kern<<<(unsigned)grid, threads, smem, stream>>>(args...);
-  return launch_status();
-}
-
 template <int POWER_MODE, int G, int HG>
 static int launch_power(const Pow2Params& p, cudaStream_t stream) {
   using Ge = Geo<G>;
   // the transform is latency bound: as many warps as shared memory (one tile each, also the staging buffer) and the
-  // register file (168 registers at 12 warps, no spills) allow
+  // register file (at 16 warps, 128 registers a thread) allow
   constexpr int NW = 16;
   const size_t smem = sizeof(float2) * (32 * 32 + NW * Ge::kTileF2) +
                       sizeof(float) * Ge::kNfft * (POWER_MODE == kIstftGrad ? 2 : 1) + sizeof(uint64_t) * NW;
@@ -1636,13 +1637,6 @@ static int launch_g(const Pow2Params& p, bool mel, cudaStream_t stream) {
 }
 
 template <int POWER_MODE>
-static int launch_any(Pow2Params& p, int n_fft, bool mel, cudaStream_t stream) {
-  if (n_fft == 1024) return launch_g<POWER_MODE, 32>(p, mel, stream);
-  if (n_fft == 512) return launch_g<POWER_MODE, 16>(p, mel, stream);
-  return launch_g<POWER_MODE, 8>(p, mel, stream);
-}
-
-template <int POWER_MODE>
 static int launch_eo(const Pow2Params& p, const float2* tw_eo, bool mel, cudaStream_t stream) {
   const int64_t grid = persistent_grid(p.total_units, kWarps);
   const size_t tables = sizeof(float2) * (1024 + 1024 + 17 * 32 + kWarps * 32 * 33);
@@ -1651,15 +1645,17 @@ static int launch_eo(const Pow2Params& p, const float2* tw_eo, bool mel, cudaStr
                          p, tw_eo);
   const size_t smem = tables + sizeof(float) * kEoSlots * kEoPitch + sizeof(int64_t) * 2 * kEoSlots +
                       sizeof(uint64_t) * (kWarps + 2) + sizeof(MelPlan) + sizeof(float4) * 32 * kEoFragSteps;
-  if (smem > kSmemLimit) return B200A_EUNSUPPORTED;
+  if (smem > kSmemLimit) return kPathDeclined;
   return launch_kernel(stft2048_mel_kernel<POWER_MODE>, grid, (kWarps + kMelWarps) * 32, smem, stream, p, tw_eo);
 }
 
 // floats of a warp's staging region: the mel kernel's region, or the float2 transpose tile of the Spectrogram and
 // gradient kernels
-static int stage_floats(int G, bool mel) {
-  if (mel) return G == 8 ? Geo<8>::kMelRegion : G == 16 ? Geo<16>::kMelRegion : Geo<32>::kMelRegion;
-  return 2 * (G == 8 ? Geo<8>::kTileF2 : G == 16 ? Geo<16>::kTileF2 : Geo<32>::kTileF2);
+static int stage_floats(int n_fft, bool mel) {
+  return with_g(n_fft, [&](auto g) {
+    using Ge = Geo<decltype(g)::value>;
+    return mel ? Ge::kMelRegion : 2 * Ge::kTileF2;
+  });
 }
 
 // The Pow2Params fields the forward and the gradient kernels fill alike: the waveform and its framing, the window,
@@ -1670,8 +1666,7 @@ static Pow2Params pow2_geometry(const b200a_frontend_desc& d, const void* ws, co
   const WsLayout l = ws_layout(d);
   const Pow2Extra e = pow2_layout(d, l.total);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
-  const int G = d.n_fft == 2048 ? 32 : d.n_fft / 32;
-  const int frames_per_unit = 2 * (32 / G);
+  const int frames_per_unit = unit_frames(d.n_fft);
   Pow2Params p{};
   p.wave = wave;
   p.length = length;
@@ -1695,22 +1690,20 @@ static Pow2Params pow2_geometry(const b200a_frontend_desc& d, const void* ws, co
 int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                       int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
                       int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd) {
-  if (!pow2_applicable(*d)) return B200A_EUNSUPPORTED;
-  if (stage == B200A_STAGE_COMPLEX && (d->n_fft > 1024 || kd != nullptr)) return B200A_EUNSUPPORTED;
+  if (!pow2_applicable(*d)) return kPathDeclined;
+  if (stage == B200A_STAGE_COMPLEX && (d->n_fft > 1024 || kd != nullptr)) return kPathDeclined;
   // Kaldi features with a 256 / 512 / 1024-point FFT; every other size takes the generic kernel
-  if (kd != nullptr && d->n_fft > 1024) return B200A_EUNSUPPORTED;
-  if (stage >= B200A_STAGE_MEL && mel_tiles(d->n_mels) > kMaxItems) return B200A_EUNSUPPORTED;  // > 512 filters
+  if (kd != nullptr && d->n_fft > 1024) return kPathDeclined;
+  if (stage >= B200A_STAGE_MEL && mel_tiles(d->n_mels) > kMaxItems) return kPathDeclined;  // > 512 filters
   const Pow2Extra e = pow2_layout(*d, ws_layout(*d).total);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   const bool eo = d->n_fft == 2048;
-  const int G = eo ? 32 : d->n_fft / 32;
-  const int frames_per_unit = 2 * (32 / G);
   const bool mel = stage >= B200A_STAGE_MEL;
-  const int staging = stage_floats(G, mel);
+  const int staging = stage_floats(d->n_fft, mel);
   Pow2Params p = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, staging);
   p.out = out;
   p.group_max = group_max;
-  p.rows_per_group = rows_per_group > 0 ? rows_per_group : 1;
+  p.rows_per_group = rows_per_group;
   p.plan = reinterpret_cast<const MelPlan*>(base + e.plan);
   p.frags = reinterpret_cast<const float4*>(base + e.frags);
   p.n_mels = d->n_mels;
@@ -1719,17 +1712,10 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   p.db_mult = d->db_multiplier;
   p.db_amin = d->db_amin;
   p.db_offset = d->db_offset;
-  // bulk staging needs 16-byte aligned sources and sizes (every unit starts at a multiple of
-  // frames_per_unit*hop, minus half + pad) and the unit's span must fit the staging buffer: the warp's mel region,
-  // or the Spectrogram kernel's float2 transpose tile
-  const int half = d->center ? d->n_fft / 2 : 0;
-  p.bulk_ok = d->hop % 4 == 0 && (half + d->pad) % 4 == 0 && row_stride % 4 == 0 &&
-              (reinterpret_cast<uintptr_t>(wave) & 15) == 0 &&
-              d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= staging;
   p.out_width = stage >= B200A_STAGE_MEL ? d->n_mels : d->n_fft / 2 + 1;
   p.out_col0 = 0;
   p.k_energy_col = -1;
-  int lead = half;
+  int64_t lead = (d->center ? d->n_fft / 2 : 0) + d->pad;
   if (kd != nullptr) {
     p.kaldi = 1;
     p.k_off = kd->snip_edges ? 0 : kd->window_size / 2 - kd->window_shift / 2;
@@ -1744,31 +1730,34 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
     p.out_col0 = kd->out_col0;
     p.pad_mode = kPadSymmetric;  // only reached when snip_edges == 0 (frames never leave the signal otherwise)
     lead = p.k_off;
-    if (!p.stage_ok) return B200A_EUNSUPPORTED;  // the conditioning reads the staged span
-    p.bulk_ok = d->hop % 4 == 0 && lead % 4 == 0 && row_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(wave) & 15) == 0;
+    if (!p.stage_ok) return kPathDeclined;  // the conditioning reads the staged span
   }
+  // the unit's span must also fit the staging buffer (the warp's mel region, or the Spectrogram kernel's float2
+  // transpose tile); the n_fft = 2048 kernels stage into tables of their own
+  p.bulk_ok = bulk_aligned(d->hop, lead, row_stride, wave) &&
+              (eo || d->n_fft + (unit_frames(d->n_fft) - 1) * (int64_t)d->hop <= staging);
   p.out_vec = (p.out_width % 4 == 0 && p.out_col0 % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0)   ? 4
               : (p.out_width % 2 == 0 && p.out_col0 % 2 == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0) ? 2
                                                                                                               : 1;
   if (eo) {
-    p.bulk_ok = d->hop % 4 == 0 && (half + d->pad) % 4 == 0 && row_stride % 4 == 0 &&
-                (reinterpret_cast<uintptr_t>(wave) & 15) == 0;
     const float2* tw_eo = reinterpret_cast<const float2*>(base + e.tw_eo);
     return d->power == 2.f ? launch_eo<2>(p, tw_eo, mel, stream) : launch_eo<0>(p, tw_eo, mel, stream);
   }
-  if (stage == B200A_STAGE_COMPLEX) return launch_any<kComplexOut>(p, d->n_fft, false, stream);
-  return d->power == 2.f ? launch_any<2>(p, d->n_fft, mel, stream) : launch_any<0>(p, d->n_fft, mel, stream);
+  return with_g(d->n_fft, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    if (stage == B200A_STAGE_COMPLEX) return launch_g<kComplexOut, G>(p, false, stream);
+    return d->power == 2.f ? launch_g<2, G>(p, mel, stream) : launch_g<0, G>(p, mel, stream);
+  });
 }
 
 // First half of b200a_istft_run for n_fft = 256 / 512 / 1024: windowed time frames into frame_buf.
 int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
                       int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, cudaStream_t stream) {
-  if (!pow2_applicable(*d) || d->n_fft > 1024) return B200A_EUNSUPPORTED;
+  if (!pow2_applicable(*d) || d->n_fft > 1024) return kPathDeclined;
   const WsLayout l = ws_layout(*d);
   const Pow2Extra e = pow2_layout(*d, l.total);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
-  const int G = d->n_fft / 32;
-  const int frames_per_unit = 2 * (32 / G);
+  const int frames_per_unit = unit_frames(d->n_fft);
   IstftPow2Params p{};
   p.spec = reinterpret_cast<const float2*>(spec);
   p.stride_row = stride_row;
@@ -1782,22 +1771,18 @@ int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float*
   p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
   p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
   const int64_t grid = persistent_grid(p.total_units, kIsWarps);
-  auto launch_g = [&](auto g) {
-    constexpr int GG = decltype(g)::value;
-    return launch_kernel(istft_pow2_kernel<GG>, grid, kIsWarps * 32, istft_smem<GG>(), stream, p);
-  };
-  if (G == 32) return launch_g(std::integral_constant<int, 32>{});
-  if (G == 16) return launch_g(std::integral_constant<int, 16>{});
-  return launch_g(std::integral_constant<int, 8>{});
+  return with_g(d->n_fft, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    return launch_kernel(istft_pow2_kernel<G>, grid, kIsWarps * 32, istft_smem<G>(), stream, p);
+  });
 }
 
 // Shared memory of the fused gradient kernel, 0 when the descriptor / stage does not take it.
 static size_t backward_smem(const b200a_frontend_desc* d, int stage) {
   if (!pow2_applicable(*d) || d->n_fft > 1024) return 0;
   if (stage != B200A_STAGE_COMPLEX && stage != B200A_STAGE_POWER && stage != B200A_STAGE_MEL) return 0;
-  const int G = d->n_fft / 32;
-  const size_t fixed = G == 32 ? bwd_smem_fixed<32>() : G == 16 ? bwd_smem_fixed<16>() : bwd_smem_fixed<8>();
-  const size_t g_rows = stage == B200A_STAGE_MEL ? sizeof(float) * kBwWarps * 2 * (32 / G) * (size_t)d->n_mels : 0;
+  const size_t fixed = with_g(d->n_fft, [](auto g) { return bwd_smem_fixed<decltype(g)::value>(); });
+  const size_t g_rows = stage == B200A_STAGE_MEL ? sizeof(float) * kBwWarps * unit_frames(d->n_fft) * (size_t)d->n_mels : 0;
   return fixed + g_rows <= (size_t)kSmemLimit ? fixed + g_rows : 0;
 }
 
@@ -1811,11 +1796,10 @@ int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int sta
   if (smem == 0) return B200A_EUNSUPPORTED;
   const WsLayout l = ws_layout(*d);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
-  const int G = d->n_fft / 32;
   BwdParams bp{};
   // edge units gather their span into the Spectrogram kernel's float2 transpose tile; bulk_ok stays 0: the tile doubles
   // as the inverse transform's, so nothing is staged into it ahead
-  bp.f = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, stage_floats(G, false));
+  bp.f = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, stage_floats(d->n_fft, false));
   bp.f.n_mels = stage == B200A_STAGE_MEL ? d->n_mels : 0;
   bp.f.stage = stage;
   bp.grad = grad;
@@ -1826,53 +1810,43 @@ int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int sta
   bp.fb = reinterpret_cast<const float*>(base + l.fb);
   bp.bands = reinterpret_cast<const int2*>(base + l.bands);
   const int64_t grid = persistent_grid(bp.f.total_units, kBwWarps);
-  auto by_stage = [&](auto g) {
-    constexpr int GG = decltype(g)::value;
-    auto kern = stage == B200A_STAGE_COMPLEX ? stft_pow2_backward_kernel<GG, B200A_STAGE_COMPLEX>
-                : stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<GG, B200A_STAGE_POWER>
-                                             : stft_pow2_backward_kernel<GG, B200A_STAGE_MEL>;
+  return with_g(d->n_fft, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    auto kern = stage == B200A_STAGE_COMPLEX ? stft_pow2_backward_kernel<G, B200A_STAGE_COMPLEX>
+                : stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<G, B200A_STAGE_POWER>
+                                             : stft_pow2_backward_kernel<G, B200A_STAGE_MEL>;
     return launch_kernel(kern, grid, kBwWarps * 32, smem, stream, bp);
-  };
-  if (G == 32) return by_stage(std::integral_constant<int, 32>{});
-  if (G == 16) return by_stage(std::integral_constant<int, 16>{});
-  return by_stage(std::integral_constant<int, 8>{});
+  });
 }
 
 // The iSTFT adjoint runs on the register FFT when n_fft is 256 / 512 / 1024 (one-sided), an edge unit's span fits the
 // Spectrogram kernel's staging tile (hop <= ~n_fft) and the frames' samples index with 32 bits.
 bool istft_backward_fused_applicable(const b200a_frontend_desc* d, int64_t frames) {
   if (!pow2_applicable(*d) || d->n_fft > 1024) return false;
-  const int G = d->n_fft / 32;
-  const int64_t span = d->n_fft + (2 * (32 / G) - 1) * (int64_t)d->hop;
-  return span <= stage_floats(G, false) && d->n_fft + (int64_t)d->hop * (frames - 1) + 2 * d->n_fft < (int64_t)1 << 31;
+  const int64_t span = d->n_fft + (unit_frames(d->n_fft) - 1) * (int64_t)d->hop;
+  return span <= stage_floats(d->n_fft, false) && d->n_fft + (int64_t)d->hop * (frames - 1) + 2 * d->n_fft < (int64_t)1 << 31;
 }
 
 // b200a_istft_backward for n_fft = 256 / 512 / 1024: the COMPLEX Spectrogram kernel in its kIstftGrad variant over g,
 // framed with a lead of `start` samples and constant padding, straight into grad_spec.
 int istft_backward_pow2(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, float* grad_spec, cudaStream_t stream) {
-  if (!istft_backward_fused_applicable(d, frames)) return B200A_EUNSUPPORTED;
-  const int G = d->n_fft / 32;
-  const int frames_per_unit = 2 * (32 / G);
-  const int staging = stage_floats(G, false);
+  if (!istft_backward_fused_applicable(d, frames)) return kPathDeclined;
   // samples at or past expected = n_fft + hop (frames - 1) get no gradient: clamp so that every index fits 32 bits
   const int64_t expected = d->n_fft + (int64_t)d->hop * (frames - 1);
   const int64_t lead = start < expected ? start : expected;
   const int64_t len = g_len < expected - lead ? g_len : expected - lead;
-  Pow2Params p = pow2_geometry(*d, ws, grad, rows, len, g_row_stride, frames, staging);
+  Pow2Params p = pow2_geometry(*d, ws, grad, rows, len, g_row_stride, frames, stage_floats(d->n_fft, false));
   p.center = 0;
   p.pad = (int)lead;
   p.pad_mode = B200A_PAD_CONSTANT;
   p.stage_ok = 1;
   p.out = grad_spec;
-  p.bulk_ok = d->hop % 4 == 0 && lead % 4 == 0 && g_row_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(grad) & 15) == 0 &&
-              d->n_fft + (frames_per_unit - 1) * (int64_t)d->hop <= staging;
+  p.bulk_ok = bulk_aligned(d->hop, lead, g_row_stride, grad);  // the span fits the tile: istft_backward_fused_applicable
   const int64_t cover = (d->n_fft + d->hop - 1) / d->hop;  // frames overlapping one sample, at most
   p.env_t_lo = cover - 1;
   p.env_t_hi = frames - cover;
-  if (G == 32) return launch_g<kIstftGrad, 32>(p, false, stream);
-  if (G == 16) return launch_g<kIstftGrad, 16>(p, false, stream);
-  return launch_g<kIstftGrad, 8>(p, false, stream);
+  return with_g(d->n_fft, [&](auto g) { return launch_g<kIstftGrad, decltype(g)::value>(p, false, stream); });
 }
 
 }  // namespace b200a

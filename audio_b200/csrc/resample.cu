@@ -386,10 +386,6 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
   const RsLayout l = rs_layout(new_r, taps);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
 
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    return B200A_ECUDA;
-
   // ---- tensor-pipe path -------------------------------------------------------------------------
   const int n_tiles = rs_tiles(new_r);
   const int xs_floats = (kRsFrames * orig_r + taps + 16 + 4 + 3) & ~3;  // rs_fill's span + its alignment shift
@@ -420,11 +416,6 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
     // device-side step count with the room granted here), otherwise they are read through L1
     p.frag_smem_bytes = (int)(((size_t)kRsSmemBudget - smem_fixed) & ~(size_t)511);  // everything that is left
     const size_t smem = smem_fixed + p.frag_smem_bytes;
-    if (cudaFuncSetAttribute(resample_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) !=
-        cudaSuccess)
-      return B200A_ECUDA;
-    int64_t grid = p.total_blocks < sms ? p.total_blocks : sms;
-    if (grid < 1) grid = 1;
     // row spread: the candidate with the fewest shared-memory bank conflicts for one A-fragment load
     // (8 rows x 4 consecutive words, rows spread*orig' words apart)
     int best_spread = 1, best_conf = 1 << 30;
@@ -448,8 +439,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
       const double idle = 1.0 - (double)items / (double)(rounds * w);
       if (idle <= best_idle + 1e-9) { best_idle = idle; warps = w; }  // ties go to more warps
     }
-    resample_mma_kernel<<<(unsigned)grid, warps * 32, smem, stream>>>(p);
-    return launch_status();
+    return launch_kernel(resample_mma_kernel, persistent_grid(p.total_blocks, 1), warps * 32, smem, stream, p);
   }
 
   // ---- direct path --------------------------------------------------------------------------------

@@ -97,11 +97,9 @@ int amplitude_to_db_impl(const float* x, int64_t groups, int64_t group_elems, fl
     int rc = fill_impl(scratch, groups, -INFINITY, stream);
     if (rc != B200A_OK) return rc;
   }
-  const int sms = device_sm_count();
-  if (sms < 0) return B200A_ECUDA;
-  unsigned bx = (unsigned)((group_elems + 255) / 256);
-  if (bx > 8u * (unsigned)sms) bx = 8u * (unsigned)sms;  // 8 CTAs per SM, grid-stride beyond
-  dim3 grid(bx, (unsigned)groups);
+  const int64_t bx = sm_capped_grid((group_elems + 255) / 256, 8);  // 8 CTAs per SM, grid-stride beyond
+  if (bx < 0) return B200A_ECUDA;
+  dim3 grid((unsigned)bx, (unsigned)groups);
   to_db_kernel<<<grid, 256, 0, stream>>>(x, group_elems, mult, amin, offset, clamp ? scratch : nullptr, out);
   if (clamp) clamp_floor_kernel<<<grid, 256, 0, stream>>>(out, group_elems, scratch, top_db);
   return launch_status();
@@ -169,10 +167,8 @@ int griffinlim_update_impl(const float* mag, int64_t ms_row, int64_t ms_bin, int
                            const float* rebuilt, const float* tprev, float momentum, int normalize, float* proj,
                            int64_t rows, int64_t bins, int64_t frames, cudaStream_t stream) {
   const int64_t total = rows * bins * frames;
-  int64_t grid = (total + 255) / 256;
-  const int sms = device_sm_count();
-  if (sms < 0) return B200A_ECUDA;
-  if (grid > 16 * (int64_t)sms) grid = 16 * (int64_t)sms;  // 16 CTAs per SM, grid-stride beyond
+  const int64_t grid = sm_capped_grid((total + 255) / 256, 16);  // 16 CTAs per SM, grid-stride beyond
+  if (grid < 0) return B200A_ECUDA;
   griffinlim_update_kernel<<<(unsigned)grid, 256, 0, stream>>>(mag, ms_row, ms_bin, ms_frame, inv_power,
                                                               reinterpret_cast<const float2*>(rebuilt),
                                                               reinterpret_cast<const float2*>(tprev), momentum, normalize,

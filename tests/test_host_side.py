@@ -159,6 +159,112 @@ def test_abi_argument_validation_without_gpu(lib):
     assert lib.b200a_num_bins(1024, 1) == 513 and lib.b200a_num_bins(1024, 0) == 1024
 
 
+def _desc(n_fft=512, hop=128, center=True, pad_mode="reflect", power=2.0, n_mels=0, **kw):
+    from audio_b200._plans import FrontendPlan
+
+    d = FrontendPlan.make_desc(n_fft, n_fft, hop, 0, center, pad_mode, True, False, False, power, n_mels)
+    for k, v in kw.items():
+        setattr(d, k, v)
+    return d
+
+
+def test_frontend_run_status_codes(lib):
+    """Every early return of b200a_frontend_run, with the status it reports; none of them reaches the GPU."""
+    L = _lib
+    fake = ctypes.c_void_p(0x1000)  # never dereferenced: every case below returns first
+
+    def run(d, stage=L.STAGE_POWER, rows=2, length=4000, row_stride=None, ptrs=True):
+        p = fake if ptrs else None
+        return lib.b200a_frontend_run(d, p, stage, p, rows, length, length if row_stride is None else row_stride, p, None, 1,
+                                      None)
+
+    assert run(None) == L.EINVAL
+    assert run(_desc(hop=0)) == L.EINVAL
+    assert run(_desc(n_fft=16384)) == L.EUNSUPPORTED
+    assert run(_desc(), stage=-1) == L.EINVAL
+    assert run(_desc(), stage=L.STAGE_FEAT + 1) == L.EINVAL
+    assert run(_desc(), stage=L.STAGE_MEL) == L.EINVAL  # no filterbank in the descriptor
+    assert run(_desc(), stage=L.STAGE_FEAT) == L.EINVAL
+    assert run(_desc(power=0.0)) == L.EINVAL
+    assert run(_desc(power=-1.0)) == L.EINVAL
+    assert run(_desc(power=float("nan"))) == L.EINVAL  # power None is valid for COMPLEX only
+    assert run(_desc(), rows=-1) == L.EINVAL
+    assert run(_desc(), length=-1, row_stride=0) == L.EINVAL
+    assert run(_desc(), row_stride=3999) == L.EINVAL
+    assert run(_desc(), ptrs=False) == L.EINVAL
+    # reflect needs n_fft/2 < length + 2 pad, circular n_fft/2 <= length + 2 pad
+    assert run(_desc(), length=256) == L.ESHORT
+    assert run(_desc(pad=10), length=236) == L.ESHORT
+    assert run(_desc(pad_mode="circular"), length=255) == L.ESHORT
+    assert run(_desc(center=False), length=511) == L.ESHORT  # too few samples for one frame
+    assert run(_desc(center=False, pad=8), length=495) == L.ESHORT
+    # an empty batch enqueues nothing and needs no pointers, whatever else is wrong except the descriptor
+    assert run(_desc(), rows=0, ptrs=False) == L.OK
+    assert run(_desc(), stage=-1, rows=0, length=10, ptrs=False) == L.OK
+    assert run(None, rows=0, ptrs=False) == L.EINVAL
+    # the backward entry point rejects the same descriptor / stage / length problems with the same codes
+    assert lib.b200a_frontend_backward(_desc(), fake, L.STAGE_POWER, fake, 2, 256, 256, fake, 0, 0, 0, fake, fake, 256,
+                                       None) == L.ESHORT
+
+
+def test_kaldi_run_status_codes(lib):
+    """Every early return of b200a_kaldi_run, with the status it reports; none of them reaches the GPU."""
+    L = _lib
+    fake = ctypes.c_void_p(0x1000)  # never dereferenced: every case below returns first
+
+    def kaldi(**kw):
+        k = L.KaldiDesc()
+        k.window_size, k.window_shift, k.padded_size, k.snip_edges, k.remove_dc_offset = 400, 160, 512, 1, 1
+        k.preemphasis, k.energy_mode, k.energy_floor, k.energy_col = 0.97, 0, 0.0, -1
+        k.out_width, k.out_col0, k.use_log = 257, 0, 1
+        for name, v in kw.items():
+            setattr(k, name, v)
+        return k
+
+    def run(k=None, d=None, stage=L.STAGE_POWER, rows=2, length=4000, row_stride=None, ptrs=True, no_kaldi=False):
+        k = None if no_kaldi else (k or kaldi())
+        d = d or _desc(hop=160, center=False)
+        p = fake if ptrs else None
+        return lib.b200a_kaldi_run(k, d, p, stage, p, rows, length, length if row_stride is None else row_stride, p, None)
+
+    assert run(no_kaldi=True) == L.EINVAL
+    assert lib.b200a_kaldi_run(kaldi(), None, fake, L.STAGE_POWER, fake, 2, 4000, 4000, fake, None) == L.EINVAL
+    assert run(d=_desc(hop=0, center=False)) == L.EINVAL
+    # the Kaldi descriptor itself
+    assert run(kaldi(window_size=1)) == L.EINVAL
+    assert run(kaldi(window_shift=0)) == L.EINVAL
+    assert run(kaldi(padded_size=256)) == L.EINVAL  # shorter than the window
+    assert run(kaldi(window_size=401, padded_size=513), d=_desc(n_fft=513, hop=160, center=False)) == L.EINVAL  # odd
+    # ... and its agreement with the front-end descriptor
+    assert run(d=_desc(n_fft=1024, hop=160, center=False)) == L.EINVAL
+    assert run(d=_desc(hop=160, center=False, win_length=400)) == L.EINVAL
+    assert run(d=_desc(hop=128, center=False)) == L.EINVAL
+    assert run(d=_desc(hop=160, center=True)) == L.EINVAL
+    assert run(d=_desc(hop=160, center=False, pad=4)) == L.EINVAL
+    assert run(d=_desc(hop=160, center=False, onesided=0)) == L.EINVAL
+    # stage, power and conditioning
+    assert run(stage=L.STAGE_COMPLEX) == L.EINVAL
+    assert run(stage=L.STAGE_FEAT) == L.EINVAL
+    assert run(stage=L.STAGE_MEL) == L.EINVAL  # no filterbank in the descriptor
+    assert run(d=_desc(hop=160, center=False, power=0.0)) == L.EINVAL
+    assert run(kaldi(preemphasis=-0.1)) == L.EINVAL
+    assert run(kaldi(preemphasis=1.5)) == L.EINVAL
+    assert run(kaldi(energy_mode=3)) == L.EINVAL
+    assert run(kaldi(energy_mode=-1)) == L.EINVAL
+    assert run(kaldi(energy_floor=-1.0)) == L.EINVAL
+    # output columns
+    assert run(kaldi(out_col0=-1)) == L.EINVAL
+    assert run(kaldi(out_col0=1)) == L.EINVAL  # 257 values from column 1 overflow a width of 257
+    assert run(kaldi(energy_col=257)) == L.EINVAL
+    # batch, pointers, lengths
+    assert run(rows=0, ptrs=False) == L.OK
+    assert run(ptrs=False) == L.EINVAL
+    assert run(rows=-1) == L.EINVAL
+    assert run(row_stride=3999) == L.EINVAL
+    assert run(length=399) == L.ESHORT  # shorter than one window
+    assert run(kaldi(snip_edges=0, window_shift=1000), d=_desc(hop=1000, center=False), length=400) == L.ESHORT  # no frame
+
+
 # ---------------- drop-in module surface ----------------------------------------------------------
 def test_state_dict_names_match_reference():
     # transforms_test.py:68-85
