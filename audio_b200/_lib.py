@@ -134,6 +134,12 @@ _SIGNATURES = {
         ctypes.c_int,
         [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p],
     ),
+    "b200a_resample_backward_workspace_bytes": (c_size_t, [c_int32, c_int32, c_int32]),
+    "b200a_resample_backward_prepare": (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_size_t, c_void_p]),
+    "b200a_resample_backward": (
+        ctypes.c_int,
+        [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p],
+    ),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

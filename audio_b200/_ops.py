@@ -1,6 +1,6 @@
 """``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
-``resample_run``.
+``resample_run`` / ``resample_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -43,6 +43,7 @@ _LIB.define(
     "resample_run(Tensor wave, Tensor workspace, Tensor kernel, int orig_r, int new_r, int width, int row_stride, "
     "int out_len, int pitch) -> Tensor"
 )
+_LIB.define("resample_backward(Tensor grad, Tensor workspace, int orig_r, int new_r, int width, int length) -> Tensor")
 
 
 def pack_desc(d: "_lib.FrontendDesc"):
@@ -182,11 +183,32 @@ def _resample_run_meta(wave, workspace, kernel, orig_r, new_r, width, row_stride
     return wave.new_empty((wave.shape[0], pitch))
 
 
+# ---- resample_backward -------------------------------------------------------------------------------------------
+def _resample_backward_cuda(grad, workspace, orig_r, new_r, width, length):
+    """(rows, out_len) upstream gradient -> (rows, length) waveform gradient."""
+    if grad.shape[0] > 0 and grad.shape[1] > 0 and grad.stride(1) != 1:
+        grad = grad.contiguous()
+    rows, out_len = grad.shape
+    dev = grad.device
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, length), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_resample_backward(
+            workspace.data_ptr(), orig_r, new_r, width, grad.data_ptr(), rows, grad.stride(0) if rows > 1 else out_len,
+            out_len, out.data_ptr(), length, length, _stream(dev))
+    _lib.check(rc, "resample_backward")
+    return out
+
+
+def _resample_backward_meta(grad, workspace, orig_r, new_r, width, length):
+    return grad.new_empty((grad.shape[0], length))
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
                             ("mfcc_finish", _mfcc_finish_cuda, _mfcc_finish_meta),
-                            ("resample_run", _resample_run_cuda, _resample_run_meta)):
+                            ("resample_run", _resample_run_cuda, _resample_run_meta),
+                            ("resample_backward", _resample_backward_cuda, _resample_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -195,3 +217,4 @@ frontend_backward = torch.ops.b200audio.frontend_backward
 istft_backward = torch.ops.b200audio.istft_backward
 mfcc_finish = torch.ops.b200audio.mfcc_finish
 resample_run = torch.ops.b200audio.resample_run
+resample_backward = torch.ops.b200audio.resample_backward

@@ -42,23 +42,30 @@ def is_inverse_differentiable() -> bool:
     return getattr(_GRAD_STATE, "inverse", False)
 
 
-def set_differentiable(mode: bool, *, inverse: bool = False) -> None:
+def is_resample_differentiable() -> bool:
+    """Whether Resample, F.resample, Speed and SpeedPerturbation accept waveforms that require grad (in this thread)."""
+    return getattr(_GRAD_STATE, "resample", False)
+
+
+def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = False) -> None:
     """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
-    ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT; it is a separate
-    switch so that vocoder inference and augmentation code does not build graphs when loss gradients are on."""
+    ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT, ``resample=True``
+    (with ``mode``) the waveform gradients of the resampler.  They are separate switches so that vocoder inference and
+    augmentation code (Speed, SpeedPerturbation) does not build graphs when loss gradients are on."""
     _GRAD_STATE.on = bool(mode)
     _GRAD_STATE.inverse = bool(mode) and bool(inverse)
+    _GRAD_STATE.resample = bool(mode) and bool(resample)
 
 
 @contextlib.contextmanager
-def differentiable(mode: bool = True, *, inverse: bool = False):
+def differentiable(mode: bool = True, *, inverse: bool = False, resample: bool = False):
     """Context manager form of :func:`set_differentiable`; restores the previous settings on exit."""
-    prev = is_differentiable(), is_inverse_differentiable()
-    set_differentiable(mode, inverse=inverse)
+    prev = is_differentiable(), is_inverse_differentiable(), is_resample_differentiable()
+    set_differentiable(mode, inverse=inverse, resample=resample)
     try:
         yield
     finally:
-        set_differentiable(prev[0], inverse=prev[1])
+        set_differentiable(prev[0], inverse=prev[1], resample=prev[2])
 
 
 def _no_autograd(t: torch.Tensor) -> None:
@@ -67,7 +74,8 @@ def _no_autograd(t: torch.Tensor) -> None:
             "audio_b200 kernels are forward-only: the input requires grad. Call under torch.no_grad() / "
             "torch.inference_mode(), or detach() the input. (Spectrogram, MelSpectrogram and F.spectrogram compute "
             "waveform gradients inside audio_b200.differentiable(); InverseSpectrogram and F.inverse_spectrogram "
-            "compute spectrogram gradients inside audio_b200.differentiable(inverse=True).)"
+            "compute spectrogram gradients inside audio_b200.differentiable(inverse=True); Resample, F.resample, Speed "
+            "and SpeedPerturbation compute waveform gradients inside audio_b200.differentiable(resample=True).)"
         )
 
 
@@ -266,8 +274,28 @@ def new_group_max(groups: int, device: torch.device) -> torch.Tensor:
     return g
 
 
+class _ResampleFunction(torch.autograd.Function):
+    """b200audio::resample_run on the packed (rows, L) waveform, sliced to out_len inside (so autograd adds no
+    slice_backward fill), with b200audio::resample_backward as its backward.  The map is linear: only the backward
+    workspace built from the forward's kernel is kept, so a kernel edited after the forward does not change the
+    gradient."""
+
+    @staticmethod
+    def forward(ctx, flat, ws, k, bws, orig_r, new_r, width, stride, out_len, pitch):
+        buf = _ops.resample_run(flat, ws, k, orig_r, new_r, width, stride, out_len, pitch)
+        ctx.bws, ctx.ratio, ctx.length = bws, (orig_r, new_r, width), flat.shape[1]
+        return buf[:, :out_len]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        grad = _ops.resample_backward(grad_out, ctx.bws, *ctx.ratio, ctx.length)
+        return grad, None, None, None, None, None, None, None, None, None
+
+
 class ResamplePlan:
-    """Per-phase tap supports of a cached sinc kernel, kept next to the kernel buffer."""
+    """Per-phase tap supports of a cached sinc kernel, kept next to the kernel buffer; the adjoint tables are built
+    from the same kernel on the first forward that wants a gradient."""
 
     def __init__(self, orig_r: int, new_r: int, width: int):
         self.orig_r, self.new_r, self.width = int(orig_r), int(new_r), int(width)
@@ -276,6 +304,8 @@ class ResamplePlan:
         self._stamp = None
         self._kernel: Optional[torch.Tensor] = None
         self._held = None  # the kernel tensor behind the stamp (see FrontendPlan._held)
+        self._bws: Optional[torch.Tensor] = None
+        self._bws_stamp = None
 
     def workspace(self, kernel: torch.Tensor):
         stamp = (kernel.data_ptr(), _version_of(kernel), str(kernel.device))
@@ -297,18 +327,39 @@ class ResamplePlan:
         self._ws, self._stamp, self._kernel, self._held = ws, stamp, k, kernel
         return ws, k
 
+    def backward_workspace(self) -> torch.Tensor:
+        """The adjoint tables of the kernel the forward workspace was last built from (call after ``workspace``)."""
+        if self._bws is not None and self._bws_stamp == self._stamp:
+            return self._bws
+        lib = _lib.lib()
+        k = self._kernel
+        dev = k.device
+        nbytes = lib.b200a_resample_backward_workspace_bytes(self.orig_r, self.new_r, self.width)
+        with torch.cuda.device(dev):
+            bws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            rc = lib.b200a_resample_backward_prepare(k.data_ptr(), self.orig_r, self.new_r, self.width, bws.data_ptr(),
+                                                     nbytes, _stream_ptr(dev))
+        _lib.check(rc, "resample_backward_prepare")
+        self._bws, self._bws_stamp = bws, self._stamp
+        return bws
+
     def run(self, kernel: torch.Tensor, waveform: torch.Tensor) -> torch.Tensor:
         _require_cuda_f32(waveform, "waveform")
-        _no_autograd(waveform)
+        grad = _wants_grad(waveform, (("kernel", kernel),), is_resample_differentiable)
+        if not grad:
+            _no_autograd(waveform)
         ws, k = self.workspace(kernel)
         if waveform.device != ws.device:
             raise RuntimeError(f"audio_b200: waveform is on {waveform.device} but the kernel buffer is on {ws.device}")
-        lib = _lib.lib()
         flat, stride = pack_rows(waveform)
         rows, length = flat.shape
         out_len = resample_len(length, self.orig_r, self.new_r)
         # the reference returns a view into (rows, frames*new') memory: keep that row pitch
         pitch = (length // self.orig_r + 1) * self.new_r
-        buf = _ops.resample_run(flat, ws, k, self.orig_r, self.new_r, self.width, stride, out_len, pitch)
-        out = buf[:, :out_len]
+        if grad:
+            out = _ResampleFunction.apply(flat, ws, k, self.backward_workspace(), self.orig_r, self.new_r, self.width,
+                                          stride, out_len, pitch)
+        else:
+            buf = _ops.resample_run(flat, ws, k, self.orig_r, self.new_r, self.width, stride, out_len, pitch)
+            out = buf[:, :out_len]
         return out.view(waveform.shape[:-1] + (out_len,)) if rows > 0 else out.reshape(waveform.shape[:-1] + (out_len,))

@@ -302,5 +302,29 @@ int b200a_resample_run(const void* workspace, const float* kernel, int32_t orig_
                            out_row_stride, out_len, static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_resample_backward_workspace_bytes(int32_t orig_r, int32_t new_r, int32_t width) {
+  if (orig_r < 1 || new_r < 1 || width < 0) return 0;
+  return resample_backward_workspace_bytes_impl(orig_r, new_r, width);
+}
+
+int b200a_resample_backward_prepare(const float* kernel, int32_t orig_r, int32_t new_r, int32_t width, void* workspace,
+                                    size_t workspace_bytes, b200a_stream stream) {
+  return resample_backward_prepare_impl(kernel, orig_r, new_r, width, workspace, workspace_bytes,
+                                        static_cast<cudaStream_t>(stream));
+}
+
+int b200a_resample_backward(const void* workspace, int32_t orig_r, int32_t new_r, int32_t width, const float* grad,
+                            int64_t rows, int64_t g_row_stride, int64_t out_len, float* grad_wave, int64_t length,
+                            int64_t grad_row_stride, b200a_stream stream) {
+  if (orig_r < 1 || new_r < 1 || width < 0 || rows < 0 || length < 0 || out_len < 0 || g_row_stride < 0)
+    return B200A_EINVAL;
+  if (out_len != b200a_resample_len(length, orig_r, new_r)) return B200A_EINVAL;
+  if (rows == 0) return B200A_OK;  // empty batch: nothing to enqueue (pointers may be null)
+  if (workspace == nullptr || grad == nullptr || grad_wave == nullptr || grad_row_stride < length) return B200A_EINVAL;
+  if (length == 0) return B200A_OK;
+  return resample_backward_impl(workspace, orig_r, new_r, width, grad, rows, g_row_stride, out_len, grad_wave, length,
+                                grad_row_stride, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

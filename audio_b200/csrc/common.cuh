@@ -151,6 +151,12 @@ int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width,
 int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r, int width, const float* wave,
                       int64_t rows, int64_t length, int64_t row_stride, float* out, int64_t out_row_stride,
                       int64_t out_len, cudaStream_t stream);
+size_t resample_backward_workspace_bytes_impl(int orig_r, int new_r, int width);
+int resample_backward_prepare_impl(const float* kernel, int orig_r, int new_r, int width, void* ws, size_t ws_bytes,
+                                   cudaStream_t stream);
+int resample_backward_impl(const void* ws, int orig_r, int new_r, int width, const float* grad, int64_t rows,
+                           int64_t g_row_stride, int64_t out_len, float* grad_wave, int64_t length,
+                           int64_t grad_row_stride, cudaStream_t stream);
 
 // ---- device helpers -----------------------------------------------------------------------
 // Index into the raw waveform row for sample i of the (constant `pad`-extended, then centre

@@ -21,6 +21,9 @@
 //     taps = 2 width + orig'), the barriers and the group table leave less than 1 KiB of kRsSmemBudget
 //     (224 KiB) for the fragments, or
 //   - `wave` is not 4-byte aligned, which no valid float pointer is.
+//
+// Adjoint (resample_backward_mma_kernel / resample_backward_direct_kernel): see the section before the host code.
+#include <algorithm>
 #include <type_traits>
 
 #include "common.cuh"
@@ -354,9 +357,391 @@ resample_direct_kernel(const float* __restrict__ wave, int64_t length, int64_t r
   }
 }
 
+// ==== adjoint (waveform gradient) ================================================================
+// With G[f][j] = g[f*new' + j] (0 past out_len) the forward's transpose is
+//     D = G * K  (frames x taps),   grad_x[s] = sum_f D[f][s + width - f*orig']  over 0 <= s + width - f*orig' < taps,
+// with K masked to each phase's live taps (the support the forward uses).  Both kernels below compute every sample of
+// [0, length) as a sum over its frames in ascending order; nothing depends on how rows are batched.
+//
+// Backward workspace: header | support[new'] | tap_range[taps] | kt[taps][new'] | cols[n_cols] | frags.
+//   tap_range[i] = (first phase, count) of the hull of the phases whose live taps include tap i;
+//   kt[i][j]     = K[j][i] when tap i is live for phase j, else 0 (gaps inside a hull read zeros);
+//   cols / frags = per group of 8 taps the 8-phase k-steps covering the union of its taps' hulls, and the masked taps as
+//                  TF32 hi/lo B fragments (only for ratios the mma kernel takes).
+constexpr int kRbMaxRows = 512;  // staged frame rows per tile (halo + owned)
+
+// Tile geometry of resample_backward_mma_kernel: a function of the ratio alone, never of the batch.
+struct RbConfig {
+  bool mma;
+  int halo;        // H = ceil(2 width / orig'): frames before the tile whose taps reach its samples
+  int rows_tile;   // R: staged frame rows (multiple of 16), R - H of them owned
+  int pitch;       // staged row pitch in floats: round8(new') + 4 (== 4 mod 8: conflict-free A-fragment loads)
+  int d_pitch;     // D row pitch in floats (== 8 mod 32: conflict-free float2 fragment stores)
+  int n_cols;      // groups of 8 taps
+  size_t smem_fixed;
+};
+
+inline RbConfig rb_config(int orig_r, int new_r, int width) {
+  RbConfig c{};
+  const int taps = 2 * width + orig_r;
+  c.halo = (2 * width + orig_r - 1) / orig_r;
+  c.n_cols = (taps + 7) / 8;
+  c.pitch = ((new_r + 7) & ~7) + 4;
+  c.d_pitch = 8 * c.n_cols + ((8 - (8 * c.n_cols) % 32) + 32) % 32;
+  if (rs_tiles(new_r) > kRsMaxTiles) return c;
+  auto fixed = [&](int R) {
+    return sizeof(float) * ((size_t)2 * R * c.pitch + (size_t)R * c.d_pitch) + sizeof(RsTile) * ((c.n_cols + 3) & ~3);
+  };
+  // the smallest R that keeps the recomputed halo at <= 1/16 of the rows (and R >= 32) and gives a tile at least 4096
+  // owned samples (fewer per-tile barriers for short frames), or the largest that fits
+  for (int R = 16; R <= kRbMaxRows; R += 16) {
+    if (R <= c.halo) continue;
+    if (fixed(R) + 1024 > (size_t)kRsSmemBudget) break;
+    c.rows_tile = R;
+    if (R >= 32 && R >= 16 * c.halo && (int64_t)(R - c.halo) * orig_r >= 4096) break;
+  }
+  c.mma = c.rows_tile > 0;
+  c.smem_fixed = c.mma ? fixed(c.rows_tile) : 0;
+  return c;
+}
+
+struct RbLayout {
+  size_t header, support, tap_range, kt, cols, frags, total;
+};
+
+inline RbLayout rb_layout(int orig_r, int new_r, int width) {
+  const int taps = 2 * width + orig_r;
+  const RbConfig c = rb_config(orig_r, new_r, width);
+  RbLayout l{};
+  size_t off = 0;
+  l.header = off;
+  off = align_up(off + sizeof(RsHeader), 256);
+  l.support = off;
+  off = align_up(off + sizeof(int2) * (size_t)new_r, 256);
+  l.tap_range = off;
+  off = align_up(off + sizeof(int2) * (size_t)taps, 256);
+  l.kt = off;
+  off = align_up(off + sizeof(float) * (size_t)taps * new_r, 256);
+  l.cols = off;
+  l.frags = off;
+  if (c.mma) {
+    off = align_up(off + sizeof(RsTile) * (size_t)c.n_cols, 256);
+    l.frags = off;  // worst case: every tap group spans every phase group
+    off = align_up(off + sizeof(float4) * 32 * (size_t)c.n_cols * rs_tiles(new_r), 256);
+  }
+  l.total = off;
+  return l;
+}
+
+// One thread per tap: the hull of the phases for which it is live; and kt, the masked transpose of the kernel.
+__global__ void resample_adjoint_table_kernel(const float* __restrict__ kernel, const int2* __restrict__ support,
+                                              int new_r, int taps, int2* tap_range, float* kt) {
+  const int64_t n = (int64_t)taps * new_r;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+    const int i = (int)(e / new_r), j = (int)(e - (int64_t)i * new_r);
+    const int2 sp = support[j];
+    kt[e] = (i >= sp.x && i < sp.x + sp.y) ? kernel[(size_t)j * taps + i] : 0.f;
+  }
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < taps; i += gridDim.x * blockDim.x) {
+    int lo = new_r, hi = -1;
+    for (int j = 0; j < new_r; ++j) {
+      const int2 sp = support[j];
+      if (i >= sp.x && i < sp.x + sp.y) {
+        lo = min(lo, j);
+        hi = j;
+      }
+    }
+    tap_range[i] = hi < 0 ? make_int2(0, 0) : make_int2(lo, hi - lo + 1);
+  }
+}
+
+// Per group of 8 taps: the 8-phase k-steps covering the union of its taps' hulls, and kt split into TF32 hi/lo parts in
+// mma.m16n8k8 B-fragment order (B[k][n] = kt[8 c + n][kstart + k]).
+__global__ void resample_backward_plan_kernel(const float* __restrict__ kt, const int2* __restrict__ tap_range,
+                                              int new_r, int taps, int n_cols, RsHeader* hdr, RsTile* cols,
+                                              float4* frags) {
+  if (threadIdx.x == 0) {
+    int acc = 0;
+    for (int cg = 0; cg < n_cols; ++cg) {
+      int lo = new_r, hi = 0;
+      for (int i = 8 * cg; i < min(8 * cg + 8, taps); ++i) {
+        const int2 tr = tap_range[i];
+        if (tr.y > 0) { lo = min(lo, tr.x); hi = max(hi, tr.x + tr.y); }
+      }
+      RsTile ct{0, 0, acc, 0};
+      if (hi > lo) {
+        ct.kstart = lo & ~7;
+        ct.nsteps = (hi - ct.kstart + 7) / 8;
+      }
+      cols[cg] = ct;
+      acc += ct.nsteps;
+    }
+    hdr->n_tiles = n_cols;
+    hdr->total_steps = acc;
+  }
+  __syncthreads();
+  for (int cg = 0; cg < n_cols; ++cg) {
+    const RsTile ct = cols[cg];
+    for (int e = threadIdx.x; e < ct.nsteps * 32; e += blockDim.x) {
+      const int s = e >> 5, lane = e & 31;
+      const int i = 8 * cg + (lane >> 2);
+      const int j0 = ct.kstart + 8 * s + (lane & 3), j1 = j0 + 4;
+      const float b0 = (i < taps && j0 < new_r) ? kt[(size_t)i * new_r + j0] : 0.f;
+      const float b1 = (i < taps && j1 < new_r) ? kt[(size_t)i * new_r + j1] : 0.f;
+      const float b0h = __uint_as_float(__float_as_uint(b0) & 0xffffe000u);
+      const float b1h = __uint_as_float(__float_as_uint(b1) & 0xffffe000u);
+      frags[(size_t)(ct.frag_off + s) * 32 + lane] = make_float4(b0h, b1h, b0 - b0h, b1 - b1h);
+    }
+  }
+}
+
+struct RbParams {
+  const float* grad;
+  int64_t g_row_stride, out_len;
+  float* out;
+  int64_t length, out_row_stride;
+  const RsHeader* hdr;
+  const RsTile* cols;
+  const float4* frags;
+  int orig_r, new_r, width, taps, n_cols;
+  int halo, rows_tile, frames_tile, pitch, d_pitch;
+  int64_t blocks_per_row, total_blocks;
+  int frag_smem_bytes;
+};
+
+// Stage the g rows of frames [f0 - H, f0 - H + R) into gs at pitch p.pitch with 4-byte asynchronous copies (the padded
+// pitch rules out one 1-D bulk copy; these need no alignment, so every view of g takes the same path).  Zeros for
+// frames before the signal, outputs past out_len and the pad columns.
+__device__ __forceinline__ void rb_fill(const RbParams& p, int64_t row, int64_t f0, float* gs, int warp, int lane,
+                                        int n_warps) {
+  const float* g = p.grad + row * p.g_row_stride;
+  const int64_t fr0 = f0 - p.halo;
+  for (int rho = warp; rho < p.rows_tile; rho += n_warps) {  // one warp per staged row, lanes along its phases
+    const int64_t m0 = (fr0 + rho) * p.new_r;
+    const int live = fr0 + rho < 0 ? 0 : (int)max((int64_t)0, min((int64_t)p.new_r, p.out_len - m0));
+    float* dst = gs + rho * p.pitch;
+    for (int j = lane; j < p.pitch; j += 32) {
+      if (j < live) cp_async4(dst + j, g + m0 + j);
+      else dst[j] = 0.f;
+    }
+  }
+}
+
+// Persistent CTAs over (row, tile of F = R - H frames): D = G * K on mma.sync m16n8k8 TF32 x 3 into shared memory, then
+// every owned sample sums its <= H + 1 contributions in ascending frame order.  One warp item = 16 frame rows x one
+// group of 8 taps over that group's k-steps; the g tile of the next iteration lands while this one is multiplied.
+__global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_backward_mma_kernel(const RbParams p) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const int stage_floats = p.rows_tile * p.pitch;
+  float* s_g = reinterpret_cast<float*>(smem_raw);                                     // [2][R][pitch]
+  float* s_d = s_g + 2 * (size_t)stage_floats;                                         // [R][d_pitch]
+  RsTile* s_cols = reinterpret_cast<RsTile*>(s_d + (size_t)p.rows_tile * p.d_pitch);  // [n_cols]
+  float4* s_frags = reinterpret_cast<float4*>(s_cols + ((p.n_cols + 3) & ~3));       // optional
+
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = tid; i < p.n_cols; i += blockDim.x) s_cols[i] = p.cols[i];
+  const int total_steps = p.hdr->total_steps;
+  const bool frags_in_smem = (size_t)total_steps * 512 <= (size_t)p.frag_smem_bytes;
+  if (frags_in_smem)
+    for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
+
+  const int n_warps = blockDim.x >> 5;
+  int64_t blk = blockIdx.x;
+  if (blk < p.total_blocks) {
+    const int64_t row = blk / p.blocks_per_row, fb = blk - row * p.blocks_per_row;
+    rb_fill(p, row, fb * p.frames_tile, s_g, warp, lane, n_warps);
+  }
+  cp_async_wait_all();
+  __syncthreads();
+  const int r = lane >> 2, c = lane & 3;
+  const int m_tiles = p.rows_tile >> 4;
+  // overlap-add: the owned samples e = (rho - H) orig' + t of a tile, walked with a fixed per-thread stride
+  const int e_step_rows = (int)(blockDim.x / p.orig_r), e_step_t = (int)(blockDim.x % p.orig_r);
+  const int own = p.frames_tile * p.orig_r;
+  const int d_step = p.d_pitch - p.orig_r;  // D address step from frame row rho, tap i to row rho - 1, tap i + orig'
+  for (int it = 0; blk < p.total_blocks; blk += gridDim.x, ++it) {
+    const int b = it & 1;
+    const int64_t nxt = blk + gridDim.x;
+    if (nxt < p.total_blocks) {  // the other buffer's readers finished before the barrier that ended the last iteration
+      const int64_t nrow = nxt / p.blocks_per_row, nfb = nxt - nrow * p.blocks_per_row;
+      rb_fill(p, nrow, nfb * p.frames_tile, s_g + (size_t)(b ^ 1) * stage_floats, warp, lane, n_warps);
+    }
+    const int64_t row = blk / p.blocks_per_row, fb = blk - row * p.blocks_per_row;
+    const int64_t f0 = fb * p.frames_tile;
+    const float* gs = s_g + (size_t)b * stage_floats;
+    int mt = 0, cg = warp;  // item (mt, cg), advanced by n_warps columns at a time
+    while (cg >= p.n_cols) { cg -= p.n_cols; ++mt; }
+    for (; mt < m_tiles;) {
+      const RsTile ct = s_cols[cg];
+      const float* a0 = gs + (size_t)(16 * mt + r) * p.pitch + ct.kstart + c;  // A[f][j] = G[f][j]: rows r and r + 8
+      const float* a1 = a0 + 8 * p.pitch;
+      // three independent accumulator chains (hi*hi, lo*hi, hi*lo), summed in a fixed order
+      float d[3][4];
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) d[ch][q] = 0.f;
+      auto contract = [&](auto in_smem) {
+        const float4* frg = (decltype(in_smem)::value ? s_frags : p.frags) + (size_t)ct.frag_off * 32 + lane;
+#pragma unroll 2
+        for (int s = 0; s < ct.nsteps; ++s) {
+          float4 bf;
+          if constexpr (decltype(in_smem)::value) bf = frg[(size_t)s * 32];
+          else bf = __ldg(frg + (size_t)s * 32);
+          const float av[4] = {a0[8 * s], a1[8 * s], a0[8 * s + 4], a1[8 * s + 4]};
+          uint32_t hi[4], lo[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) split_tf32(av[q], hi[q], lo[q]);
+          mma_tf32(d[0], hi, __float_as_uint(bf.x), __float_as_uint(bf.y));
+          mma_tf32(d[1], lo, __float_as_uint(bf.x), __float_as_uint(bf.y));
+          mma_tf32(d[2], hi, __float_as_uint(bf.z), __float_as_uint(bf.w));
+        }
+      };
+      if (frags_in_smem) contract(std::true_type{});
+      else contract(std::false_type{});
+      // D rows = frame rows 16 mt + r (+ 8); columns 2c, 2c + 1 = taps 8 cg + 2c (+ 1)
+      float* drow = s_d + (size_t)(16 * mt + r) * p.d_pitch + 8 * cg + 2 * c;
+      *reinterpret_cast<float2*>(drow) = make_float2(d[0][0] + (d[1][0] + d[2][0]), d[0][1] + (d[1][1] + d[2][1]));
+      *reinterpret_cast<float2*>(drow + 8 * p.d_pitch) =
+          make_float2(d[0][2] + (d[1][2] + d[2][2]), d[0][3] + (d[1][3] + d[2][3]));
+      cg += n_warps;
+      while (cg >= p.n_cols) { cg -= p.n_cols; ++mt; }
+    }
+    __syncthreads();  // the D tile is complete
+    // overlap-add: owned sample e (0 <= e < F orig') is s = f0 orig' - width + e, tap t = e mod orig' of frame row
+    // rho = H + e / orig'; it sums D[rho - h][t + h orig'] for h = H .. 0 (ascending frames) while t + h orig' < taps
+    float* orow = p.out + row * p.out_row_stride;
+    const int64_t s_own = f0 * p.orig_r - p.width;
+    const int e_lo = s_own < 0 ? (int)min((int64_t)own, -s_own) : 0;
+    const int e_hi = (int)min((int64_t)own, p.length - s_own);
+    int e = e_lo + tid;
+    int rho = p.halo + e / p.orig_r, t = e - (rho - p.halo) * p.orig_r;
+    for (; e < e_hi; e += blockDim.x) {
+      const float* dp = s_d + ((int64_t)rho * p.d_pitch + t + (int64_t)p.halo * (p.orig_r - p.d_pitch));
+      float acc = 0.f;
+      for (int h = p.halo, i = t + p.halo * p.orig_r; h >= 0; --h, i -= p.orig_r, dp += d_step)
+        if (i < p.taps) acc += *dp;
+      orow[s_own + e] = acc;
+      rho += e_step_rows;
+      t += e_step_t;
+      if (t >= p.orig_r) { t -= p.orig_r; ++rho; }
+    }
+    cp_async_wait_all();  // the next tile has landed ...
+    __syncthreads();      // ... for everyone, and the D tile and buffer b are free
+  }
+}
+
+// One input sample per thread (any ratio): its frames in ascending order, over each frame the live phases of tap
+// i = s + width - f orig' from the transposed table.
+__global__ void __launch_bounds__(256)
+resample_backward_direct_kernel(const float* __restrict__ grad, int64_t rows, int64_t g_row_stride, int64_t out_len,
+                                const int2* __restrict__ tap_range, const float* __restrict__ kt, int orig_r, int new_r,
+                                int width, int taps, float* __restrict__ out, int64_t length, int64_t out_row_stride) {
+  for (int64_t row = blockIdx.y; row < rows; row += gridDim.y) {
+    const float* __restrict__ g = grad + row * g_row_stride;
+    for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < length; s += (int64_t)gridDim.x * blockDim.x) {
+      const int64_t u = s + width;
+      const int64_t f_lo = u - taps + 1 <= 0 ? 0 : (u - taps + orig_r) / orig_r;
+      const int64_t f_hi = u / orig_r;
+      float acc = 0.f;
+      for (int64_t f = f_lo; f <= f_hi; ++f) {
+        const int i = (int)(u - f * orig_r);
+        const int2 tr = tap_range[i];
+        const float* __restrict__ k = kt + (size_t)i * new_r;
+        const int64_t base = f * new_r;
+        for (int q = 0; q < tr.y; ++q) {
+          const int j = tr.x + q;
+          if (base + j >= out_len) break;
+          acc = fmaf(k[j], g[base + j], acc);
+        }
+      }
+      out[row * out_row_stride + s] = acc;
+    }
+  }
+}
+
 }  // namespace
 
 size_t resample_workspace_bytes_impl(int new_r, int taps) { return rs_layout(new_r, taps).total; }
+
+size_t resample_backward_workspace_bytes_impl(int orig_r, int new_r, int width) {
+  return rb_layout(orig_r, new_r, width).total;
+}
+
+int resample_backward_prepare_impl(const float* kernel, int orig_r, int new_r, int width, void* ws, size_t ws_bytes,
+                                   cudaStream_t stream) {
+  if (kernel == nullptr || ws == nullptr || orig_r < 1 || new_r < 1 || width < 0) return B200A_EINVAL;
+  const int taps = 2 * width + orig_r;
+  const RbLayout l = rb_layout(orig_r, new_r, width);
+  if (ws_bytes < l.total) return B200A_EWORKSPACE;
+  const RbConfig c = rb_config(orig_r, new_r, width);
+  unsigned char* base = static_cast<unsigned char*>(ws);
+  if (cudaMemsetAsync(base + l.header, 0, sizeof(RsHeader), stream) != cudaSuccess) return B200A_ECUDA;
+  RsHeader* hdr = reinterpret_cast<RsHeader*>(base + l.header);
+  int2* support = reinterpret_cast<int2*>(base + l.support);
+  int2* tap_range = reinterpret_cast<int2*>(base + l.tap_range);
+  float* kt = reinterpret_cast<float*>(base + l.kt);
+  resample_support_kernel<<<(new_r + 7) / 8, 256, 0, stream>>>(kernel, new_r, taps, orig_r, width, hdr, support);
+  const int64_t elems = (int64_t)taps * new_r;
+  const unsigned grid = (unsigned)std::min<int64_t>(std::max<int64_t>((elems + 255) / 256, (taps + 255) / 256), 4096);
+  resample_adjoint_table_kernel<<<grid, 256, 0, stream>>>(kernel, support, new_r, taps, tap_range, kt);
+  if (c.mma)
+    resample_backward_plan_kernel<<<1, 256, 0, stream>>>(kt, tap_range, new_r, taps, c.n_cols, hdr,
+                                                         reinterpret_cast<RsTile*>(base + l.cols),
+                                                         reinterpret_cast<float4*>(base + l.frags));
+  return launch_status();
+}
+
+int resample_backward_impl(const void* ws, int orig_r, int new_r, int width, const float* grad, int64_t rows,
+                           int64_t g_row_stride, int64_t out_len, float* grad_wave, int64_t length,
+                           int64_t grad_row_stride, cudaStream_t stream) {
+  const int taps = 2 * width + orig_r;
+  const RbLayout l = rb_layout(orig_r, new_r, width);
+  const RbConfig c = rb_config(orig_r, new_r, width);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  if (c.mma) {
+    RbParams p{};
+    p.grad = grad;
+    p.g_row_stride = g_row_stride;
+    p.out_len = out_len;
+    p.out = grad_wave;
+    p.length = length;
+    p.out_row_stride = grad_row_stride;
+    p.hdr = reinterpret_cast<const RsHeader*>(base + l.header);
+    p.cols = reinterpret_cast<const RsTile*>(base + l.cols);
+    p.frags = reinterpret_cast<const float4*>(base + l.frags);
+    p.orig_r = orig_r;
+    p.new_r = new_r;
+    p.width = width;
+    p.taps = taps;
+    p.n_cols = c.n_cols;
+    p.halo = c.halo;
+    p.rows_tile = c.rows_tile;
+    p.frames_tile = c.rows_tile - c.halo;
+    p.pitch = c.pitch;
+    p.d_pitch = c.d_pitch;
+    const int64_t own_frames = (length - 1 + width) / orig_r + 1;  // frames whose first tap lands on [0, length)
+    p.blocks_per_row = (own_frames + p.frames_tile - 1) / p.frames_tile;
+    p.total_blocks = rows * p.blocks_per_row;
+    p.frag_smem_bytes = (int)(((size_t)kRsSmemBudget - c.smem_fixed) & ~(size_t)511);
+    const size_t smem = c.smem_fixed + p.frag_smem_bytes;
+    const int items = (c.rows_tile / 16) * c.n_cols;
+    int warps = 8;
+    double best_idle = 2.0;
+    for (int w = 8; w <= kRsMaxWarps; ++w) {
+      const int rounds = (items + w - 1) / w;
+      const double idle = 1.0 - (double)items / (double)(rounds * w);
+      if (idle <= best_idle + 1e-9) { best_idle = idle; warps = w; }  // ties go to more warps
+    }
+    return launch_kernel(resample_backward_mma_kernel, persistent_grid(p.total_blocks, 1), warps * 32, smem, stream, p);
+  }
+  unsigned bx = (unsigned)std::min<int64_t>((length + 255) / 256, 4096);
+  dim3 grid(bx, (unsigned)std::min<int64_t>(rows, 65535));
+  resample_backward_direct_kernel<<<grid, 256, 0, stream>>>(
+      grad, rows, g_row_stride, out_len, reinterpret_cast<const int2*>(base + l.tap_range),
+      reinterpret_cast<const float*>(base + l.kt), orig_r, new_r, width, taps, grad_wave, length, grad_row_stride);
+  return launch_status();
+}
 
 int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width, void* ws, size_t ws_bytes,
                           cudaStream_t stream) {

@@ -323,6 +323,28 @@ int b200a_resample_run(const void* workspace, const float* kernel, int32_t orig_
                        int64_t row_stride, float* out, int64_t out_row_stride, int64_t out_len,
                        b200a_stream stream);
 
+/*
+ * Waveform gradient of b200a_resample_run.  With o' = orig_r, n' = new_r, w = width, taps = 2w + o', K the kernel
+ * masked to each phase's live taps (the support b200a_resample_prepare finds) and g the upstream gradient:
+ *   G[f][j] = g[f n' + j] for f n' + j < out_len, else 0;   D = G K   (frames x taps);
+ *   grad_wave[s] = sum_f D[f][s + w - f o']  over the frames with 0 <= s + w - f o' < taps,  0 <= s < length.
+ * The forward workspace and b200a_resample_prepare are unchanged: a resampler that never differentiates pays nothing.
+ */
+/* Bytes of the backward workspace for this ratio; 0 for an invalid one. */
+size_t b200a_resample_backward_workspace_bytes(int32_t orig_r, int32_t new_r, int32_t width);
+/* Adjoint tables from the cached kernel [new_r][2*width + orig_r]: per-phase supports (same rule as the forward),
+ * per-tap live phase ranges + the transposed masked taps (direct kernel), the per-8-tap-column k-step plan and TF32
+ * hi/lo B fragments (mma kernel).  The backward never reads the live `kernel` buffer afterwards.
+ * B200A_EWORKSPACE when workspace_bytes < b200a_resample_backward_workspace_bytes(orig_r, new_r, width). */
+int b200a_resample_backward_prepare(const float* kernel, int32_t orig_r, int32_t new_r, int32_t width,
+                                    void* workspace, size_t workspace_bytes, b200a_stream stream);
+/* grad_wave[r][s], s < length, every sample written; grad row r at grad + r*g_row_stride (0 allowed: expanded
+ * gradients), unit element stride, out_len = b200a_resample_len(length, orig_r, new_r) values per row.
+ * Deterministic, no atomics, every row independent; the kernel is chosen by the ratio alone. */
+int b200a_resample_backward(const void* workspace, int32_t orig_r, int32_t new_r, int32_t width,
+                            const float* grad, int64_t rows, int64_t g_row_stride, int64_t out_len,
+                            float* grad_wave, int64_t length, int64_t grad_row_stride, b200a_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

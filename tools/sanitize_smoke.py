@@ -37,6 +37,9 @@ K.mfcc_batch(x * 1000, subtract_mean=True)
 K.spectrogram_batch(x * 1000)
 T.Resample(44100, 16000).cuda()(x)
 T.Resample(16000, 22050, resampling_method="sinc_interp_kaiser").cuda()(x)
+with audio_b200.differentiable(resample=True):  # resampler waveform gradients: the mma kernel, the direct kernel
+    for o, n in ((44100, 16000), (2003, 1999)):
+        T.Resample(o, n).cuda()(x.clone().requires_grad_()).sum().backward()
 T.GriffinLim(n_fft=512, hop_length=128, n_iter=3, length=12000, rand_init=False).cuda()(
     T.Spectrogram(n_fft=512, hop_length=128).cuda()(x))
 T.PitchShift(16000, 12).cuda()(x)
