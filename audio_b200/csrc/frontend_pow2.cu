@@ -26,6 +26,7 @@
 #include <type_traits>
 #include <utility>
 
+#include "band_mma.cuh"
 #include "common.cuh"
 #include "f32x2.cuh"
 #include "ptx.cuh"
@@ -71,14 +72,8 @@ struct Geo {
 };
 
 // The mel contraction D[16 frames][n_mels] = P[16][bins] * F[bins][n_mels] is cut into ITEMS =
-// groups of 8 filters with the k-steps where the group is non-zero, spread over the contraction warps
-// by descending size.
-struct MelItem {
-  int tile;      // filter group: filters [8 tile, 8 tile + 8)
-  int kstart;    // first bin of the first k-step (multiple of 8)
-  int nsteps;    // k-steps
-  int frag_off;  // index of the first step in the fragment array
-};
+// groups of 8 filters with the k-steps where the group is non-zero (band_mma.cuh's tiles), spread over the
+// contraction warps by descending size.
 struct MelPlan {  // built on the device by prepare_mma_kernel
   int n_tiles, n_items, total_steps, n_work;
   // n_fft = 2048 kernel: the filter groups of each of its kMelWarps contraction warps
@@ -87,7 +82,7 @@ struct MelPlan {  // built on the device by prepare_mma_kernel
   // 16-warp mel kernel: warp w contracts work[work_begin[w] .. work_begin[w + 1]), entries (16-frame tile << 8) | group
   int work_begin[kUniWarps + 4];
   unsigned short work[kMaxMTiles * kMaxItems];
-  MelItem items[kMaxItems];
+  BandTile items[kMaxItems];
 };
 
 struct Pow2Extra {  // tables appended to the generic workspace
@@ -765,36 +760,18 @@ __global__ void __launch_bounds__(NW * 32, 1) stft_pow2_power_kernel(const Pow2P
 // store.  pw: the tile's 16 power rows (pitch PITCH); o_lo / o_hi, g_lo / g_hi: output offset (or -1) and top_db
 // group of rows r and r + 8 (r = lane / 4).
 template <int PITCH>
-__device__ __forceinline__ void contract_item(const Pow2Params& p, const MelItem& mi, const float4* s_frags,
+__device__ __forceinline__ void contract_item(const Pow2Params& p, const BandTile& mi, const float4* s_frags,
                                               bool frags_in_smem, int lane, const float* pw, int64_t o_lo,
                                               int64_t o_hi, int64_t g_lo, int64_t g_hi, GroupMax& gmax) {
   const int r = lane >> 2, c = lane & 3;
   const float* a_lo_row = pw + (size_t)r * PITCH + mi.kstart + c;
   const float* a_hi_row = a_lo_row + 8 * PITCH;
-  // three independent accumulator chains (hi*hi, lo*hi, hi*lo), summed in a fixed order
-  float d0[4] = {0.f, 0.f, 0.f, 0.f}, d1[4] = {0.f, 0.f, 0.f, 0.f}, d2[4] = {0.f, 0.f, 0.f, 0.f};
-  auto contract = [&](auto in_smem) {
-    const float4* fr = (decltype(in_smem)::value ? s_frags : p.frags) + (size_t)mi.frag_off * 32 + lane;
-#pragma unroll 4
-    for (int s = 0; s < mi.nsteps; ++s) {
-      float4 bf;
-      if constexpr (decltype(in_smem)::value) bf = fr[(size_t)s * 32];
-      else bf = __ldg(fr + (size_t)s * 32);
-      const float av[4] = {a_lo_row[8 * s], a_hi_row[8 * s], a_lo_row[8 * s + 4], a_hi_row[8 * s + 4]};
-      uint32_t hi[4], lo[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) split_tf32(av[q], hi[q], lo[q]);
-      mma_tf32(d0, hi, __float_as_uint(bf.x), __float_as_uint(bf.y));
-      mma_tf32(d1, lo, __float_as_uint(bf.x), __float_as_uint(bf.y));
-      mma_tf32(d2, hi, __float_as_uint(bf.z), __float_as_uint(bf.w));
-    }
-  };
-  if (frags_in_smem) contract(std::true_type{});
-  else contract(std::false_type{});
+  float acc[1][3][4];
+  band_contract<1, 4>(mi, s_frags, p.frags, frags_in_smem, lane, {a_lo_row, a_hi_row}, acc);
   float d[4];
 #pragma unroll
-  for (int q = 0; q < 4; ++q) d[q] = d0[q] + (d1[q] + d2[q]);
-  const int n0 = 8 * mi.tile + 2 * c;
+  for (int q = 0; q < 4; ++q) d[q] = band_sum(acc[0], q);
+  const int n0 = 8 * mi.group + 2 * c;
   const bool n0_ok = n0 < p.n_mels, n1_ok = n0 + 1 < p.n_mels;
   if (p.k_log) {  // Kaldi fbank: log(max(mel, FLT_EPSILON)), kaldi.py:629-631
 #pragma unroll
@@ -849,10 +826,7 @@ __device__ __forceinline__ bool load_mel_plan(const Pow2Params& p, MelPlan* s_pl
   const int* src = reinterpret_cast<const int*>(p.plan);
   int* dst = reinterpret_cast<int*>(s_plan);
   for (int i = tid; i < (int)(sizeof(MelPlan) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
-  const int total_steps = p.plan->total_steps;
-  const bool frags_in_smem = total_steps <= max_steps;
-  if (frags_in_smem)
-    for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
+  const bool frags_in_smem = stage_band_frags(p.frags, p.plan->total_steps, max_steps, s_frags);
   for (int i = tid; i < slots * (pitch - bins); i += blockDim.x) {
     const int r = i / (pitch - bins), c = i - r * (pitch - bins);
     s_pow[r * pitch + bins + c] = 0.f;
@@ -1468,7 +1442,8 @@ __global__ void prepare_tw2d_kernel(float2* tw2d, int G) {
 // every (16-frame tile, group) pair of an iteration spread over the kUniWarps warps the same way.
 __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __restrict__ bands, int n_bins, int n_mels,
                                    int n_tiles, int n_mtiles, MelPlan* plan, float4* frags) {
-  __shared__ int t_kstart[kMaxItems], t_steps[kMaxItems], order[kMaxItems];
+  __shared__ BandTile tiles[kMaxItems];
+  __shared__ int order[kMaxItems];
   __shared__ unsigned char owner[kMaxMTiles * kMaxItems];
   if (threadIdx.x == 0) {
     int total = 0;
@@ -1478,10 +1453,9 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
         const int2 b = bands[m];
         if (b.y > b.x) { lo = min(lo, b.x); hi = max(hi, b.y); }
       }
-      t_kstart[t] = hi > lo ? (lo & ~7) : 0;
-      t_steps[t] = hi > lo ? (hi - t_kstart[t] + 7) / 8 : 0;
-      plan->items[t] = MelItem{t, t_kstart[t], t_steps[t], total};
-      total += t_steps[t];
+      tiles[t] = band_tile(t, lo, hi, total);
+      plan->items[t] = tiles[t];
+      total += tiles[t].nsteps;
     }
     plan->n_tiles = n_tiles;
     plan->n_items = n_tiles;
@@ -1495,14 +1469,14 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
     for (int k = 0; k < n_tiles; ++k) {
       int best = -1;
       for (int i = 0; i < n_tiles; ++i)
-        if (!used[i] && (best < 0 || t_steps[i] > t_steps[best])) best = i;
+        if (!used[i] && (best < 0 || tiles[i].nsteps > tiles[best].nsteps)) best = i;
       used[best] = true;
       order[k] = best;
       int w = 0;
       for (int q = 1; q < kMelWarps; ++q)
         if (load[q] < load[w] || (load[q] == load[w] && plan->warp_cnt[q] < plan->warp_cnt[w])) w = q;
       plan->warp_items[w][plan->warp_cnt[w]++] = best;
-      load[w] += t_steps[best] + 2;  // + epilogue cost
+      load[w] += tiles[best].nsteps + 2;  // + epilogue cost
     }
     // the same for the (tile, group) pairs over the 16 uniform warps, then listed warp by warp
     for (int w = 0; w < kUniWarps; ++w) { load[w] = 0; cnt[w] = 0; }
@@ -1513,7 +1487,7 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
           if (load[q] < load[w] || (load[q] == load[w] && cnt[q] < cnt[w])) w = q;
         owner[k * n_mtiles + mt] = (unsigned char)w;
         ++cnt[w];
-        load[w] += t_steps[order[k]] + 2;
+        load[w] += tiles[order[k]].nsteps + 2;
       }
     int begin = 0;
     for (int w = 0; w < kUniWarps; ++w) {
@@ -1527,20 +1501,9 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
         plan->work[cnt[owner[k * n_mtiles + mt]]++] = (unsigned short)((mt << 8) | order[k]);
   }
   __syncthreads();
-  int off = 0;
-  for (int t = 0; t < n_tiles; ++t) {
-    for (int i = threadIdx.x; i < t_steps[t] * 32; i += blockDim.x) {
-      const int s = i >> 5, lane = i & 31;
-      const int n = 8 * t + (lane >> 2);
-      const int k0 = t_kstart[t] + 8 * s + (lane & 3), k1 = k0 + 4;
-      const float b0 = (n < n_mels && k0 < n_bins) ? fb[(size_t)k0 * n_mels + n] : 0.f;
-      const float b1 = (n < n_mels && k1 < n_bins) ? fb[(size_t)k1 * n_mels + n] : 0.f;
-      const float b0h = __uint_as_float(__float_as_uint(b0) & 0xffffe000u);
-      const float b1h = __uint_as_float(__float_as_uint(b1) & 0xffffe000u);
-      frags[(size_t)(off + s) * 32 + lane] = make_float4(b0h, b1h, b0 - b0h, b1 - b1h);
-    }
-    off += t_steps[t];
-  }
+  for (int t = 0; t < n_tiles; ++t)
+    write_band_frags(tiles[t], frags,
+                     [&](int n, int k) { return (n < n_mels && k < n_bins) ? fb[(size_t)k * n_mels + n] : 0.f; });
 }
 
 static_assert(kMaxItemsPerWarp * kMelWarps >= kMaxItems,

@@ -13,7 +13,8 @@
 // mma.sync.m16n8k8 TF32 tiles of 16 frames x 8 phases over just the k-steps where those 8 phases have
 // live taps, with error-compensated operands (X_hi*K_hi + X_lo*K_hi + X_hi*K_lo, ~2^-21 relative).
 // No padded copy of the input, no (rows, new', frames) intermediate; the output is written already
-// interleaved and truncated.  Each input sample is read from HBM once, each output written once.
+// interleaved and truncated.  Each input sample is read from HBM once, each output written once.  The plan (per
+// phase group its k-steps and hi/lo fragments) and the contraction are the banded product of band_mma.cuh.
 //
 // Fallback (resample_direct_kernel): one output per thread over the phase's live taps.  It runs when
 //   - new' > 1024 (more than kRsMaxTiles groups of 8 phases), or
@@ -24,8 +25,8 @@
 //
 // Adjoint (resample_backward_mma_kernel / resample_backward_direct_kernel): see the section before the host code.
 #include <algorithm>
-#include <type_traits>
 
+#include "band_mma.cuh"
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -37,13 +38,6 @@ constexpr int kRsMaxWarps = 24;      // warps per CTA are chosen per ratio so th
 constexpr int kRsFrames = 32;        // frames per CTA tile (two 16-row MMA tiles)
 constexpr int kRsMaxTiles = 128;     // groups of 8 phases  (new' <= 1024)
 constexpr int kRsSmemBudget = 224 * 1024;
-
-struct RsTile {  // one group of 8 phases
-  int kstart;      // first tap of its first k-step (multiple of 8)
-  int nsteps;      // 8-tap k-steps covering the union of the group's live taps
-  int frag_off;    // first step in the fragment array
-  int pad;         // keeps a tile 16 bytes: one vector load
-};
 
 struct RsHeader {
   uint32_t magic;
@@ -58,6 +52,25 @@ struct RsLayout {
 
 inline int rs_tiles(int new_r) { return (new_r + 7) / 8; }
 
+// Warps per CTA of the mma kernels for `items` equal warp items per tile: the count in [8, kRsMaxWarps] that leaves the
+// fewest warps idle in the last round (ties go to more warps).
+inline int rs_warps(int items) {
+  int warps = 8;
+  double best_idle = 2.0;
+  for (int w = 8; w <= kRsMaxWarps; ++w) {
+    const int rounds = (items + w - 1) / w;
+    const double idle = 1.0 - (double)items / (double)(rounds * w);
+    if (idle <= best_idle + 1e-9) { best_idle = idle; warps = w; }
+  }
+  return warps;
+}
+
+// Shared memory granted to an mma kernel's fragment copy: what smem_fixed leaves of the budget, in whole 512-byte
+// k-steps.  The kernel stages the fragments when the plan's step count fits, otherwise it reads them through L1.
+inline int rs_frag_smem_bytes(size_t smem_fixed) {
+  return (int)(((size_t)kRsSmemBudget - smem_fixed) & ~(size_t)511);
+}
+
 inline RsLayout rs_layout(int new_r, int taps) {
   RsLayout l{};
   size_t off = 0;
@@ -66,7 +79,7 @@ inline RsLayout rs_layout(int new_r, int taps) {
   l.support = off;
   off = align_up(off + sizeof(int2) * (size_t)new_r, 256);
   l.tiles = off;
-  off = align_up(off + sizeof(RsTile) * (size_t)rs_tiles(new_r), 256);
+  off = align_up(off + sizeof(BandTile) * (size_t)rs_tiles(new_r), 256);
   l.frags = off;  // worst case: every group spans every tap
   const size_t nt = rs_tiles(new_r) <= kRsMaxTiles ? rs_tiles(new_r) : 0;
   off = align_up(off + sizeof(float4) * 32 * nt * ((size_t)taps / 8 + 2), 256);
@@ -110,43 +123,31 @@ __global__ void resample_support_kernel(const float* __restrict__ kernel, int ne
   }
 }
 
-// Per group of 8 phases: the k-steps its live taps span, and the taps split into TF32 hi/lo parts in
-// mma.m16n8k8 B-fragment order (B[k][n] = K[8 t + n][kstart + k]).
-__global__ void resample_plan_kernel(const float* __restrict__ kernel, const int2* __restrict__ support, int new_r,
-                                     int taps, int n_tiles, RsHeader* hdr, RsTile* tiles, float4* frags) {
+// The banded-product plan of a row-major matrix M[rows][k] whose row i is live on k in [range[i].x, range[i].x +
+// range[i].y): per group of 8 rows the k-steps covering the union of their ranges, and M split into TF32 hi/lo
+// B fragments (B[k][n] = M[n][k]).  The forward plans K[phases][taps] over the supports, the adjoint kt[taps][phases]
+// over the tap hulls.
+__global__ void resample_plan_kernel(const float* __restrict__ m, const int2* __restrict__ range, int rows, int k,
+                                     int n_groups, RsHeader* hdr, BandTile* tiles, float4* frags) {
   if (threadIdx.x == 0) {
     int acc = 0;
-    for (int t = 0; t < n_tiles; ++t) {
-      int lo = taps, hi = 0;
-      for (int j = 8 * t; j < min(8 * t + 8, new_r); ++j) {
-        const int2 sp = support[j];
-        if (sp.y > 0) { lo = min(lo, sp.x); hi = max(hi, sp.x + sp.y); }
+    for (int g = 0; g < n_groups; ++g) {
+      int lo = k, hi = 0;
+      for (int i = 8 * g; i < min(8 * g + 8, rows); ++i) {
+        const int2 r = range[i];
+        if (r.y > 0) { lo = min(lo, r.x); hi = max(hi, r.x + r.y); }
       }
-      RsTile rt{0, 0, acc, 0};
-      if (hi > lo) {
-        rt.kstart = lo & ~7;
-        rt.nsteps = (hi - rt.kstart + 7) / 8;
-      }
-      tiles[t] = rt;
-      acc += rt.nsteps;
+      const BandTile t = band_tile(g, lo, hi, acc);
+      tiles[g] = t;
+      acc += t.nsteps;
     }
-    hdr->n_tiles = n_tiles;
+    hdr->n_tiles = n_groups;
     hdr->total_steps = acc;
   }
   __syncthreads();
-  for (int t = 0; t < n_tiles; ++t) {
-    const RsTile rt = tiles[t];
-    for (int i = threadIdx.x; i < rt.nsteps * 32; i += blockDim.x) {
-      const int s = i >> 5, lane = i & 31;
-      const int j = 8 * t + (lane >> 2);
-      const int k0 = rt.kstart + 8 * s + (lane & 3), k1 = k0 + 4;
-      const float b0 = (j < new_r && k0 < taps) ? kernel[(size_t)j * taps + k0] : 0.f;
-      const float b1 = (j < new_r && k1 < taps) ? kernel[(size_t)j * taps + k1] : 0.f;
-      const float b0h = __uint_as_float(__float_as_uint(b0) & 0xffffe000u);
-      const float b1h = __uint_as_float(__float_as_uint(b1) & 0xffffe000u);
-      frags[(size_t)(rt.frag_off + s) * 32 + lane] = make_float4(b0h, b1h, b0 - b0h, b1 - b1h);
-    }
-  }
+  for (int g = 0; g < n_groups; ++g)
+    write_band_frags(tiles[g], frags,
+                     [&](int n, int kk) { return (n < rows && kk < k) ? m[(size_t)n * k + kk] : 0.f; });
 }
 
 struct RsParams {
@@ -155,7 +156,7 @@ struct RsParams {
   float* out;
   int64_t out_row_stride, out_len;
   const RsHeader* hdr;
-  const RsTile* tiles;
+  const BandTile* tiles;
   const float4* frags;
   int orig_r, new_r, width, taps, n_tiles;
   int64_t frames;           // output frames per row = ceil(out_len / new_r)
@@ -226,15 +227,12 @@ __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_mma_kernel(const
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* s_x = reinterpret_cast<float*>(smem_raw);                              // [2][xs_floats]
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_x + 2 * (size_t)p.xs_floats);  // [2]
-  RsTile* s_tiles = reinterpret_cast<RsTile*>(s_bar + 2);                       // [n_tiles]
+  BandTile* s_tiles = reinterpret_cast<BandTile*>(s_bar + 2);                   // [n_tiles]
   float4* s_frags = reinterpret_cast<float4*>(s_tiles + ((p.n_tiles + 3) & ~3));  // optional
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = tid; i < p.n_tiles; i += blockDim.x) s_tiles[i] = p.tiles[i];
-  const int total_steps = p.hdr->total_steps;
-  const bool frags_in_smem = (size_t)total_steps * 512 <= (size_t)p.frag_smem_bytes;
-  if (frags_in_smem)
-    for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
+  const bool frags_in_smem = stage_band_frags(p.frags, p.hdr->total_steps, p.frag_smem_bytes / 512, s_frags);
   if (tid == 0) {
     mbar_init(s_bar + 0, 1);
     mbar_init(s_bar + 1, 1);
@@ -269,7 +267,7 @@ __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_mma_kernel(const
     const float* xs = s_x + (size_t)b * p.xs_floats + shift[b];
     float* orow = p.out + row * p.out_row_stride;
     for (int t = warp; t < p.n_tiles; t += n_warps) {  // one phase group, both 16-frame halves
-      const RsTile rt = s_tiles[t];
+      const BandTile rt = s_tiles[t];
       // A[f][i] = xs[f*orig' + i].  MMA row rho of 16-frame half h is frame_of(S, h, rho): the 8 rows one load
       // instruction touches are S frames apart so that their 4-word windows fall into different banks
       // (S*orig' == 4 (mod 8) words for odd orig').
@@ -280,36 +278,8 @@ __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_mma_kernel(const
         fr[q] = frame_of(p.row_spread, q >> 1, r + 8 * (q & 1));
         arow[q] = xs + (size_t)fr[q] * p.orig_r + rt.kstart + c;
       }
-      // per half: three independent accumulator chains (hi*hi, lo*hi, hi*lo), summed in a fixed order
-      float d[2][3][4];
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int ch = 0; ch < 3; ++ch)
-#pragma unroll
-          for (int q = 0; q < 4; ++q) d[h][ch][q] = 0.f;
-      auto contract = [&](auto in_smem) {
-        const float4* frg = (decltype(in_smem)::value ? s_frags : p.frags) + (size_t)rt.frag_off * 32 + lane;
-#pragma unroll 2
-        for (int s = 0; s < rt.nsteps; ++s) {
-          float4 bf;
-          if constexpr (decltype(in_smem)::value) bf = frg[(size_t)s * 32];
-          else bf = __ldg(frg + (size_t)s * 32);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const float av[4] = {arow[2 * h][8 * s], arow[2 * h + 1][8 * s], arow[2 * h][8 * s + 4],
-                                 arow[2 * h + 1][8 * s + 4]};
-            uint32_t hi[4], lo[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) split_tf32(av[q], hi[q], lo[q]);
-            mma_tf32(d[h][0], hi, __float_as_uint(bf.x), __float_as_uint(bf.y));
-            mma_tf32(d[h][1], lo, __float_as_uint(bf.x), __float_as_uint(bf.y));
-            mma_tf32(d[h][2], hi, __float_as_uint(bf.z), __float_as_uint(bf.w));
-          }
-        }
-      };
-      if (frags_in_smem) contract(std::true_type{});
-      else contract(std::false_type{});
+      float d[2][3][4];  // both halves share each B fragment load
+      band_contract<2, 2>(rt, s_frags, p.frags, frags_in_smem, lane, arow, d);
       // D rows = frames; columns 2c, 2c+1 = phases 8t + 2c (+1): out index = f*new' + phase
       const int j0 = 8 * t + 2 * c;
       const bool pair_ok = j0 + 1 < p.new_r && (p.new_r & 1) == 0 && (p.out_row_stride & 1) == 0;
@@ -317,8 +287,7 @@ __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_mma_kernel(const
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int half_row = 0; half_row < 2; ++half_row) {
-          const float v0 = d[h][0][2 * half_row] + (d[h][1][2 * half_row] + d[h][2][2 * half_row]);
-          const float v1 = d[h][0][2 * half_row + 1] + (d[h][1][2 * half_row + 1] + d[h][2][2 * half_row + 1]);
+          const float v0 = band_sum(d[h], 2 * half_row), v1 = band_sum(d[h], 2 * half_row + 1);
           const int64_t m = (f0 + fr[2 * h + half_row]) * p.new_r + j0;
           if (pair_ok && m + 1 < p.out_len) {
             *reinterpret_cast<float2*>(orow + m) = make_float2(v0, v1);  // m even, row pitch even: 8-byte aligned
@@ -366,8 +335,9 @@ resample_direct_kernel(const float* __restrict__ wave, int64_t length, int64_t r
 // Backward workspace: header | support[new'] | tap_range[taps] | kt[taps][new'] | cols[n_cols] | frags.
 //   tap_range[i] = (first phase, count) of the hull of the phases whose live taps include tap i;
 //   kt[i][j]     = K[j][i] when tap i is live for phase j, else 0 (gaps inside a hull read zeros);
-//   cols / frags = per group of 8 taps the 8-phase k-steps covering the union of its taps' hulls, and the masked taps as
-//                  TF32 hi/lo B fragments (only for ratios the mma kernel takes).
+//   cols / frags = the forward's banded-product plan, run on kt and tap_range: per group of 8 taps the 8-phase k-steps
+//                  covering the union of its taps' hulls, and the masked taps as TF32 hi/lo B fragments (only for
+//                  ratios the mma kernel takes).
 constexpr int kRbMaxRows = 512;  // staged frame rows per tile (halo + owned)
 
 // Tile geometry of resample_backward_mma_kernel: a function of the ratio alone, never of the batch.
@@ -390,7 +360,7 @@ inline RbConfig rb_config(int orig_r, int new_r, int width) {
   c.d_pitch = 8 * c.n_cols + ((8 - (8 * c.n_cols) % 32) + 32) % 32;
   if (rs_tiles(new_r) > kRsMaxTiles) return c;
   auto fixed = [&](int R) {
-    return sizeof(float) * ((size_t)2 * R * c.pitch + (size_t)R * c.d_pitch) + sizeof(RsTile) * ((c.n_cols + 3) & ~3);
+    return sizeof(float) * ((size_t)2 * R * c.pitch + (size_t)R * c.d_pitch) + sizeof(BandTile) * ((c.n_cols + 3) & ~3);
   };
   // the smallest R that keeps the recomputed halo at <= 1/16 of the rows (and R >= 32) and gives a tile at least 4096
   // owned samples (fewer per-tile barriers for short frames), or the largest that fits
@@ -425,7 +395,7 @@ inline RbLayout rb_layout(int orig_r, int new_r, int width) {
   l.cols = off;
   l.frags = off;
   if (c.mma) {
-    off = align_up(off + sizeof(RsTile) * (size_t)c.n_cols, 256);
+    off = align_up(off + sizeof(BandTile) * (size_t)c.n_cols, 256);
     l.frags = off;  // worst case: every tap group spans every phase group
     off = align_up(off + sizeof(float4) * 32 * (size_t)c.n_cols * rs_tiles(new_r), 256);
   }
@@ -455,53 +425,13 @@ __global__ void resample_adjoint_table_kernel(const float* __restrict__ kernel, 
   }
 }
 
-// Per group of 8 taps: the 8-phase k-steps covering the union of its taps' hulls, and kt split into TF32 hi/lo parts in
-// mma.m16n8k8 B-fragment order (B[k][n] = kt[8 c + n][kstart + k]).
-__global__ void resample_backward_plan_kernel(const float* __restrict__ kt, const int2* __restrict__ tap_range,
-                                              int new_r, int taps, int n_cols, RsHeader* hdr, RsTile* cols,
-                                              float4* frags) {
-  if (threadIdx.x == 0) {
-    int acc = 0;
-    for (int cg = 0; cg < n_cols; ++cg) {
-      int lo = new_r, hi = 0;
-      for (int i = 8 * cg; i < min(8 * cg + 8, taps); ++i) {
-        const int2 tr = tap_range[i];
-        if (tr.y > 0) { lo = min(lo, tr.x); hi = max(hi, tr.x + tr.y); }
-      }
-      RsTile ct{0, 0, acc, 0};
-      if (hi > lo) {
-        ct.kstart = lo & ~7;
-        ct.nsteps = (hi - ct.kstart + 7) / 8;
-      }
-      cols[cg] = ct;
-      acc += ct.nsteps;
-    }
-    hdr->n_tiles = n_cols;
-    hdr->total_steps = acc;
-  }
-  __syncthreads();
-  for (int cg = 0; cg < n_cols; ++cg) {
-    const RsTile ct = cols[cg];
-    for (int e = threadIdx.x; e < ct.nsteps * 32; e += blockDim.x) {
-      const int s = e >> 5, lane = e & 31;
-      const int i = 8 * cg + (lane >> 2);
-      const int j0 = ct.kstart + 8 * s + (lane & 3), j1 = j0 + 4;
-      const float b0 = (i < taps && j0 < new_r) ? kt[(size_t)i * new_r + j0] : 0.f;
-      const float b1 = (i < taps && j1 < new_r) ? kt[(size_t)i * new_r + j1] : 0.f;
-      const float b0h = __uint_as_float(__float_as_uint(b0) & 0xffffe000u);
-      const float b1h = __uint_as_float(__float_as_uint(b1) & 0xffffe000u);
-      frags[(size_t)(ct.frag_off + s) * 32 + lane] = make_float4(b0h, b1h, b0 - b0h, b1 - b1h);
-    }
-  }
-}
-
 struct RbParams {
   const float* grad;
   int64_t g_row_stride, out_len;
   float* out;
   int64_t length, out_row_stride;
   const RsHeader* hdr;
-  const RsTile* cols;
+  const BandTile* cols;
   const float4* frags;
   int orig_r, new_r, width, taps, n_cols;
   int halo, rows_tile, frames_tile, pitch, d_pitch;
@@ -533,17 +463,14 @@ __device__ __forceinline__ void rb_fill(const RbParams& p, int64_t row, int64_t 
 __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_backward_mma_kernel(const RbParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int stage_floats = p.rows_tile * p.pitch;
-  float* s_g = reinterpret_cast<float*>(smem_raw);                                     // [2][R][pitch]
-  float* s_d = s_g + 2 * (size_t)stage_floats;                                         // [R][d_pitch]
-  RsTile* s_cols = reinterpret_cast<RsTile*>(s_d + (size_t)p.rows_tile * p.d_pitch);  // [n_cols]
-  float4* s_frags = reinterpret_cast<float4*>(s_cols + ((p.n_cols + 3) & ~3));       // optional
+  float* s_g = reinterpret_cast<float*>(smem_raw);                                         // [2][R][pitch]
+  float* s_d = s_g + 2 * (size_t)stage_floats;                                             // [R][d_pitch]
+  BandTile* s_cols = reinterpret_cast<BandTile*>(s_d + (size_t)p.rows_tile * p.d_pitch);  // [n_cols]
+  float4* s_frags = reinterpret_cast<float4*>(s_cols + ((p.n_cols + 3) & ~3));           // optional
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = tid; i < p.n_cols; i += blockDim.x) s_cols[i] = p.cols[i];
-  const int total_steps = p.hdr->total_steps;
-  const bool frags_in_smem = (size_t)total_steps * 512 <= (size_t)p.frag_smem_bytes;
-  if (frags_in_smem)
-    for (int i = tid; i < total_steps * 32; i += blockDim.x) s_frags[i] = p.frags[i];
+  const bool frags_in_smem = stage_band_frags(p.frags, p.hdr->total_steps, p.frag_smem_bytes / 512, s_frags);
 
   const int n_warps = blockDim.x >> 5;
   int64_t blk = blockIdx.x;
@@ -572,38 +499,15 @@ __global__ void __launch_bounds__(kRsMaxWarps * 32, 1) resample_backward_mma_ker
     int mt = 0, cg = warp;  // item (mt, cg), advanced by n_warps columns at a time
     while (cg >= p.n_cols) { cg -= p.n_cols; ++mt; }
     for (; mt < m_tiles;) {
-      const RsTile ct = s_cols[cg];
+      const BandTile ct = s_cols[cg];
       const float* a0 = gs + (size_t)(16 * mt + r) * p.pitch + ct.kstart + c;  // A[f][j] = G[f][j]: rows r and r + 8
       const float* a1 = a0 + 8 * p.pitch;
-      // three independent accumulator chains (hi*hi, lo*hi, hi*lo), summed in a fixed order
-      float d[3][4];
-#pragma unroll
-      for (int ch = 0; ch < 3; ++ch)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) d[ch][q] = 0.f;
-      auto contract = [&](auto in_smem) {
-        const float4* frg = (decltype(in_smem)::value ? s_frags : p.frags) + (size_t)ct.frag_off * 32 + lane;
-#pragma unroll 2
-        for (int s = 0; s < ct.nsteps; ++s) {
-          float4 bf;
-          if constexpr (decltype(in_smem)::value) bf = frg[(size_t)s * 32];
-          else bf = __ldg(frg + (size_t)s * 32);
-          const float av[4] = {a0[8 * s], a1[8 * s], a0[8 * s + 4], a1[8 * s + 4]};
-          uint32_t hi[4], lo[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) split_tf32(av[q], hi[q], lo[q]);
-          mma_tf32(d[0], hi, __float_as_uint(bf.x), __float_as_uint(bf.y));
-          mma_tf32(d[1], lo, __float_as_uint(bf.x), __float_as_uint(bf.y));
-          mma_tf32(d[2], hi, __float_as_uint(bf.z), __float_as_uint(bf.w));
-        }
-      };
-      if (frags_in_smem) contract(std::true_type{});
-      else contract(std::false_type{});
+      float d[1][3][4];
+      band_contract<1, 2>(ct, s_frags, p.frags, frags_in_smem, lane, {a0, a1}, d);
       // D rows = frame rows 16 mt + r (+ 8); columns 2c, 2c + 1 = taps 8 cg + 2c (+ 1)
       float* drow = s_d + (size_t)(16 * mt + r) * p.d_pitch + 8 * cg + 2 * c;
-      *reinterpret_cast<float2*>(drow) = make_float2(d[0][0] + (d[1][0] + d[2][0]), d[0][1] + (d[1][1] + d[2][1]));
-      *reinterpret_cast<float2*>(drow + 8 * p.d_pitch) =
-          make_float2(d[0][2] + (d[1][2] + d[2][2]), d[0][3] + (d[1][3] + d[2][3]));
+      *reinterpret_cast<float2*>(drow) = make_float2(band_sum(d[0], 0), band_sum(d[0], 1));
+      *reinterpret_cast<float2*>(drow + 8 * p.d_pitch) = make_float2(band_sum(d[0], 2), band_sum(d[0], 3));
       cg += n_warps;
       while (cg >= p.n_cols) { cg -= p.n_cols; ++mt; }
     }
@@ -686,9 +590,9 @@ int resample_backward_prepare_impl(const float* kernel, int orig_r, int new_r, i
   const unsigned grid = (unsigned)std::min<int64_t>(std::max<int64_t>((elems + 255) / 256, (taps + 255) / 256), 4096);
   resample_adjoint_table_kernel<<<grid, 256, 0, stream>>>(kernel, support, new_r, taps, tap_range, kt);
   if (c.mma)
-    resample_backward_plan_kernel<<<1, 256, 0, stream>>>(kt, tap_range, new_r, taps, c.n_cols, hdr,
-                                                         reinterpret_cast<RsTile*>(base + l.cols),
-                                                         reinterpret_cast<float4*>(base + l.frags));
+    resample_plan_kernel<<<1, 256, 0, stream>>>(kt, tap_range, taps, new_r, c.n_cols, hdr,
+                                                reinterpret_cast<BandTile*>(base + l.cols),
+                                                reinterpret_cast<float4*>(base + l.frags));
   return launch_status();
 }
 
@@ -708,7 +612,7 @@ int resample_backward_impl(const void* ws, int orig_r, int new_r, int width, con
     p.length = length;
     p.out_row_stride = grad_row_stride;
     p.hdr = reinterpret_cast<const RsHeader*>(base + l.header);
-    p.cols = reinterpret_cast<const RsTile*>(base + l.cols);
+    p.cols = reinterpret_cast<const BandTile*>(base + l.cols);
     p.frags = reinterpret_cast<const float4*>(base + l.frags);
     p.orig_r = orig_r;
     p.new_r = new_r;
@@ -723,16 +627,9 @@ int resample_backward_impl(const void* ws, int orig_r, int new_r, int width, con
     const int64_t own_frames = (length - 1 + width) / orig_r + 1;  // frames whose first tap lands on [0, length)
     p.blocks_per_row = (own_frames + p.frames_tile - 1) / p.frames_tile;
     p.total_blocks = rows * p.blocks_per_row;
-    p.frag_smem_bytes = (int)(((size_t)kRsSmemBudget - c.smem_fixed) & ~(size_t)511);
+    p.frag_smem_bytes = rs_frag_smem_bytes(c.smem_fixed);
     const size_t smem = c.smem_fixed + p.frag_smem_bytes;
-    const int items = (c.rows_tile / 16) * c.n_cols;
-    int warps = 8;
-    double best_idle = 2.0;
-    for (int w = 8; w <= kRsMaxWarps; ++w) {
-      const int rounds = (items + w - 1) / w;
-      const double idle = 1.0 - (double)items / (double)(rounds * w);
-      if (idle <= best_idle + 1e-9) { best_idle = idle; warps = w; }  // ties go to more warps
-    }
+    const int warps = rs_warps((c.rows_tile / 16) * c.n_cols);  // items: (16-row M tile, tap group)
     return launch_kernel(resample_backward_mma_kernel, persistent_grid(p.total_blocks, 1), warps * 32, smem, stream, p);
   }
   unsigned bx = (unsigned)std::min<int64_t>((length + 255) / 256, 4096);
@@ -756,7 +653,7 @@ int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width,
   resample_support_kernel<<<(new_r + 7) / 8, 256, 0, stream>>>(kernel, new_r, taps, orig_r, width, hdr, support);
   if (rs_tiles(new_r) <= kRsMaxTiles)
     resample_plan_kernel<<<1, 256, 0, stream>>>(kernel, support, new_r, taps, rs_tiles(new_r), hdr,
-                                                reinterpret_cast<RsTile*>(base + l.tiles),
+                                                reinterpret_cast<BandTile*>(base + l.tiles),
                                                 reinterpret_cast<float4*>(base + l.frags));
   return launch_status();
 }
@@ -774,7 +671,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
   // ---- tensor-pipe path -------------------------------------------------------------------------
   const int n_tiles = rs_tiles(new_r);
   const int xs_floats = (kRsFrames * orig_r + taps + 16 + 4 + 3) & ~3;  // rs_fill's span + its alignment shift
-  const size_t smem_fixed = sizeof(float) * 2 * (size_t)xs_floats + 16 + sizeof(RsTile) * ((n_tiles + 3) & ~3);
+  const size_t smem_fixed = sizeof(float) * 2 * (size_t)xs_floats + 16 + sizeof(BandTile) * ((n_tiles + 3) & ~3);
   const bool aligned = (reinterpret_cast<uintptr_t>(wave) & 3) == 0;  // any float pointer; rows may have any pitch
   if (n_tiles <= kRsMaxTiles && aligned && smem_fixed + 1024 <= (size_t)kRsSmemBudget) {
     RsParams p{};
@@ -786,7 +683,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
     p.out_row_stride = out_row_stride;
     p.out_len = out_len;
     p.hdr = reinterpret_cast<const RsHeader*>(base + l.header);
-    p.tiles = reinterpret_cast<const RsTile*>(base + l.tiles);
+    p.tiles = reinterpret_cast<const BandTile*>(base + l.tiles);
     p.frags = reinterpret_cast<const float4*>(base + l.frags);
     p.orig_r = orig_r;
     p.new_r = new_r;
@@ -797,9 +694,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
     p.blocks_per_row = (p.frames + kRsFrames - 1) / kRsFrames;
     p.total_blocks = rows * p.blocks_per_row;
     p.xs_floats = xs_floats;
-    // fragments go to shared memory when they fit next to the staging buffers (the kernel compares the
-    // device-side step count with the room granted here), otherwise they are read through L1
-    p.frag_smem_bytes = (int)(((size_t)kRsSmemBudget - smem_fixed) & ~(size_t)511);  // everything that is left
+    p.frag_smem_bytes = rs_frag_smem_bytes(smem_fixed);
     const size_t smem = smem_fixed + p.frag_smem_bytes;
     // row spread: the candidate with the fewest shared-memory bank conflicts for one A-fragment load
     // (8 rows x 4 consecutive words, rows spread*orig' words apart)
@@ -815,15 +710,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
       if (worst < best_conf) { best_conf = worst; best_spread = spread; }
     }
     p.row_spread = best_spread;
-    // warps: n_tiles items (phase groups) per tile; prefer the largest count that divides them evenly
-    const int items = n_tiles;
-    int warps = 8;
-    double best_idle = 2.0;
-    for (int w = 8; w <= kRsMaxWarps; ++w) {
-      const int rounds = (items + w - 1) / w;
-      const double idle = 1.0 - (double)items / (double)(rounds * w);
-      if (idle <= best_idle + 1e-9) { best_idle = idle; warps = w; }  // ties go to more warps
-    }
+    const int warps = rs_warps(n_tiles);  // items: phase groups
     return launch_kernel(resample_mma_kernel, persistent_grid(p.total_blocks, 1), warps * 32, smem, stream, p);
   }
 
