@@ -1461,7 +1461,8 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
     plan->n_items = n_tiles;
     plan->total_steps = total;
     plan->n_work = n_mtiles * n_tiles;
-    // longest-processing-time-first assignment of the groups to the contraction warps
+    // longest-processing-time-first assignment of the groups to the contraction warps whose lists have room (a skewed
+    // bank, a few full-band groups and many empty ones, would otherwise pile more than kMaxItemsPerWarp on one warp)
     int load[kUniWarps], cnt[kUniWarps];
     bool used[kMaxItems];
     for (int w = 0; w < kMelWarps; ++w) { load[w] = 0; plan->warp_cnt[w] = 0; }
@@ -1472,9 +1473,11 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
         if (!used[i] && (best < 0 || tiles[i].nsteps > tiles[best].nsteps)) best = i;
       used[best] = true;
       order[k] = best;
-      int w = 0;
-      for (int q = 1; q < kMelWarps; ++q)
-        if (load[q] < load[w] || (load[q] == load[w] && plan->warp_cnt[q] < plan->warp_cnt[w])) w = q;
+      int w = -1;
+      for (int q = 0; q < kMelWarps; ++q)
+        if (plan->warp_cnt[q] < kMaxItemsPerWarp &&
+            (w < 0 || load[q] < load[w] || (load[q] == load[w] && plan->warp_cnt[q] < plan->warp_cnt[w])))
+          w = q;
       plan->warp_items[w][plan->warp_cnt[w]++] = best;
       load[w] += tiles[best].nsteps + 2;  // + epilogue cost
     }
@@ -1506,6 +1509,9 @@ __global__ void prepare_mma_kernel(const float* __restrict__ fb, const int2* __r
                      [&](int n, int k) { return (n < n_mels && k < n_bins) ? fb[(size_t)k * n_mels + n] : 0.f; });
 }
 
+// prepare_mma_kernel gives a group only to a warp with fewer than kMaxItemsPerWarp groups; while groups remain, the
+// warps hold fewer than kMaxItems <= kMelWarps * kMaxItemsPerWarp of them, so one such warp always exists.  (The 16-warp
+// kernel's work list is one array of kMaxMTiles * kMaxItems entries, cut into per-warp ranges: no per-warp cap.)
 static_assert(kMaxItemsPerWarp * kMelWarps >= kMaxItems,
               "every filter group must find a place in a contraction warp's list");
 

@@ -98,14 +98,16 @@ def test_many_filters_take_the_generic_path():
 
 def test_dense_filterbank_matrix():
     """A filterbank without band structure (every bin feeds every filter): fragments no longer fit in
-    shared memory and are streamed from global memory."""
+    shared memory and are streamed from global memory, at every register-FFT size."""
     x = randn(3, 9000, 2)
-    m = T.MelSpectrogram(16000, n_fft=1024, hop_length=256, n_mels=48).to(DEV)
-    fb = torch.rand(513, 48, generator=torch.Generator().manual_seed(9))
-    m.mel_scale.fb.copy_(fb.to(DEV))
-    got = m(x.to(DEV)).cpu().numpy()
-    exp = O.mel_spectrogram(x.numpy(), sample_rate=16000, n_fft=1024, hop_length=256, n_mels=48, fb=fb.numpy())
-    scaled_tol_close(got, exp)
+    for n_fft in (256, 512, 1024, 2048):
+        m = T.MelSpectrogram(16000, n_fft=n_fft, hop_length=n_fft // 4, n_mels=48).to(DEV)
+        fb = torch.rand(n_fft // 2 + 1, 48, generator=torch.Generator().manual_seed(9))
+        m.mel_scale.fb.copy_(fb.to(DEV))
+        got = m(x.to(DEV)).cpu().numpy()
+        exp = O.mel_spectrogram(x.numpy(), sample_rate=16000, n_fft=n_fft, hop_length=n_fft // 4, n_mels=48,
+                                fb=fb.numpy())
+        scaled_tol_close(got, exp, what=f"n_fft={n_fft}")
 
 
 @pytest.mark.parametrize("orig,new", [(44100, 16000), (16000, 44100), (48000, 44100), (16000, 8000), (8000, 16000),

@@ -19,6 +19,14 @@ for n_fft in (256, 512, 1024, 2048, 400):
     T.Spectrogram(n_fft=n_fft, hop_length=n_fft // 4).cuda()(x)
     spec = T.Spectrogram(n_fft=n_fft, hop_length=n_fft // 4, power=None).cuda()(x)
     T.InverseSpectrogram(n_fft=n_fft, hop_length=n_fft // 4).cuda()(spec, 12000)
+# mel plans at their limits: 512 mels with empty filter groups at n_fft 256; at n_fft 2048 a skewed bank (3 full-band
+# groups, 61 empty ones) that would put more than 32 groups on one contraction warp without the per-warp cap
+T.MelSpectrogram(16000, n_fft=256, hop_length=64, n_mels=512).cuda()(x)
+skewed = T.MelSpectrogram(16000, n_fft=2048, hop_length=512, n_mels=512).cuda()
+skewed.mel_scale.fb.zero_()
+for t in (5, 31, 60):
+    skewed.mel_scale.fb[:, 8 * t : 8 * t + 8] = torch.rand(1025, 8, device="cuda")
+skewed(x)
 with audio_b200.differentiable():  # waveform gradients: the fused path (512 / 1024), the composition path (400 / 2048)
     for mod in (T.MelSpectrogram(16000, n_fft=1024, hop_length=256, n_mels=40), T.Spectrogram(n_fft=512, power=1.0),
                 T.Spectrogram(n_fft=512, power=None), T.MelSpectrogram(16000, n_fft=2048, hop_length=512, n_mels=40),
