@@ -101,6 +101,23 @@ _SIGNATURES = {
         ctypes.c_int,
         [c_void_p, c_int64, c_int64, c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p],
     ),
+    "b200a_mfcc_backward_scratch_bytes": (c_size_t, [POINTER(FrontendDesc), c_int64, c_int64, c_int64]),
+    "b200a_mfcc_backward": (
+        ctypes.c_int,
+        [POINTER(FrontendDesc), c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
+         c_int64, c_float, c_void_p, c_void_p, c_void_p],
+    ),
+    "b200a_amplitude_to_db_backward_scratch_bytes": (c_size_t, [c_int64, c_int64]),
+    "b200a_amplitude_to_db_backward": (
+        ctypes.c_int,
+        [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p,
+         c_void_p],
+    ),
+    "b200a_apply_fbank_backward": (
+        ctypes.c_int,
+        [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p],
+    ),
+    "b200a_ratio_backward": (ctypes.c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
     "b200a_istft_run": (
         ctypes.c_int,
         [POINTER(FrontendDesc), c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int64,

@@ -1,6 +1,7 @@
 """``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
-``resample_run`` / ``resample_backward``.
+``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
+``resample_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -22,6 +23,7 @@ from . import _lib
 _DESC_INTS = ("n_fft", "win_length", "hop", "pad", "center", "pad_mode", "onesided", "frame_length_norm", "window_norm",
               "n_mels", "n_mfcc", "log_mels")
 _DESC_FLOATS = ("power", "db_multiplier", "db_amin", "db_offset")
+DESC_N_MELS = _DESC_INTS.index("n_mels")
 
 _LIB = torch.library.Library("b200audio", "DEF")
 _LIB.define(
@@ -39,6 +41,16 @@ _LIB.define(
     "mfcc_finish(Tensor feat, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? group_max, int rows_per_group, "
     "float top_db) -> Tensor"
 )
+_LIB.define(
+    "mfcc_backward(Tensor grad, Tensor feat, Tensor mel, Tensor? group_max, Tensor workspace, int[] desc_i, "
+    "float[] desc_f, int rows_per_group, float top_db) -> Tensor"
+)
+_LIB.define(
+    "amplitude_to_db_backward(Tensor grad, Tensor x, Tensor? group_max, int groups, float multiplier, float amin, "
+    "float offset, float top_db) -> Tensor"
+)
+_LIB.define("apply_fbank_backward(Tensor grad, Tensor fb) -> Tensor")
+_LIB.define("ratio_backward(Tensor grad, Tensor pairs) -> Tensor")
 _LIB.define(
     "resample_run(Tensor wave, Tensor workspace, Tensor kernel, int orig_r, int new_r, int width, int row_stride, "
     "int out_len, int pitch) -> Tensor"
@@ -166,6 +178,94 @@ def _mfcc_finish_meta(feat, workspace, desc_i, desc_f, group_max, rows_per_group
     return feat.new_empty((feat.shape[0], feat.shape[1], int(desc_i[_DESC_INTS.index("n_mfcc")])))
 
 
+# ---- mfcc_backward -----------------------------------------------------------------------------------------------
+def _mfcc_backward_cuda(grad, feat, mel, group_max, workspace, desc_i, desc_f, rows_per_group, top_db):
+    """(rows, T, n_mfcc) cepstral gradient at any element strides -> (rows, T, n_mels) mel-stage gradient."""
+    d = _unpack_desc(desc_i, desc_f)
+    rows, frames, n_mels = mel.shape
+    dev = mel.device
+    gs = grad.stride()
+    lib = _lib.lib()
+    clamp = group_max is not None and top_db >= 0 and not d.log_mels
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, n_mels), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_mfcc_backward_scratch_bytes(d, rows, frames, rows_per_group) if clamp else 0
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
+        rc = lib.b200a_mfcc_backward(
+            d, workspace.data_ptr(), grad.data_ptr(), gs[0], gs[1], gs[2], feat.data_ptr(), mel.data_ptr(),
+            None if group_max is None else group_max.data_ptr(), rows, frames, rows_per_group, float(top_db),
+            None if scratch is None else scratch.data_ptr(), out.data_ptr(), _stream(dev))
+    _lib.check(rc, "mfcc_backward")
+    return out
+
+
+def _mfcc_backward_meta(grad, feat, mel, group_max, workspace, desc_i, desc_f, rows_per_group, top_db):
+    return mel.new_empty(mel.shape)
+
+
+# ---- amplitude_to_db_backward ------------------------------------------------------------------------------------
+def _amplitude_to_db_backward_cuda(grad, x, group_max, groups, multiplier, amin, offset, top_db):
+    """Gradient of amplitude_to_DB on the contiguous input x; ``grad`` is read contiguous or as an expanded scalar
+    (all strides 0) and copied otherwise."""
+    expanded = all(s == 0 for s in grad.stride())
+    if not expanded and not grad.is_contiguous():
+        grad = grad.contiguous()
+    dev = x.device
+    lib = _lib.lib()
+    group_elems = x.numel() // groups if groups > 0 else 0
+    clamp = group_max is not None and top_db >= 0
+    with torch.cuda.device(dev):
+        out = torch.empty(x.shape, dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_amplitude_to_db_backward_scratch_bytes(groups, group_elems) if clamp else 0
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
+        rc = lib.b200a_amplitude_to_db_backward(
+            x.data_ptr(), grad.data_ptr(), 0 if expanded else 1, groups, group_elems, float(multiplier), float(amin), float(offset),
+            float(top_db), None if group_max is None else group_max.data_ptr(),
+            None if scratch is None else scratch.data_ptr(), out.data_ptr(), _stream(dev))
+    _lib.check(rc, "amplitude_to_db_backward")
+    return out
+
+
+def _amplitude_to_db_backward_meta(grad, x, group_max, groups, multiplier, amin, offset, top_db):
+    return x.new_empty(x.shape)
+
+
+# ---- apply_fbank_backward ----------------------------------------------------------------------------------------
+def _apply_fbank_backward_cuda(grad, fb):
+    """(rows, T, n_filters) MelScale output gradient at any element strides -> (rows, T, n_bins) frame-major."""
+    rows, frames, n_filters = grad.shape
+    n_bins = fb.shape[0]
+    dev = grad.device
+    gs = grad.stride()
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, n_bins), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_apply_fbank_backward(grad.data_ptr(), rows, n_filters, frames, gs[0], gs[2], gs[1],
+                                                   fb.data_ptr(), n_bins, out.data_ptr(), _stream(dev))
+    _lib.check(rc, "apply_fbank_backward")
+    return out
+
+
+def _apply_fbank_backward_meta(grad, fb):
+    return grad.new_empty((grad.shape[0], grad.shape[1], fb.shape[0]))
+
+
+# ---- ratio_backward ----------------------------------------------------------------------------------------------
+def _ratio_backward_cuda(grad, pairs):
+    """(rows, T) SpectralCentroid gradient at any element strides -> (rows, T, 2) gradient of the (N, D) pairs."""
+    rows, frames = grad.shape
+    dev = grad.device
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, 2), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_ratio_backward(pairs.data_ptr(), grad.data_ptr(), rows, frames, grad.stride(0),
+                                             grad.stride(1), out.data_ptr(), _stream(dev))
+    _lib.check(rc, "ratio_backward")
+    return out
+
+
+def _ratio_backward_meta(grad, pairs):
+    return pairs.new_empty(pairs.shape)
+
+
 # ---- resample_run ------------------------------------------------------------------------------------------------
 def _resample_run_cuda(wave, workspace, kernel, orig_r, new_r, width, row_stride, out_len, pitch):
     rows, length = wave.shape
@@ -207,6 +307,10 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
                             ("mfcc_finish", _mfcc_finish_cuda, _mfcc_finish_meta),
+                            ("mfcc_backward", _mfcc_backward_cuda, _mfcc_backward_meta),
+                            ("amplitude_to_db_backward", _amplitude_to_db_backward_cuda, _amplitude_to_db_backward_meta),
+                            ("apply_fbank_backward", _apply_fbank_backward_cuda, _apply_fbank_backward_meta),
+                            ("ratio_backward", _ratio_backward_cuda, _ratio_backward_meta),
                             ("resample_run", _resample_run_cuda, _resample_run_meta),
                             ("resample_backward", _resample_backward_cuda, _resample_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
@@ -216,5 +320,9 @@ frontend_run = torch.ops.b200audio.frontend_run
 frontend_backward = torch.ops.b200audio.frontend_backward
 istft_backward = torch.ops.b200audio.istft_backward
 mfcc_finish = torch.ops.b200audio.mfcc_finish
+mfcc_backward = torch.ops.b200audio.mfcc_backward
+amplitude_to_db_backward = torch.ops.b200audio.amplitude_to_db_backward
+apply_fbank_backward = torch.ops.b200audio.apply_fbank_backward
+ratio_backward = torch.ops.b200audio.ratio_backward
 resample_run = torch.ops.b200audio.resample_run
 resample_backward = torch.ops.b200audio.resample_backward

@@ -47,25 +47,34 @@ def is_resample_differentiable() -> bool:
     return getattr(_GRAD_STATE, "resample", False)
 
 
-def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = False) -> None:
+def is_feature_differentiable() -> bool:
+    """Whether MFCC, LFCC, AmplitudeToDB, MelScale and SpectralCentroid accept inputs that require grad (in this
+    thread)."""
+    return getattr(_GRAD_STATE, "features", False)
+
+
+def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = False, features: bool = False) -> None:
     """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
     ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT, ``resample=True``
-    (with ``mode``) the waveform gradients of the resampler.  They are separate switches so that vocoder inference and
-    augmentation code (Speed, SpeedPerturbation) does not build graphs when loss gradients are on."""
+    (with ``mode``) the waveform gradients of the resampler, ``features=True`` (with ``mode``) the input gradients of
+    MFCC, LFCC, AmplitudeToDB, MelScale and SpectralCentroid.  They are separate switches so that vocoder inference and
+    augmentation code (Speed, SpeedPerturbation) does not build graphs when loss gradients are on, and so that the
+    top_db clamp's gradient -- every clamped element's share goes to the group maximum -- is opted into knowingly."""
     _GRAD_STATE.on = bool(mode)
     _GRAD_STATE.inverse = bool(mode) and bool(inverse)
     _GRAD_STATE.resample = bool(mode) and bool(resample)
+    _GRAD_STATE.features = bool(mode) and bool(features)
 
 
 @contextlib.contextmanager
-def differentiable(mode: bool = True, *, inverse: bool = False, resample: bool = False):
+def differentiable(mode: bool = True, *, inverse: bool = False, resample: bool = False, features: bool = False):
     """Context manager form of :func:`set_differentiable`; restores the previous settings on exit."""
-    prev = is_differentiable(), is_inverse_differentiable(), is_resample_differentiable()
-    set_differentiable(mode, inverse=inverse, resample=resample)
+    prev = is_differentiable(), is_inverse_differentiable(), is_resample_differentiable(), is_feature_differentiable()
+    set_differentiable(mode, inverse=inverse, resample=resample, features=features)
     try:
         yield
     finally:
-        set_differentiable(prev[0], inverse=prev[1], resample=prev[2])
+        set_differentiable(prev[0], inverse=prev[1], resample=prev[2], features=prev[3])
 
 
 def _no_autograd(t: torch.Tensor) -> None:
@@ -75,7 +84,9 @@ def _no_autograd(t: torch.Tensor) -> None:
             "torch.inference_mode(), or detach() the input. (Spectrogram, MelSpectrogram and F.spectrogram compute "
             "waveform gradients inside audio_b200.differentiable(); InverseSpectrogram and F.inverse_spectrogram "
             "compute spectrogram gradients inside audio_b200.differentiable(inverse=True); Resample, F.resample, Speed "
-            "and SpeedPerturbation compute waveform gradients inside audio_b200.differentiable(resample=True).)"
+            "and SpeedPerturbation compute waveform gradients inside audio_b200.differentiable(resample=True); MFCC, LFCC, "
+            "AmplitudeToDB, MelScale and SpectralCentroid compute input gradients inside "
+            "audio_b200.differentiable(features=True).)"
         )
 
 
@@ -111,6 +122,36 @@ class _FrontendFunction(torch.autograd.Function):
         (flat,) = ctx.saved_tensors
         grad = _ops.frontend_backward(flat, ctx.ws, ctx.desc_i, ctx.desc_f, ctx.stage, ctx.stride, grad_out)
         return grad, None, None, None, None, None, None, None
+
+
+class _MfccFunction(torch.autograd.Function):
+    """MFCC / LFCC from the packed (rows, L) waveform: the same STAGE_FEAT + mfcc_finish launches as the no-grad path, so
+    the cepstra are bit-identical to it.  Saved: the waveform (save_for_backward), the pre-clamp features, the group
+    maxima and the forward's workspace -- a window, filterbank or DCT edited before backward does not change the
+    gradient.  Backward: the mel stage recomputed, the feature adjoint (b200audio::mfcc_backward), the mel-stage
+    waveform gradient (b200audio::frontend_backward)."""
+
+    @staticmethod
+    def forward(ctx, flat, ws, desc_i, desc_f, frames, stride, groups, rows_per_group, top_db):
+        n_mels = desc_i[_ops.DESC_N_MELS]
+        gmax = new_group_max(groups, flat.device) if groups > 0 else None
+        feat = _ops.frontend_run(flat, ws, desc_i, desc_f, _lib.STAGE_FEAT, frames, n_mels, stride, gmax, rows_per_group)
+        out = _ops.mfcc_finish(feat, ws, desc_i, desc_f, gmax, rows_per_group, top_db)
+        ctx.save_for_backward(flat)
+        ctx.feat, ctx.gmax, ctx.ws = feat, gmax, ws
+        ctx.args = desc_i, desc_f, frames, stride, rows_per_group, top_db
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        (flat,) = ctx.saved_tensors
+        desc_i, desc_f, frames, stride, rows_per_group, top_db = ctx.args
+        mel = _ops.frontend_run(flat, ctx.ws, desc_i, desc_f, _lib.STAGE_MEL, frames, desc_i[_ops.DESC_N_MELS], stride,
+                                None, 1)
+        g_mel = _ops.mfcc_backward(grad_out, ctx.feat, mel, ctx.gmax, ctx.ws, desc_i, desc_f, rows_per_group, top_db)
+        grad = _ops.frontend_backward(flat, ctx.ws, desc_i, desc_f, _lib.STAGE_MEL, stride, g_mel)
+        return grad, None, None, None, None, None, None, None, None
 
 
 def _version_of(t: torch.Tensor) -> int:
@@ -225,36 +266,51 @@ class FrontendPlan:
         group_max: Optional[torch.Tensor] = None,
         rows_per_group: int = 1,
         constants=None,
+        switch=is_differentiable,
     ) -> torch.Tensor:
         """Launch the fused kernel; returns the FRAME-MAJOR result (rows, T, width[, 2]).
 
         ``constants``: ``(name, tensor)`` pairs of the module buffers the workspace was built from, given by the entry
-        points that support waveform gradients (COMPLEX / POWER / MEL stages); ``None`` keeps the call forward-only.
+        points that support waveform gradients (COMPLEX / POWER / MEL stages) when ``switch()`` is on; ``None`` keeps
+        the call forward-only.
         """
         _require_cuda_f32(waveform, "waveform")
-        grad = constants is not None and _wants_grad(waveform, constants)
+        grad = constants is not None and _wants_grad(waveform, constants, switch)
         if not grad:
             _no_autograd(waveform)
-        if waveform.device != ws.device:
-            raise RuntimeError(f"audio_b200: waveform is on {waveform.device} but the module buffers are on {ws.device}")
-        lib = _lib.lib()
-        d = self.desc
-        flat, stride = pack_rows(waveform)
-        rows, length = flat.shape
-        frames = self.frames(length)
-        if frames < 1:
-            raise RuntimeError(
-                f"audio_b200: waveform of {length} samples is too short for n_fft={d.n_fft} "
-                f"(center={bool(d.center)}, pad={d.pad})"
-            )
-        n_bins = lib.b200a_num_bins(d.n_fft, d.onesided)
-        width = d.n_mels if stage >= _lib.STAGE_MEL else n_bins
+        flat, stride, frames = self._pack(ws, waveform)
+        n_bins = _lib.lib().b200a_num_bins(self.desc.n_fft, self.desc.onesided)
+        width = self.desc.n_mels if stage >= _lib.STAGE_MEL else n_bins
         # through the dispatcher (b200audio::frontend_run, audio_b200/_ops.py): allocates `out`, launches on the
         # current stream of the waveform's device, raises on a negative status
         desc_i, desc_f = self._packed_desc()
         if grad:
             return _FrontendFunction.apply(flat, ws, desc_i, desc_f, stage, frames, width, stride)
         return _ops.frontend_run(flat, ws, desc_i, desc_f, stage, frames, width, stride, group_max, rows_per_group)
+
+    def _pack(self, ws: torch.Tensor, waveform: torch.Tensor):
+        """The packed (rows, L) waveform, its row stride and its frame count."""
+        if waveform.device != ws.device:
+            raise RuntimeError(f"audio_b200: waveform is on {waveform.device} but the module buffers are on {ws.device}")
+        d = self.desc
+        flat, stride = pack_rows(waveform)
+        length = flat.shape[1]
+        frames = self.frames(length)
+        if frames < 1:
+            raise RuntimeError(
+                f"audio_b200: waveform of {length} samples is too short for n_fft={d.n_fft} "
+                f"(center={bool(d.center)}, pad={d.pad})"
+            )
+        return flat, stride, frames
+
+    def mfcc_grad(self, ws: torch.Tensor, waveform: torch.Tensor, groups: int, rows_per_group: int,
+                  top_db: Optional[float]) -> torch.Tensor:
+        """The FEAT stage + mfcc_finish of an input that requires grad (the caller checked the feature switch and the
+        constant buffers): the frame-major (rows, T, n_mfcc) cepstra of ``_MfccFunction``.  ``groups`` > 0 clamps."""
+        flat, stride, frames = self._pack(ws, waveform)
+        desc_i, desc_f = self._packed_desc()
+        return _MfccFunction.apply(flat, ws, desc_i, desc_f, frames, stride, groups, rows_per_group,
+                                   -1.0 if top_db is None else float(top_db))
 
     def mfcc_finish(self, ws, feat, group_max, rows_per_group: int, top_db: Optional[float]) -> torch.Tensor:
         desc_i, desc_f = self._packed_desc()

@@ -177,6 +177,65 @@ int b200a_amplitude_to_db(const float* x, int64_t groups, int64_t group_elems, f
                               static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_mfcc_backward_scratch_bytes(const b200a_frontend_desc* desc, int64_t rows, int64_t frames,
+                                         int64_t rows_per_group) {
+  if (validate_desc(desc) != B200A_OK || desc->n_mels <= 0 || desc->n_mfcc <= 0) return 0;
+  if (rows < 0 || frames < 0 || rows_per_group < 1) return 0;
+  return mfcc_backward_scratch(rows, frames, rows_per_group);
+}
+
+int b200a_mfcc_backward(const b200a_frontend_desc* desc, const void* workspace, const float* grad, int64_t g_stride_row,
+                        int64_t g_stride_frame, int64_t g_stride_col, const float* feat, const float* mel,
+                        const float* group_max, int64_t rows, int64_t frames, int64_t rows_per_group, float top_db,
+                        void* scratch, float* grad_mel, b200a_stream stream) {
+  int rc = validate_desc(desc);
+  if (rc != B200A_OK) return rc;
+  if (desc->n_mels <= 0 || desc->n_mfcc <= 0 || rows < 0 || frames < 0) return B200A_EINVAL;
+  if (g_stride_row < 0 || g_stride_frame < 0 || g_stride_col < 0) return B200A_EINVAL;
+  const bool clamp = !desc->log_mels && group_max != nullptr && top_db >= 0.f;
+  if (clamp && rows_per_group < 1) return B200A_EINVAL;
+  if (rows == 0 || frames == 0) return B200A_OK;  // nothing to enqueue (pointers may be null)
+  if (workspace == nullptr || grad == nullptr || mel == nullptr || grad_mel == nullptr) return B200A_EINVAL;
+  if (clamp && (feat == nullptr || scratch == nullptr)) return B200A_EINVAL;
+  return mfcc_backward_impl(desc, workspace, grad, g_stride_row, g_stride_frame, g_stride_col, feat, mel, group_max, rows,
+                            frames, rows_per_group, top_db, scratch, grad_mel, static_cast<cudaStream_t>(stream));
+}
+
+size_t b200a_amplitude_to_db_backward_scratch_bytes(int64_t groups, int64_t group_elems) {
+  if (groups < 0 || group_elems < 0) return 0;
+  return amplitude_to_db_backward_scratch(groups, group_elems);
+}
+
+int b200a_amplitude_to_db_backward(const float* x, const float* grad, int64_t g_stride, int64_t groups, int64_t group_elems,
+                                   float multiplier, float amin, float offset, float top_db, const float* group_max,
+                                   void* scratch, float* grad_x, b200a_stream stream) {
+  if (groups < 0 || group_elems < 0 || (g_stride != 0 && g_stride != 1)) return B200A_EINVAL;
+  if (groups == 0 || group_elems == 0) return B200A_OK;
+  if (x == nullptr || grad == nullptr || grad_x == nullptr) return B200A_EINVAL;
+  if (group_max != nullptr && top_db >= 0.f && scratch == nullptr) return B200A_EINVAL;
+  return amplitude_to_db_backward_impl(x, grad, g_stride, groups, group_elems, multiplier, amin, offset, top_db, group_max,
+                                       scratch, grad_x, static_cast<cudaStream_t>(stream));
+}
+
+int b200a_apply_fbank_backward(const float* grad, int64_t rows, int64_t n_filters, int64_t frames, int64_t stride_row,
+                               int64_t stride_filter, int64_t stride_frame, const float* fb, int64_t n_bins, float* grad_spec,
+                               b200a_stream stream) {
+  if (rows < 0 || n_filters < 1 || n_filters > 0x7fffffffLL || frames < 0 || n_bins < 1) return B200A_EINVAL;
+  if (stride_row < 0 || stride_filter < 0 || stride_frame < 0) return B200A_EINVAL;
+  if (rows == 0 || frames == 0) return B200A_OK;
+  if (grad == nullptr || fb == nullptr || grad_spec == nullptr) return B200A_EINVAL;
+  return apply_fbank_backward_impl(grad, rows, n_filters, frames, stride_row, stride_filter, stride_frame, fb, n_bins,
+                                   grad_spec, static_cast<cudaStream_t>(stream));
+}
+
+int b200a_ratio_backward(const float* pairs, const float* grad, int64_t rows, int64_t frames, int64_t stride_row,
+                         int64_t stride_frame, float* grad_pairs, b200a_stream stream) {
+  if (rows < 0 || frames < 0 || stride_row < 0 || stride_frame < 0) return B200A_EINVAL;
+  if (rows == 0 || frames == 0) return B200A_OK;
+  if (pairs == nullptr || grad == nullptr || grad_pairs == nullptr) return B200A_EINVAL;
+  return ratio_backward_impl(pairs, grad, rows, frames, stride_row, stride_frame, grad_pairs, static_cast<cudaStream_t>(stream));
+}
+
 int b200a_istft_run(const b200a_frontend_desc* desc, const void* workspace, const float* spec, int64_t rows,
                     int64_t frames, int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf,
                     float* out, int64_t out_row_stride, int64_t start, int64_t out_len, b200a_stream stream) {

@@ -144,6 +144,22 @@ int phase_vocoder_impl(const float* spec, int64_t s_row, int64_t s_bin, int64_t 
                        int64_t frames_in, double rate, const float* phase_advance, float* out, int64_t frames_out,
                        cudaStream_t stream);
 
+// feature_backward.cu: input gradients of MFCC / LFCC after the mel stage, AmplitudeToDB, MelScale, SpectralCentroid
+size_t mfcc_backward_scratch(int64_t rows, int64_t frames, int64_t rows_per_group);
+int mfcc_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t gs_row, int64_t gs_frame,
+                       int64_t gs_col, const float* feat, const float* mel, const float* group_max, int64_t rows,
+                       int64_t frames, int64_t rows_per_group, float top_db, void* scratch, float* grad_mel,
+                       cudaStream_t stream);
+size_t amplitude_to_db_backward_scratch(int64_t groups, int64_t group_elems);
+int amplitude_to_db_backward_impl(const float* x, const float* grad, int64_t g_stride, int64_t groups, int64_t group_elems,
+                                  float mult, float amin, float offset, float top_db, const float* group_max, void* scratch,
+                                  float* grad_x, cudaStream_t stream);
+int apply_fbank_backward_impl(const float* grad, int64_t rows, int64_t n_filters, int64_t frames, int64_t gs_row,
+                              int64_t gs_filter, int64_t gs_frame, const float* fb, int64_t n_bins, float* grad_spec,
+                              cudaStream_t stream);
+int ratio_backward_impl(const float* pairs, const float* grad, int64_t rows, int64_t frames, int64_t gs_row,
+                        int64_t gs_frame, float* grad_pairs, cudaStream_t stream);
+
 // resample.cu
 size_t resample_workspace_bytes_impl(int new_r, int taps);
 int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width, void* ws, size_t ws_bytes,
@@ -215,6 +231,13 @@ __device__ __forceinline__ int2 filter_range(const int2* bands, int n_mels, int 
     }
   }
   return hi > lo ? make_int2(lo, hi) : make_int2(0, 0);
+}
+
+// AmplitudeToDB's map (functional.py:385-386): mult * log10(max(x, amin)) - offset.  to_db_kernel and the adjoint's
+// recompute of it (feature_backward.cu) share this one expression, so the adjoint's ties with the forward's group maxima
+// are exact.
+__device__ __forceinline__ float db_value(float x, float mult, float amin, float offset) {
+  return mult * log10f(fmaxf(x, amin)) - offset;
 }
 
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {

@@ -32,7 +32,7 @@ to_db_kernel(const float* __restrict__ x, int64_t group_elems, float mult, float
   float* oi = out + g * group_elems;
   float local = -CUDART_INF_F;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < group_elems; i += (int64_t)gridDim.x * blockDim.x) {
-    const float v = mult * log10f(fmaxf(xi[i], amin)) - offset;
+    const float v = db_value(xi[i], mult, amin, offset);
     oi[i] = v;
     local = fmaxf(local, v);
   }

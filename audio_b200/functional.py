@@ -8,8 +8,11 @@ private helpers ``transforms`` imports (``_get_sinc_resample_kernel`` 1305-1402,
 ``_apply_sinc_resample_kernel`` 1405-1432).
 
 Differences, all explicit (never a silent fallback): CUDA float32 tensors only, forward only except the waveform
-gradient of ``spectrogram`` (and of the MelSpectrogram path) inside ``audio_b200.differentiable()`` and the spectrogram
-gradient of ``inverse_spectrogram`` inside ``audio_b200.differentiable(inverse=True)``.
+gradient of ``spectrogram`` (and of the MelSpectrogram path) inside ``audio_b200.differentiable()``, the spectrogram
+gradient of ``inverse_spectrogram`` inside ``audio_b200.differentiable(inverse=True)``, the waveform gradient of
+``resample`` / ``speed`` inside ``audio_b200.differentiable(resample=True)``, and the input gradients of
+``amplitude_to_DB``, ``spectral_centroid`` and the MFCC / LFCC / MelScale paths inside
+``audio_b200.differentiable(features=True)``.
 """
 from __future__ import annotations
 
@@ -27,7 +30,7 @@ from . import _lib, _ops
 from ._bookkeeping import resample_ratio
 from ._constants import create_dct, linear_fbanks, melscale_fbanks, sinc_resample_kernel
 from ._plans import (FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad,
-                     is_inverse_differentiable, new_group_max)
+                     is_feature_differentiable, is_inverse_differentiable, new_group_max)
 
 __all__ = [
     "spectrogram",
@@ -396,37 +399,75 @@ def amplitude_to_DB(
     x: Tensor, multiplier: float, amin: float, db_multiplier: float, top_db: Optional[float] = None
 ) -> Tensor:
     _require_cuda_f32(x, "x")
+    if _wants_grad(x, (), is_feature_differentiable, "x"):
+        return _AmplitudeToDBFunction.apply(x, float(multiplier), float(amin), float(multiplier) * float(db_multiplier),
+                                            top_db)
     _no_autograd(x)
-    xc = x.contiguous()
+    return _amplitude_to_db_run(x.contiguous(), multiplier, amin, float(multiplier) * float(db_multiplier), top_db)[0]
+
+
+def _amplitude_to_db_run(xc: Tensor, multiplier: float, amin: float, offset: float, top_db: Optional[float]):
+    """b200a_amplitude_to_db on the contiguous ``xc``: (output, group maxima or None, groups)."""
     out = torch.empty_like(xc)
     if xc.numel() == 0:
-        return out
+        return out, None, 0
     groups = _db_groups(xc.shape) if top_db is not None else 1
     dev = xc.device
     with torch.cuda.device(dev):
         scratch = torch.empty(groups, dtype=torch.float32, device=dev)
         rc = _lib.lib().b200a_amplitude_to_db(
-            xc.data_ptr(), groups, xc.numel() // groups, float(multiplier), float(amin),
-            float(multiplier) * float(db_multiplier), -1.0 if top_db is None else float(top_db),
-            scratch.data_ptr(), out.data_ptr(), _stream_ptr(dev),
+            xc.data_ptr(), groups, xc.numel() // groups, float(multiplier), float(amin), float(offset),
+            -1.0 if top_db is None else float(top_db), scratch.data_ptr(), out.data_ptr(), _stream_ptr(dev),
         )
     _lib.check(rc, "amplitude_to_db")
-    return out
+    return out, scratch if top_db is not None else None, groups
+
+
+class _AmplitudeToDBFunction(torch.autograd.Function):
+    """amplitude_to_DB with b200audio::amplitude_to_db_backward as its backward.  Saved: the input (save_for_backward,
+    so in-place edits of it are detected) and the forward's group maxima, against which the backward's recomputed dB
+    values tie exactly."""
+
+    @staticmethod
+    def forward(ctx, x, multiplier, amin, offset, top_db):
+        xc = x.contiguous()
+        out, gmax, groups = _amplitude_to_db_run(xc, multiplier, amin, offset, top_db)
+        ctx.save_for_backward(x)
+        ctx.xc = None if xc is x else xc
+        ctx.gmax, ctx.args = gmax, (groups, multiplier, amin, offset, -1.0 if top_db is None else float(top_db))
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        xc = x if ctx.xc is None else ctx.xc
+        if xc.numel() == 0:
+            return torch.zeros_like(xc), None, None, None, None
+        return _ops.amplitude_to_db_backward(g, xc, ctx.gmax, *ctx.args), None, None, None, None
 
 
 def _apply_fbank(specgram: Tensor, fb: Tensor) -> Tensor:
     """MelScale.forward on an existing spectrogram of logical shape (..., n_bins, T)."""
     _require_cuda_f32(specgram, "specgram")
     _require_cuda_f32(fb, "fb")
-    _no_autograd(specgram)
+    grad = _wants_grad(specgram, (("fb", fb),), is_feature_differentiable, "spectrogram")
+    if not grad:
+        _no_autograd(specgram)
     n_bins, frames = specgram.shape[-2], specgram.shape[-1]
     if fb.shape[0] != n_bins:
         raise RuntimeError(f"mat1 and mat2 shapes cannot be multiplied: n_bins={n_bins} vs fb {tuple(fb.shape)}")
     lead = specgram.shape[:-2]
     s3 = specgram.reshape((-1, n_bins, frames))
-    rows = s3.shape[0]
+    out = _MelScaleFunction.apply(s3, fb) if grad else _apply_fbank_run(s3, fb)
+    return out.reshape(lead + out.shape[-2:]).transpose(-1, -2)
+
+
+def _apply_fbank_run(s3: Tensor, fb: Tensor) -> Tensor:
+    """b200a_apply_fbank on the (rows, n_bins, T) spectrogram: the frame-major (rows, T, n_filters) product."""
+    rows, n_bins, frames = s3.shape
     fbc = fb.contiguous()
-    dev = specgram.device
+    dev = s3.device
     with torch.cuda.device(dev):
         out = torch.empty((rows, frames, fb.shape[1]), dtype=torch.float32, device=dev)
         rc = _lib.lib().b200a_apply_fbank(
@@ -434,7 +475,24 @@ def _apply_fbank(specgram: Tensor, fb: Tensor) -> Tensor:
             fbc.data_ptr(), fb.shape[1], out.data_ptr(), _stream_ptr(dev),
         )
     _lib.check(rc, "apply_fbank")
-    return out.reshape(lead + out.shape[-2:]).transpose(-1, -2)
+    return out
+
+
+class _MelScaleFunction(torch.autograd.Function):
+    """MelScale on its own with b200audio::apply_fbank_backward as its backward.  The map is linear in the spectrogram:
+    only the filterbank is saved (save_for_backward, so an in-place edit of it before backward is an error, as it is for
+    torch's matmul)."""
+
+    @staticmethod
+    def forward(ctx, s3, fb):
+        ctx.save_for_backward(fb)
+        return _apply_fbank_run(s3, fb)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (fb,) = ctx.saved_tensors
+        return _ops.apply_fbank_backward(g, fb.contiguous()).transpose(1, 2), None
 
 
 # ---- fused MelSpectrogram / MFCC (what the transforms call) -----------------------------------
@@ -453,6 +511,7 @@ def mfcc(
     top_db: Optional[float],
     log_mels: bool,
     process_group=None,
+    fb_name: str = "fb",
 ) -> Tensor:
     """MelSpectrogram -> dB/log -> DCT: fused front-end kernel + clamp/DCT kernel.
 
@@ -460,6 +519,9 @@ def mfcc(
     (reference functional.py:395-399): for a waveform of dim <= 2 ONE maximum is shared by the
     whole batch, for dim >= 3 each leading item has its own.  ``process_group`` (optional)
     extends the shared maximum across ranks with one all-reduce(MAX) of that scalar.
+
+    Inside ``audio_b200.differentiable(features=True)`` a waveform that requires grad gets its gradient
+    (``_MfccFunction``); ``fb_name`` names the filterbank buffer in the error for one that requires grad.
     """
     ws = plan.workspace(window, fb, dct_mat)
     rows = 1
@@ -470,9 +532,19 @@ def mfcc(
         rows_per_group = waveform.shape[-2] if waveform.dim() >= 2 else 1
         rows_per_group = max(int(rows_per_group), 1)
         groups = max((rows + rows_per_group - 1) // rows_per_group, 1)
-        gmax = new_group_max(groups, waveform.device)
     else:
-        rows_per_group, gmax = 1, None
+        rows_per_group, groups = 1, 0
+    _require_cuda_f32(waveform, "waveform")
+    if _wants_grad(waveform, (("window", window), (fb_name, fb), ("dct_mat", dct_mat)), is_feature_differentiable):
+        if process_group is not None:
+            raise RuntimeError(
+                "audio_b200: MFCC / LFCC gradients with a process_group are not implemented (the sharded backward would "
+                "need the routed top_db sums all-reduced and the group maximum located across ranks); set "
+                "process_group = None, or detach() the waveform"
+            )
+        out = plan.mfcc_grad(ws, waveform, groups, rows_per_group, top_db if clamp else None)
+        return _unpack(out, waveform)
+    gmax = new_group_max(groups, waveform.device) if clamp else None
     feat = plan.run(ws, _lib.STAGE_FEAT, waveform, gmax, rows_per_group)
     if clamp and waveform.dim() <= 2:
         gmax = _exchange_group_max(gmax, process_group)
@@ -575,10 +647,36 @@ def spectral_centroid(
     freqs = torch.linspace(0, sample_rate // 2, steps=1 + n_fft // 2, device=dev)
     fb = torch.stack([freqs, torch.ones_like(freqs)], dim=1).contiguous()
     ws = plan.workspace(window, fb, None)
-    pairs = plan.run(ws, _lib.STAGE_MEL, waveform)  # (rows, T, 2)
+    # with the feature switch on, the mel stage differentiates (_FrontendFunction) and so does the ratio
+    constants = (("window", window),)
+    grad = _wants_grad(waveform, constants, is_feature_differentiable)
+    pairs = plan.run(ws, _lib.STAGE_MEL, waveform, constants=constants if grad else None,
+                     switch=is_feature_differentiable)  # (rows, T, 2)
+    out = _RatioFunction.apply(pairs) if grad else _ratio_run(pairs)
+    return out.reshape(waveform.shape[:-1] + (out.shape[1],))
+
+
+def _ratio_run(pairs: Tensor) -> Tensor:
+    """b200a_ratio_f32 on the (rows, T, 2) pairs: (rows, T) ratios."""
     rows, frames, _ = pairs.shape
+    dev = pairs.device
     with torch.cuda.device(dev):
         out = torch.empty((rows, frames), dtype=torch.float32, device=dev)
         rc = _lib.lib().b200a_ratio_f32(pairs.data_ptr(), rows * frames, out.data_ptr(), _stream_ptr(dev))
     _lib.check(rc, "ratio_f32")
-    return out.reshape(waveform.shape[:-1] + (frames,))
+    return out
+
+
+class _RatioFunction(torch.autograd.Function):
+    """SpectralCentroid's N / D per frame with b200audio::ratio_backward as its backward; the pairs are saved."""
+
+    @staticmethod
+    def forward(ctx, pairs):
+        ctx.save_for_backward(pairs)
+        return _ratio_run(pairs)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (pairs,) = ctx.saved_tensors
+        return _ops.ratio_backward(g, pairs)

@@ -9,6 +9,11 @@ existing call sites keep working after ``import audio_b200.transforms as T``.
 ``forward`` launches hand-written sm_90a kernels through the C ABI; MelSpectrogram and MFCC
 do NOT chain their sub-modules' forwards (that would round-trip the (B, T, n_fft/2+1) power
 spectrum through HBM) -- they read the sub-modules' buffers and launch the fused kernel.
+
+Gradients are opt-in, per thread: Spectrogram and MelSpectrogram inside ``audio_b200.differentiable()``,
+InverseSpectrogram with ``inverse=True``, Resample / Speed / SpeedPerturbation with ``resample=True``, and MFCC,
+LFCC, AmplitudeToDB, MelScale and SpectralCentroid with ``features=True``.  GriffinLim, TimeStretch, PitchShift and
+the Kaldi features are forward-only.
 """
 from __future__ import annotations
 
@@ -407,7 +412,8 @@ class LFCC(torch.nn.Module):
         if self._plan is None or self._plan.desc.key() != plan.desc.key():
             self._plan = plan
         return F.mfcc(
-            self._plan, spec.window, self.filter_mat, self.dct_mat, waveform, db.top_db, self.log_lf, self.process_group
+            self._plan, spec.window, self.filter_mat, self.dct_mat, waveform, db.top_db, self.log_lf, self.process_group,
+            fb_name="filter_mat",
         )
 
 

@@ -191,6 +191,70 @@ int b200a_amplitude_to_db(const float* x, int64_t groups, int64_t group_elems, f
 
 int b200a_fill_f32(float* dst, int64_t n, float value, b200a_stream stream);
 
+/* ---- input gradients of the feature stages (MFCC / LFCC, AmplitudeToDB, MelScale, SpectralCentroid) -------------- */
+/*
+ * The top_db clamp c = max(d, thr), thr = group_max[g] - top_db (functional.py:399), differentiates as torch's maximum
+ * and amax do: an element keeps its gradient where d > thr and half of it where d == thr; the rest goes to thr, is
+ * summed over the group (R_g) and split evenly over the count_g elements equal to group_max[g]:
+ *   g_d[e] = g[e] ([d > thr] + 1/2 [d == thr]) + [d == group_max[g]] R_g / count_g.
+ * Deterministic: R_g is summed in a fixed order through `scratch` (per-tile partials, then one fixed-order reduction per
+ * group), never with float atomics, so reruns are bit-identical.  Without a clamp the call is one elementwise pass.
+ */
+/* Bytes of scratch b200a_mfcc_backward needs with a clamp (per-tile partials + one float per group); 0 for an invalid
+ * request. */
+size_t b200a_mfcc_backward_scratch_bytes(const b200a_frontend_desc* desc, int64_t rows, int64_t frames,
+                                         int64_t rows_per_group);
+/*
+ * Mel-stage gradient of b200a_mfcc_finish o (the dB / log map of B200A_STAGE_FEAT), with the forward's workspace:
+ *   g_d[r][t][m] = sum_j dct[m][j] g[r][t][j]                               (the DCT, _transforms.py:708)
+ *   log_mels:  grad_mel = g_d / (mel + 1e-6)
+ *   dB:        grad_mel = g_d' * db_multiplier / (ln10 mel) where mel >= db_amin, else 0 (clamp(min=amin) passes the
+ *              gradient at mel == amin);  g_d' = g_d through the top_db clamp above when group_max != NULL, top_db >= 0
+ *   grad      : [rows][T][n_mfcc] cepstral gradient at element strides (0 allowed: expanded gradients)
+ *   feat      : [rows][T][n_mels] the forward's B200A_STAGE_FEAT output (pre-clamp d): masks and ties read it
+ *   mel       : [rows][T][n_mels] b200a_frontend_run(B200A_STAGE_MEL) of the same waveform: the derivative reads it
+ *   group_max : the maxima the forward clamped with; rows_per_group as in b200a_frontend_run
+ *   scratch   : b200a_mfcc_backward_scratch_bytes(desc, rows, T, rows_per_group) bytes (clamp only, else may be NULL)
+ *   grad_mel  : [rows][T][n_mels], every element written; feed it to b200a_frontend_backward(B200A_STAGE_MEL)
+ * The DCT is staged in shared memory: B200A_EUNSUPPORTED when n_mels x n_mfcc needs more than ~200 KB.
+ */
+int b200a_mfcc_backward(const b200a_frontend_desc* desc, const void* workspace, const float* grad, int64_t g_stride_row,
+                        int64_t g_stride_frame, int64_t g_stride_col, const float* feat, const float* mel,
+                        const float* group_max, int64_t rows, int64_t frames, int64_t rows_per_group, float top_db,
+                        void* scratch, float* grad_mel, b200a_stream stream);
+/* Bytes of scratch b200a_amplitude_to_db_backward needs with a clamp; 0 for an invalid request. */
+size_t b200a_amplitude_to_db_backward_scratch_bytes(int64_t groups, int64_t group_elems);
+/*
+ * Gradient of b200a_amplitude_to_db: d = mult * log10(max(x, amin)) - offset is recomputed from x by the expression the
+ * forward uses, so ties with the forward's maxima are exact; then grad_x = g_d' * mult / (ln10 x) where x >= amin, else 0.
+ *   x         : the forward's input, `groups` contiguous chunks of `group_elems` floats
+ *   grad      : grad[e * g_stride], g_stride 1 (contiguous) or 0 (expanded scalar)
+ *   group_max : the forward's `scratch` ([groups] maxima) when it clamped (top_db >= 0), else NULL
+ *   scratch   : b200a_amplitude_to_db_backward_scratch_bytes(groups, group_elems) bytes (clamp only)
+ *   grad_x    : groups * group_elems floats, every element written
+ */
+int b200a_amplitude_to_db_backward(const float* x, const float* grad, int64_t g_stride, int64_t groups, int64_t group_elems,
+                                   float multiplier, float amin, float offset, float top_db, const float* group_max,
+                                   void* scratch, float* grad_x, b200a_stream stream);
+/*
+ * Spectrogram gradient of b200a_apply_fbank (the transpose of MelScale.forward):
+ *   grad_spec[r][t][k] = sum_m fb[k][m] grad[r][m][t]
+ *   grad      : logical [rows][n_filters][T] at element strides (0 allowed)
+ *   fb        : [n_bins][n_filters], row-major
+ *   grad_spec : FRAME-MAJOR [rows][T][n_bins], every element written.  No atomics; rows <= 65535.
+ */
+int b200a_apply_fbank_backward(const float* grad, int64_t rows, int64_t n_filters, int64_t frames, int64_t stride_row,
+                               int64_t stride_filter, int64_t stride_frame, const float* fb, int64_t n_bins, float* grad_spec,
+                               b200a_stream stream);
+/*
+ * Gradient of b200a_ratio_f32 for SpectralCentroid: y = N / D per frame gives
+ *   grad_pairs[r][t] = (g / D, -g N / D^2),  (N, D) = pairs[r][t],  g = grad[r * stride_row + t * stride_frame]
+ * which b200a_frontend_backward(B200A_STAGE_MEL) with the [f | 1] filterbank takes back to the waveform.
+ *   pairs, grad_pairs : [rows][T][2]
+ */
+int b200a_ratio_backward(const float* pairs, const float* grad, int64_t rows, int64_t frames, int64_t stride_row,
+                         int64_t stride_frame, float* grad_pairs, b200a_stream stream);
+
 /*
  * out[i] = pairs[i][0] / pairs[i][1].  Last step of F.spectral_centroid (functional.py:1257-1299): the
  * fused front end is run with the two-column "filterbank" [bin frequency | 1] on the magnitude

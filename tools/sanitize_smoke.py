@@ -37,6 +37,14 @@ with audio_b200.differentiable(inverse=True):  # spectrogram gradients: fused (2
     for n_fft, pad in ((256, 0), (1024, 5), (400, 3), (2048, 0)):
         spec = T.Spectrogram(n_fft=n_fft, hop_length=n_fft // 4, power=None).cuda()(x).requires_grad_()
         T.InverseSpectrogram(n_fft=n_fft, hop_length=n_fft // 4, pad=pad).cuda()(spec, 11000).sum().backward()
+with audio_b200.differentiable(features=True):  # feature gradients: MFCC clamp + ties, log path, LFCC, the stand-alones
+    for mod, xin in ((T.MFCC(16000, n_mfcc=13, melkwargs=dict(n_fft=512, hop_length=160, n_mels=40)), x),
+                     (T.MFCC(16000, n_mfcc=20, log_mels=True), x.reshape(1, 3, -1)),
+                     (T.LFCC(16000, n_lfcc=13, speckwargs=dict(n_fft=400)), x),
+                     (T.SpectralCentroid(16000, n_fft=512), x)):
+        mod.cuda()(xin.clone().requires_grad_()).sum().backward()
+    spec = T.Spectrogram(n_fft=400).cuda()(x).requires_grad_()
+    T.AmplitudeToDB(top_db=0.0)(T.MelScale(40, 16000, n_stft=201).cuda()(spec)).sum().backward()
 T.MFCC(16000, n_mfcc=13, melkwargs=dict(n_fft=512, hop_length=160, n_mels=40)).cuda()(x)
 T.MFCC(16000, n_mfcc=40, melkwargs=dict(n_fft=1024, hop_length=256, n_mels=80)).cuda()(x.reshape(1, 3, -1))
 for kw in (dict(num_mel_bins=40, snip_edges=False, use_energy=True), dict(num_mel_bins=23), dict(frame_length=20.0, round_to_power_of_two=False)):
