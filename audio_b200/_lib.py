@@ -142,6 +142,13 @@ _SIGNATURES = {
         ctypes.c_int,
         [POINTER(KaldiDesc), POINTER(FrontendDesc), c_void_p, c_int32, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p],
     ),
+    "b200a_kaldi_backward": (
+        ctypes.c_int,
+        [POINTER(KaldiDesc), POINTER(FrontendDesc), c_void_p, c_int32, c_void_p, c_int64, c_int64, c_int64, c_void_p,
+         c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int64, c_void_p],
+    ),
+    "b200a_kaldi_backward_scratch_bytes": (
+        c_size_t, [POINTER(KaldiDesc), POINTER(FrontendDesc), c_int32, c_int64, c_int64]),
     "b200a_subtract_column_mean": (ctypes.c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p]),
     "b200a_fill_f32": (ctypes.c_int, [c_void_p, c_int64, c_float, c_void_p]),
     "b200a_ratio_f32": (ctypes.c_int, [c_void_p, c_int64, c_void_p, c_void_p]),

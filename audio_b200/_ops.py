@@ -1,7 +1,7 @@
 """``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
-``resample_backward``.
+``resample_backward`` / ``kaldi_run`` / ``kaldi_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -56,6 +56,18 @@ _LIB.define(
     "int out_len, int pitch) -> Tensor"
 )
 _LIB.define("resample_backward(Tensor grad, Tensor workspace, int orig_r, int new_r, int width, int length) -> Tensor")
+_LIB.define(
+    "kaldi_run(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int[] kaldi_i, float[] kaldi_f, int stage, "
+    "int frames, int width, int row_stride) -> Tensor"
+)
+_LIB.define(
+    "kaldi_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int[] kaldi_i, float[] kaldi_f, "
+    "int stage, int row_stride, Tensor grad_out) -> Tensor"
+)
+
+_KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
+               "out_width", "out_col0", "use_log")
+_KALDI_FLOATS = ("preemphasis", "energy_floor")
 
 
 def pack_desc(d: "_lib.FrontendDesc"):
@@ -69,6 +81,19 @@ def _unpack_desc(desc_i: List[int], desc_f: List[float]) -> "_lib.FrontendDesc":
     for k, v in zip(_DESC_FLOATS, desc_f):
         setattr(d, k, float(v))
     return d
+
+
+def pack_kaldi_desc(k: "_lib.KaldiDesc"):
+    return [int(getattr(k, f)) for f in _KALDI_INTS], [float(getattr(k, f)) for f in _KALDI_FLOATS]
+
+
+def _unpack_kaldi_desc(kaldi_i: List[int], kaldi_f: List[float]) -> "_lib.KaldiDesc":
+    k = _lib.KaldiDesc()
+    for f, v in zip(_KALDI_INTS, kaldi_i):
+        setattr(k, f, int(v))
+    for f, v in zip(_KALDI_FLOATS, kaldi_f):
+        setattr(k, f, float(v))
+    return k
 
 
 def _stream(dev: torch.device) -> int:
@@ -303,6 +328,46 @@ def _resample_backward_meta(grad, workspace, orig_r, new_r, width, length):
     return grad.new_empty((grad.shape[0], length))
 
 
+# ---- kaldi_run / kaldi_backward ---------------------------------------------------------------------------------
+def _kaldi_run_cuda(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, frames, width, row_stride):
+    """(rows, L) waveform -> (rows, frames, width) Kaldi feature rows (b200a_kaldi_run)."""
+    d, k = _unpack_desc(desc_i, desc_f), _unpack_kaldi_desc(kaldi_i, kaldi_f)
+    rows, length = wave.shape
+    dev = wave.device
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, width), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_kaldi_run(k, d, workspace.data_ptr(), stage, wave.data_ptr(), rows, length, row_stride,
+                                        out.data_ptr(), _stream(dev))
+    _lib.check(rc, "kaldi_run")
+    return out
+
+
+def _kaldi_run_meta(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, frames, width, row_stride):
+    return wave.new_empty((wave.shape[0], frames, width), dtype=torch.float32)
+
+
+def _kaldi_backward_cuda(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, row_stride, grad_out):
+    """(rows, frames, width) feature-row gradient at any element strides -> (rows, L) waveform gradient."""
+    d, k = _unpack_desc(desc_i, desc_f), _unpack_kaldi_desc(kaldi_i, kaldi_f)
+    rows, length = wave.shape
+    dev = wave.device
+    gs = grad_out.stride()
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        grad = torch.empty((rows, length), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_kaldi_backward_scratch_bytes(k, d, stage, rows, length)
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        rc = lib.b200a_kaldi_backward(k, d, workspace.data_ptr(), stage, wave.data_ptr(), rows, length, row_stride,
+                                      grad_out.data_ptr(), gs[0], gs[1], gs[2], scratch.data_ptr(), grad.data_ptr(), length,
+                                      _stream(dev))
+    _lib.check(rc, "kaldi_backward")
+    return grad
+
+
+def _kaldi_backward_meta(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, row_stride, grad_out):
+    return wave.new_empty(wave.shape, dtype=torch.float32)
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
@@ -312,7 +377,9 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("apply_fbank_backward", _apply_fbank_backward_cuda, _apply_fbank_backward_meta),
                             ("ratio_backward", _ratio_backward_cuda, _ratio_backward_meta),
                             ("resample_run", _resample_run_cuda, _resample_run_meta),
-                            ("resample_backward", _resample_backward_cuda, _resample_backward_meta)):
+                            ("resample_backward", _resample_backward_cuda, _resample_backward_meta),
+                            ("kaldi_run", _kaldi_run_cuda, _kaldi_run_meta),
+                            ("kaldi_backward", _kaldi_backward_cuda, _kaldi_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -326,3 +393,5 @@ apply_fbank_backward = torch.ops.b200audio.apply_fbank_backward
 ratio_backward = torch.ops.b200audio.ratio_backward
 resample_run = torch.ops.b200audio.resample_run
 resample_backward = torch.ops.b200audio.resample_backward
+kaldi_run = torch.ops.b200audio.kaldi_run
+kaldi_backward = torch.ops.b200audio.kaldi_backward

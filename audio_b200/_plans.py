@@ -53,28 +53,40 @@ def is_feature_differentiable() -> bool:
     return getattr(_GRAD_STATE, "features", False)
 
 
-def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = False, features: bool = False) -> None:
+def is_kaldi_differentiable() -> bool:
+    """Whether compliance.kaldi spectrogram, fbank and mfcc (and their ``_batch`` forms) accept waveforms that require
+    grad (in this thread)."""
+    return getattr(_GRAD_STATE, "kaldi", False)
+
+
+def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = False, features: bool = False,
+                       kaldi: bool = False) -> None:
     """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
     ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT, ``resample=True``
     (with ``mode``) the waveform gradients of the resampler, ``features=True`` (with ``mode``) the input gradients of
-    MFCC, LFCC, AmplitudeToDB, MelScale and SpectralCentroid.  They are separate switches so that vocoder inference and
-    augmentation code (Speed, SpeedPerturbation) does not build graphs when loss gradients are on, and so that the
-    top_db clamp's gradient -- every clamped element's share goes to the group maximum -- is opted into knowingly."""
+    MFCC, LFCC, AmplitudeToDB, MelScale and SpectralCentroid, ``kaldi=True`` (with ``mode``) the waveform gradients of
+    the Kaldi spectrogram, fbank and mfcc.  They are separate switches so that vocoder inference, augmentation code
+    (Speed, SpeedPerturbation) and Kaldi feature preprocessing in data pipelines do not build graphs when loss
+    gradients are on, and so that the top_db clamp's gradient -- every clamped element's share goes to the group
+    maximum -- is opted into knowingly."""
     _GRAD_STATE.on = bool(mode)
     _GRAD_STATE.inverse = bool(mode) and bool(inverse)
     _GRAD_STATE.resample = bool(mode) and bool(resample)
     _GRAD_STATE.features = bool(mode) and bool(features)
+    _GRAD_STATE.kaldi = bool(mode) and bool(kaldi)
 
 
 @contextlib.contextmanager
-def differentiable(mode: bool = True, *, inverse: bool = False, resample: bool = False, features: bool = False):
+def differentiable(mode: bool = True, *, inverse: bool = False, resample: bool = False, features: bool = False,
+                   kaldi: bool = False):
     """Context manager form of :func:`set_differentiable`; restores the previous settings on exit."""
-    prev = is_differentiable(), is_inverse_differentiable(), is_resample_differentiable(), is_feature_differentiable()
-    set_differentiable(mode, inverse=inverse, resample=resample, features=features)
+    prev = (is_differentiable(), is_inverse_differentiable(), is_resample_differentiable(), is_feature_differentiable(),
+            is_kaldi_differentiable())
+    set_differentiable(mode, inverse=inverse, resample=resample, features=features, kaldi=kaldi)
     try:
         yield
     finally:
-        set_differentiable(prev[0], inverse=prev[1], resample=prev[2], features=prev[3])
+        set_differentiable(prev[0], inverse=prev[1], resample=prev[2], features=prev[3], kaldi=prev[4])
 
 
 def _no_autograd(t: torch.Tensor) -> None:
@@ -86,7 +98,8 @@ def _no_autograd(t: torch.Tensor) -> None:
             "compute spectrogram gradients inside audio_b200.differentiable(inverse=True); Resample, F.resample, Speed "
             "and SpeedPerturbation compute waveform gradients inside audio_b200.differentiable(resample=True); MFCC, LFCC, "
             "AmplitudeToDB, MelScale and SpectralCentroid compute input gradients inside "
-            "audio_b200.differentiable(features=True).)"
+            "audio_b200.differentiable(features=True); compliance.kaldi spectrogram, fbank and mfcc compute waveform "
+            "gradients inside audio_b200.differentiable(kaldi=True).)"
         )
 
 

@@ -8,8 +8,15 @@ per-frame work -- framing (snip_edges or mirrored edges), DC removal, log energy
 FFT, power, mel projection, log -- is ONE fused kernel launch (``b200a_kaldi_run``), followed where asked for by the
 DCT (``b200a_mfcc_finish``) and the column-mean subtraction (``b200a_subtract_column_mean``).
 
-Differences, all explicit: CUDA float32 waveforms only, forward only, and ``dither`` must be 0 (the reference draws it
-with ``torch.randn`` per frame element, which no other generator reproduces).  ``fbank_batch`` / ``mfcc_batch`` /
+Waveform gradients are opt-in: inside ``audio_b200.differentiable(kaldi=True)`` a waveform that requires grad gets
+torch's autograd of the reference op sequence, ties of the log floor and the energy floor included, from
+``b200a_kaldi_backward`` (the same launches run forward, so the features are bit-identical to the no-grad call).
+Outside it, or with only the other switches on, a waveform that requires grad raises "forward-only": Kaldi features
+are usually data-pipeline preprocessing.  Gradients with respect to the window, mel banks, DCT or lifter, and
+second-order gradients, are not offered.
+
+Differences, all explicit: CUDA float32 waveforms only, and ``dither`` must be 0 (the reference draws it with
+``torch.randn`` per frame element, which no other generator reproduces).  ``fbank_batch`` / ``mfcc_batch`` /
 ``spectrogram_batch`` are extensions that take ``(batch, time)`` and return ``(batch, frames, features)``.
 """
 from __future__ import annotations
@@ -20,9 +27,12 @@ from typing import Dict, Tuple
 import torch
 from torch import Tensor
 
-from .. import _lib
+from torch.autograd.function import once_differentiable
+
+from .. import _lib, _ops
 from .._constants import create_dct
-from .._plans import FrontendPlan, _no_autograd, _require_cuda_f32, _stream_ptr, pack_rows
+from .._plans import (FrontendPlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad, is_kaldi_differentiable,
+                      pack_rows)
 
 __all__ = [
     "get_mel_banks",
@@ -243,6 +253,57 @@ class _KaldiPlan:
 _PLANS: Dict[tuple, _KaldiPlan] = {}
 
 
+def _launch(flat: Tensor, plan: _KaldiPlan, kd_lists, stage: int, frames: int, width: int, stride: int,
+            subtract_mean: bool) -> Tensor:
+    """The forward launches: b200a_kaldi_run [+ b200a_mfcc_finish] [+ b200a_subtract_column_mean]."""
+    out = _ops.kaldi_run(flat, plan.ws, *plan.front._packed_desc(), *kd_lists, stage, frames, width, stride)
+    if plan.finish is not None:
+        out = plan.finish.mfcc_finish(plan.finish_ws, out, None, 1, None)
+    if subtract_mean:
+        dev = out.device
+        with torch.cuda.device(dev):
+            rc = _lib.lib().b200a_subtract_column_mean(out.data_ptr(), out.shape[0], out.shape[1], out.shape[2],
+                                                       _stream_ptr(dev))
+        _lib.check(rc, "subtract_column_mean")
+    return out
+
+
+class _KaldiFunction(torch.autograd.Function):
+    """The Kaldi features of the packed (rows, L) waveform with exactly the no-grad launches (so the output is
+    bit-identical to the no-grad call), and their waveform gradient: the column-mean subtraction (symmetric, its own
+    adjoint), the MFCC finishing matrix transposed (b200audio::apply_fbank_backward), then b200audio::kaldi_backward.
+    The waveform goes through save_for_backward, so in-place edits of it are detected; the plan (workspace, finishing
+    matrix) is held, so its eviction from the cache cannot free what backward reads."""
+
+    @staticmethod
+    def forward(ctx, flat, plan, kd_lists, stage, frames, width, stride, subtract_mean):
+        out = _launch(flat, plan, kd_lists, stage, frames, width, stride, subtract_mean)
+        ctx.save_for_backward(flat)
+        ctx.plan, ctx.args = plan, (kd_lists, stage, frames, width, stride, subtract_mean)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        (flat,) = ctx.saved_tensors
+        plan = ctx.plan
+        kd_lists, stage, frames, width, stride, subtract_mean = ctx.args
+        g = grad_out
+        if subtract_mean:
+            g = g.contiguous().clone()
+            dev = g.device
+            with torch.cuda.device(dev):
+                rc = _lib.lib().b200a_subtract_column_mean(g.data_ptr(), g.shape[0], g.shape[1], g.shape[2],
+                                                           _stream_ptr(dev))
+            _lib.check(rc, "subtract_column_mean")
+        if plan.finish is not None:  # one row of rows * T frames: the op's row limit never applies
+            rows = g.shape[0]
+            g = _ops.apply_fbank_backward(g.contiguous().reshape(1, rows * frames, g.shape[2]), plan.matrix)
+            g = g.reshape(rows, frames, width)
+        grad = _ops.kaldi_backward(flat, plan.ws, *plan.front._packed_desc(), *kd_lists, stage, stride, g)
+        return grad, None, None, None, None, None, None, None
+
+
 def _select_channel(waveform: Tensor, channel: int) -> Tensor:
     channel = max(channel, 0)
     assert channel < waveform.size(0), "Invalid channel {} for size {}".format(channel, waveform.size(0))
@@ -252,7 +313,9 @@ def _select_channel(waveform: Tensor, channel: int) -> Tensor:
 def _features(kind: str, rows: Tensor, o: dict) -> Tensor:
     """rows (B, n) -> (B, m, width) Kaldi features of `kind` for the option dict `o` (all keys of the public API)."""
     _require_cuda_f32(rows, "waveform")
-    _no_autograd(rows)
+    grad = _wants_grad(rows, (), is_kaldi_differentiable)
+    if not grad:
+        _no_autograd(rows)
     if o["dither"] != 0.0:
         raise RuntimeError(
             "audio_b200.compliance.kaldi: dither != 0 is not implemented (the reference draws the noise with "
@@ -333,18 +396,14 @@ def _features(kind: str, rows: Tensor, o: dict) -> Tensor:
 
     flat, stride = pack_rows(rows)
     batch = flat.shape[0]
+    stage = _lib.STAGE_MEL if mel else _lib.STAGE_POWER
+    if frames > 0 and batch > 0:
+        args = (flat, plan, _ops.pack_kaldi_desc(kd), stage, frames, width, stride, bool(o["subtract_mean"]))
+        return _KaldiFunction.apply(*args) if grad else _launch(*args)
     with torch.cuda.device(dev):
         out = torch.empty((batch, frames, width), dtype=torch.float32, device=dev)
-        if frames > 0 and batch > 0:
-            rc = lib.b200a_kaldi_run(kd, plan.front.desc, plan.ws.data_ptr(), _lib.STAGE_MEL if mel else _lib.STAGE_POWER,
-                                     flat.data_ptr(), batch, num_samples, stride, out.data_ptr(), _stream_ptr(dev))
-            _lib.check(rc, "kaldi_run")
     if kind == "mfcc" and frames > 0:
         out = plan.finish.mfcc_finish(plan.finish_ws, out, None, 1, None)
-    if o["subtract_mean"] and frames > 0 and batch > 0:
-        with torch.cuda.device(dev):
-            rc = lib.b200a_subtract_column_mean(out.data_ptr(), batch, frames, out.shape[-1], _stream_ptr(dev))
-        _lib.check(rc, "subtract_column_mean")
     return out
 
 

@@ -294,9 +294,8 @@ int64_t b200a_kaldi_num_frames(int64_t length, int32_t window_size, int32_t wind
   return (length + window_shift / 2) / window_shift;
 }
 
-int b200a_kaldi_run(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* desc, const void* workspace,
-                    int32_t stage, const float* wave, int64_t rows, int64_t length, int64_t row_stride,
-                    float* out, b200a_stream stream) {
+// The descriptor checks b200a_kaldi_run and b200a_kaldi_backward share.
+static int validate_kaldi(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* desc, int32_t stage) {
   if (kaldi == nullptr) return B200A_EINVAL;
   int rc = validate_desc(desc);
   if (rc != B200A_OK) return rc;
@@ -314,6 +313,14 @@ int b200a_kaldi_run(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* de
   if (kaldi->out_col0 < 0 || kaldi->out_col0 + values > kaldi->out_width ||
       kaldi->energy_col >= kaldi->out_width)
     return B200A_EINVAL;
+  return B200A_OK;
+}
+
+int b200a_kaldi_run(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* desc, const void* workspace,
+                    int32_t stage, const float* wave, int64_t rows, int64_t length, int64_t row_stride,
+                    float* out, b200a_stream stream) {
+  const int rc = validate_kaldi(kaldi, desc, stage);
+  if (rc != B200A_OK) return rc;
   if (rows == 0) return B200A_OK;
   if (workspace == nullptr || wave == nullptr || out == nullptr) return B200A_EINVAL;
   if (rows < 0 || length < 0 || row_stride < length) return B200A_EINVAL;
@@ -322,6 +329,33 @@ int b200a_kaldi_run(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* de
   if (frames < 1) return B200A_ESHORT;
   return frontend_run_impl(desc, workspace, stage, wave, rows, length, row_stride, frames, out, nullptr, 1,
                            static_cast<cudaStream_t>(stream), kaldi);
+}
+
+size_t b200a_kaldi_backward_scratch_bytes(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* desc, int32_t stage,
+                                          int64_t rows, int64_t length) {
+  if (validate_kaldi(kaldi, desc, stage) != B200A_OK || rows < 0 || length < kaldi->window_size) return 0;
+  const int64_t frames = b200a_kaldi_num_frames(length, kaldi->window_size, kaldi->window_shift, kaldi->snip_edges);
+  if (frames < 1) return 0;
+  return kaldi_backward_scratch(kaldi, desc, stage, rows, length, frames);
+}
+
+int b200a_kaldi_backward(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* desc, const void* workspace,
+                         int32_t stage, const float* wave, int64_t rows, int64_t length, int64_t row_stride,
+                         const float* grad_out, int64_t g_stride_row, int64_t g_stride_frame, int64_t g_stride_col,
+                         void* scratch, float* grad_wave, int64_t grad_row_stride, b200a_stream stream) {
+  const int rc = validate_kaldi(kaldi, desc, stage);
+  if (rc != B200A_OK) return rc;
+  if (g_stride_row < 0 || g_stride_frame < 0 || g_stride_col < 0) return B200A_EINVAL;
+  if (rows == 0) return B200A_OK;
+  if (workspace == nullptr || wave == nullptr || grad_out == nullptr || scratch == nullptr || grad_wave == nullptr)
+    return B200A_EINVAL;
+  if (rows < 0 || length < 0 || row_stride < length || grad_row_stride < length) return B200A_EINVAL;
+  if (length < kaldi->window_size) return B200A_ESHORT;
+  const int64_t frames = b200a_kaldi_num_frames(length, kaldi->window_size, kaldi->window_shift, kaldi->snip_edges);
+  if (frames < 1) return B200A_ESHORT;
+  return kaldi_backward_impl(kaldi, desc, workspace, stage, wave, rows, length, row_stride, frames, grad_out, g_stride_row,
+                             g_stride_frame, g_stride_col, scratch, grad_wave, grad_row_stride,
+                             static_cast<cudaStream_t>(stream));
 }
 
 int b200a_subtract_column_mean(float* x, int64_t rows, int64_t frames, int64_t width, b200a_stream stream) {

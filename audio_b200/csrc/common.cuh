@@ -12,6 +12,7 @@ constexpr uint32_t kWsMagic = 0xB200A0D1u;
 constexpr int kMaxStages = 16;
 constexpr int kMaxFft = 8192;
 constexpr float kKaldiEps = 1.1920928955078125e-07f;  // numeric_limits<float>::epsilon(), kaldi.py:21-22
+constexpr int kPadSymmetric = 4;  // internal pad mode: x[-1-j] = x[j], x[L+j] = x[L-1-j] (Kaldi snip_edges = false)
 
 // Device-side header at the start of a front-end workspace.
 struct WsHeader {
@@ -93,10 +94,12 @@ int validate_desc(const b200a_frontend_desc* d);
 int frontend_prepare_impl(const b200a_frontend_desc* d, const float* window, const float* fb, const float* dct, void* ws,
                           size_t ws_bytes, cudaStream_t stream);
 // The forward front end: the register-FFT kernels when they take the call, the Stockham kernel otherwise.  kd: Kaldi
-// framing and conditioning, or null.
+// framing and conditioning, or null.  kaldi_prelog: the Kaldi gradient's recompute -- the values before the log and
+// the frame energy E in place of its floored log, from the same kernel (so bit-identical to what the forward logged).
+// The COMPLEX stage with kd writes the conditioned spectrum only (no energy column).
 int frontend_run_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                       int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
-                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd);
+                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd, bool kaldi_prelog = false);
 int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
                    int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, float* out,
                    int64_t out_row_stride, int64_t start, int64_t out_len, cudaStream_t stream);
@@ -110,6 +113,12 @@ int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const floa
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);
 int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* feat, int64_t rows, int64_t frames,
                      const float* group_max, int64_t rows_per_group, float top_db, float* out, cudaStream_t stream);
+size_t kaldi_backward_scratch(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d, int stage, int64_t rows,
+                              int64_t length, int64_t frames);
+int kaldi_backward_impl(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d, const void* ws, int stage,
+                        const float* wave, int64_t rows, int64_t length, int64_t row_stride, int64_t frames,
+                        const float* grad, int64_t gs_row, int64_t gs_frame, int64_t gs_col, void* scratch,
+                        float* grad_wave, int64_t grad_row_stride, cudaStream_t stream);
 
 // frontend_pow2.cu: the register-FFT path.  frontend_run_pow2, istft_frames_pow2 and istft_backward_pow2 return
 // kPathDeclined when it does not take the call.
@@ -117,13 +126,18 @@ size_t pow2_workspace_extra(const b200a_frontend_desc* d);
 int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaStream_t stream);
 int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                       int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
-                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd);
+                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd, bool kaldi_prelog);
 int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
                       int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, cudaStream_t stream);
 bool backward_fused_applicable(const b200a_frontend_desc* d, int stage);
 int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                            int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
                            int64_t gs_frame, int64_t gs_col, float* frame_buf, cudaStream_t stream);
+bool kaldi_backward_fused_applicable(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, int stage, int64_t length);
+int kaldi_backward_pow2(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, const void* ws, int stage,
+                        const float* wave, int64_t rows, int64_t length, int64_t row_stride, int64_t frames,
+                        const float* grad, int64_t gs_row, int64_t gs_frame, int64_t gs_col, float* frame_buf,
+                        cudaStream_t stream);
 bool istft_backward_fused_applicable(const b200a_frontend_desc* d, int64_t frames);
 int istft_backward_pow2(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, float* grad_spec, cudaStream_t stream);

@@ -110,6 +110,7 @@ struct GenericParams {
   int out_width, out_col0;
   // Kaldi framing and per-frame conditioning (compliance/kaldi.py:44-83, :153-226); kaldi == 0: torch.stft framing
   int kaldi, k_win, k_snip, k_dc, k_energy_mode, k_energy_col, k_log;
+  int k_prelog;  // the gradient's recompute: the energy column receives E itself, not its floored log
   float k_preemph, k_energy_floor;
 };
 
@@ -300,8 +301,11 @@ __global__ void __launch_bounds__(256) stft_generic_kernel(const GenericParams p
       const int64_t t = t0 + f;
       if (p.k_energy_mode != 0 && p.k_energy_col >= 0 && t < p.frames) {
         for (int o = 16; o > 0; o >>= 1) energy += __shfl_xor_sync(0xffffffffu, energy, o);
-        float le = logf(fmaxf(energy, kKaldiEps));
-        if (p.k_energy_floor > 0.f) le = fmaxf(le, logf(p.k_energy_floor));
+        float le = energy;
+        if (!p.k_prelog) {
+          le = logf(fmaxf(energy, kKaldiEps));
+          if (p.k_energy_floor > 0.f) le = fmaxf(le, logf(p.k_energy_floor));
+        }
         if (lane == 0) p.out[(row * p.frames + t) * p.out_width + p.k_energy_col] = le;
       }
     }
@@ -689,7 +693,8 @@ static int launch_stockham(void (*kern)(Params), Params p, int64_t rows, int64_t
 
 static int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                                 int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
-                                int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd) {
+                                int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd,
+                                bool kaldi_prelog) {
   const WsLayout l = ws_layout(*d);
   const unsigned char* base = static_cast<const unsigned char*>(ws);
   GenericParams p{};
@@ -729,10 +734,12 @@ static int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, in
     p.k_snip = kd->snip_edges;
     p.k_dc = kd->remove_dc_offset;
     p.k_preemph = kd->preemphasis;
-    p.k_energy_mode = kd->energy_col >= 0 ? kd->energy_mode : 0;
+    // the COMPLEX stage's output is the spectrum alone: no energy column to write into
+    p.k_energy_mode = kd->energy_col >= 0 && stage != B200A_STAGE_COMPLEX ? kd->energy_mode : 0;
     p.k_energy_floor = kd->energy_floor;
     p.k_energy_col = kd->energy_col;
-    p.k_log = kd->use_log;
+    p.k_log = kaldi_prelog ? 0 : kd->use_log;
+    p.k_prelog = kaldi_prelog;
     p.out_width = kd->out_width;
     p.out_col0 = kd->out_col0;
   }
@@ -741,13 +748,13 @@ static int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, in
 
 int frontend_run_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                       int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
-                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd) {
+                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd, bool kaldi_prelog) {
   if (rows_per_group < 1) rows_per_group = 1;
   const int rc = frontend_run_pow2(d, ws, stage, wave, rows, length, row_stride, frames, out, group_max, rows_per_group,
-                                   stream, kd);
+                                   stream, kd, kaldi_prelog);
   if (rc != kPathDeclined) return rc;
   return frontend_run_generic(d, ws, stage, wave, rows, length, row_stride, frames, out, group_max, rows_per_group, stream,
-                              kd);
+                              kd, kaldi_prelog);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -955,9 +962,12 @@ __global__ void __launch_bounds__(256) spec_vjp_kernel(const SpecVjpParams p) {
 // sample was copied to (itself, its reflect / circular images, or the replicated edge runs) receives sum_t dframe[t][i -
 // t hop]; positions in ascending order, frames in ascending t, no atomics, so the result is reproducible bit for bit
 // and independent of the other rows.  Samples no frame covers get 0.  bad (may be null): frames whose gradient is NaN.
+// Frame t holds flen samples at a pitch of n_fft floats and starts at position t hop of the padded signal, which begins
+// `half` samples before sample 0.  kPadSymmetric (Kaldi's mirrored edges, frontend_generic.cu:kaldi_sample): half is
+// win/2 - shift/2, negative when shift > win, and sample s is read at positions -1 - s, s and 2 length - 1 - s.
 __global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict__ frame_buf, const int* __restrict__ bad,
-                                                         int n_fft, int hop, int64_t frames, int64_t length, int pad,
-                                                         int half, int pad_mode, int64_t blocks_per_row,
+                                                         int n_fft, int flen, int hop, int64_t frames, int64_t length,
+                                                         int pad, int half, int pad_mode, int64_t blocks_per_row,
                                                          float* __restrict__ grad, int64_t grad_row_stride) {
   const int64_t row = blockIdx.x / blocks_per_row;
   const int64_t s = (blockIdx.x - row * blocks_per_row) * (int64_t)blockDim.x + threadIdx.x;
@@ -965,8 +975,9 @@ __global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict
   const float* fb = frame_buf + row * frames * n_fft;
   const int* fl = bad == nullptr ? nullptr : bad + row * frames;
   auto at = [&](int64_t i, float acc) {
-    const int64_t t_lo = i - n_fft + 1 <= 0 ? 0 : (i - n_fft + hop) / hop;  // ceil((i - n_fft + 1) / hop)
-    int64_t t_hi = i / hop;
+    // i < 0: before the first frame (a negative Kaldi lead)
+    const int64_t t_lo = i - flen + 1 <= 0 ? 0 : (i - flen + hop) / hop;  // ceil((i - flen + 1) / hop)
+    int64_t t_hi = i < 0 ? -1 : i / hop;
     if (t_hi > frames - 1) t_hi = frames - 1;
     for (int64_t t = t_lo; t <= t_hi; ++t) {
       const float v = fb[t * n_fft + (i - t * hop)];
@@ -976,7 +987,11 @@ __global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict
   };
   const int64_t ext = length + 2 * (int64_t)pad, j = s + pad;  // j: index in the constant pre-padded signal
   float acc = 0.f;
-  if (half == 0 || pad_mode == B200A_PAD_CONSTANT) {
+  if (pad_mode == kPadSymmetric) {
+    acc = at(half - 1 - s, acc);
+    acc = at(half + s, acc);
+    acc = at(half + 2 * length - 1 - s, acc);
+  } else if (half == 0 || pad_mode == B200A_PAD_CONSTANT) {
     acc = at(half + j, acc);
   } else if (pad_mode == B200A_PAD_REFLECT) {
     if (j >= 1 && j <= half) acc = at(half - j, acc);
@@ -1004,12 +1019,43 @@ size_t frontend_backward_scratch(const b200a_frontend_desc* d, int stage, int64_
   return align_up(sizeof(float2) * n * n_bins, 256) + frame_bytes + align_up(sizeof(int) * n, 256);
 }
 
+// The composition's middle: the forward spectrum `spec` (frame-major, onesided) becomes H * N * scale^2 in place
+// (spec_vjp_kernel), then scale * w * N * irfft(H) of every frame goes to frame_buf (the iSTFT frame stage).
+static int spec_vjp_frames(const b200a_frontend_desc* d, const void* ws, int stage, float2* spec, const float* grad,
+                           int64_t gs_row, int64_t gs_frame, int64_t gs_col, int* bad, int64_t rows, int64_t frames,
+                           float* frame_buf, cudaStream_t stream) {
+  const WsLayout l = ws_layout(*d);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const int64_t n = rows * frames;
+  const int n_bins = d->onesided ? d->n_fft / 2 + 1 : d->n_fft;
+  SpecVjpParams p{};
+  p.spec = spec;
+  p.grad = grad;
+  p.gs_row = gs_row;
+  p.gs_frame = gs_frame;
+  p.gs_col = gs_col;
+  p.bad = bad;
+  p.fb = reinterpret_cast<const float*>(base + l.fb);
+  p.bands = reinterpret_cast<const int2*>(base + l.bands);
+  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.frames = frames;
+  p.total = n;
+  p.n_fft = d->n_fft;
+  p.n_bins = n_bins;
+  p.n_mels = d->n_mels;
+  p.stage = stage;
+  p.power = d->power;
+  const size_t smem = stage == B200A_STAGE_MEL ? sizeof(int2) * n_bins : 0;
+  const int rc = launch_kernel(spec_vjp_kernel, sm_capped_grid((n + 7) / 8, 8), 256, smem, stream, p);
+  if (rc != B200A_OK) return rc;
+  return istft_frames_impl(d, ws, reinterpret_cast<const float*>(spec), rows, frames, frames * n_bins, 1, n_bins, frame_buf,
+                           stream);
+}
+
 int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                            int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
                            int64_t gs_frame, int64_t gs_col, void* scratch, float* grad_wave, int64_t grad_row_stride,
                            cudaStream_t stream) {
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
   const int64_t n = rows * frames;
   unsigned char* sc = static_cast<unsigned char*>(scratch);
   float* frame_buf;
@@ -1029,35 +1075,15 @@ int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int sta
     rc = frontend_run_impl(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames, spec_f, nullptr, 1, stream,
                            nullptr);
     if (rc != B200A_OK) return rc;
-    SpecVjpParams p{};
-    p.spec = spec;
-    p.grad = grad;
-    p.gs_row = gs_row;
-    p.gs_frame = gs_frame;
-    p.gs_col = gs_col;
-    p.bad = bad;
-    p.fb = reinterpret_cast<const float*>(base + l.fb);
-    p.bands = reinterpret_cast<const int2*>(base + l.bands);
-    p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
-    p.frames = frames;
-    p.total = n;
-    p.n_fft = d->n_fft;
-    p.n_bins = n_bins;
-    p.n_mels = d->n_mels;
-    p.stage = stage;
-    p.power = d->power;
-    const size_t smem = stage == B200A_STAGE_MEL ? sizeof(int2) * n_bins : 0;
-    rc = launch_kernel(spec_vjp_kernel, sm_capped_grid((n + 7) / 8, 8), 256, smem, stream, p);
-    if (rc != B200A_OK) return rc;
-    rc = istft_frames_impl(d, ws, spec_f, rows, frames, frames * n_bins, 1, n_bins, frame_buf, stream);
+    rc = spec_vjp_frames(d, ws, stage, spec, grad, gs_row, gs_frame, gs_col, bad, rows, frames, frame_buf, stream);
   }
   if (rc != B200A_OK) return rc;
   const int64_t bpr = (length + 255) / 256;
   if (bpr == 0) return B200A_OK;
   if (rows * bpr > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  frame_fold_kernel<<<(unsigned)(rows * bpr), 256, 0, stream>>>(frame_buf, bad, d->n_fft, d->hop, frames, length, d->pad,
-                                                                d->center ? d->n_fft / 2 : 0, d->pad_mode, bpr, grad_wave,
-                                                                grad_row_stride);
+  frame_fold_kernel<<<(unsigned)(rows * bpr), 256, 0, stream>>>(frame_buf, bad, d->n_fft, d->n_fft, d->hop, frames, length,
+                                                                d->pad, d->center ? d->n_fft / 2 : 0, d->pad_mode, bpr,
+                                                                grad_wave, grad_row_stride);
   return launch_status();
 }
 
@@ -1127,6 +1153,203 @@ int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const floa
   if (grid < 0) return B200A_ECUDA;
   istft_grad_scale_kernel<<<(unsigned)grid, 256, 0, stream>>>(
       reinterpret_cast<float2*>(grad_spec), n, d->n_fft, n_bins, reinterpret_cast<const WsHeader*>(base + l.header));
+  return launch_status();
+}
+
+// ------------------------------------------------------------------------------------------
+// waveform gradient of the Kaldi features (b200a_kaldi_backward), torch's autograd of compliance/kaldi.py:154-316,
+// :600-645 in reverse: the log and energy floor at the recomputed pre-log values (kaldi_log_vjp_kernel), the power /
+// mel adjoint and the inverse transform (spec_vjp_frames), the per-frame conditioning adjoint (kaldi_cond_vjp_kernel)
+// and the framing fold (frame_fold_kernel, kPadSymmetric for mirrored edges).
+// ------------------------------------------------------------------------------------------
+// d log(max(v, eps)) / dv times g, with torch's rules: 1/v above eps, half of 1/eps on the tie, 0 below
+__device__ __forceinline__ float kaldi_log_vjp(float v, float g) {
+  return v > kKaldiEps ? g / v : (v == kKaldiEps ? 0.5f * (g / kKaldiEps) : 0.f);
+}
+
+// One thread per (frame, column) of the feature rows.  pre: the forward's values before the log, and E at the energy
+// column (frontend_run_impl with kaldi_prelog).  In place, each value column becomes dL/dv and the energy column 0 (a
+// spectrogram's bin 0 holds the energy: |X_0|^2 gets no gradient); dL/dE of each frame goes to g_energy.  The floor is
+// compared with logf(energy_floor), the value the forward clamps with, so ties are the forward's ties.
+__global__ void __launch_bounds__(256) kaldi_log_vjp_kernel(const float* __restrict__ grad, int64_t gs_row, int64_t gs_frame,
+                                                            int64_t gs_col, float* __restrict__ pre,
+                                                            float* __restrict__ g_energy, int64_t frames, int64_t n,
+                                                            int width, int energy_col, int has_energy, int use_log,
+                                                            float energy_floor) {
+  const int64_t total = n * width;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t f = i / width, row = f / frames, t = f - row * frames;
+    const int c = (int)(i - f * width);
+    const float g = grad[row * gs_row + t * gs_frame + c * gs_col];
+    const float v = pre[i];
+    if (c == energy_col) {
+      if (has_energy) {
+        float gl = g;
+        if (energy_floor > 0.f) {
+          const float le = logf(fmaxf(v, kKaldiEps)), fl = logf(energy_floor);
+          gl = le > fl ? g : (le == fl ? 0.5f * g : 0.f);
+        }
+        g_energy[f] = kaldi_log_vjp(v, gl);
+      }
+      pre[i] = 0.f;
+    } else {
+      pre[i] = use_log ? kaldi_log_vjp(v, g) : g;
+    }
+  }
+}
+
+struct KaldiCondParams {
+  float* frame_buf;        // [rows][frames][n_fft]: w * dL/dv in, dL/d(raw frame) out (first win samples)
+  const float* g_energy;   // [rows][frames] dL/dE (energy_mode != 0)
+  const float* wave;
+  const float* window;     // [n_fft] Kaldi window, zero beyond win
+  int64_t length, row_stride, frames, total;
+  int n_fft, win, hop, snip, dc, energy_mode;
+  float preemph;
+};
+
+// Step 6 of the adjoint, one warp per frame, in place: d_p = w (d_v + 2 v g_E) [windowed energy], pre-emphasis
+// d_s[n] = d_p[n] - c d_p[n+1] (d_s[0] = (1 - c) d_p[0] - c d_p[1]), d_s += 2 s g_E [raw energy], DC removal
+// d_s - mean(d_s).  s and v (only with an energy column) are re-gathered from the waveform the way the forward forms
+// them.  Fixed lane order and shuffle tree: reruns are bit-identical.
+__global__ void __launch_bounds__(256) kaldi_cond_vjp_kernel(const KaldiCondParams p) {
+  const int lane = threadIdx.x & 31, win = p.win;
+  const float c = p.preemph;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t f = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); f < p.total; f += warps) {
+    const int64_t row = f / p.frames, t = f - row * p.frames;
+    const float* __restrict__ x = p.wave + row * p.row_stride;
+    float* d = p.frame_buf + f * p.n_fft;
+    auto raw = [&](int n) { return kaldi_sample(x, p.length, t, n, win, p.hop, p.snip); };
+    const float ge = p.energy_mode != 0 ? p.g_energy[f] : 0.f;
+    float mean = 0.f;
+    if (p.energy_mode != 0 && p.dc) {
+      float sum = 0.f;
+      for (int n = lane; n < win; n += 32) sum += raw(n);
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      mean = sum / (float)win;
+    }
+    auto dp = [&](int n) {
+      if (n >= win) return 0.f;
+      float v = d[n];
+      if (p.energy_mode == 2) {
+        const float w = p.window[n];
+        const float vn = ((raw(n) - mean) - c * (raw(n > 0 ? n - 1 : 0) - mean)) * w;
+        v = fmaf(w, 2.f * vn * ge, v);
+      }
+      return v;
+    };
+    float sum = 0.f;
+    for (int base = 0; base < win; base += 32) {
+      const int n = base + lane;
+      float ds = 0.f;
+      if (n < win) {
+        const float a = dp(n), b = dp(n + 1);
+        ds = (n == 0 ? (1.f - c) * a : a) - c * b;
+        if (p.energy_mode == 1) ds = fmaf(2.f * (raw(n) - mean), ge, ds);
+      }
+      __syncwarp();  // every lane has read d[n + 1] before it is overwritten
+      if (n < win) d[n] = ds;
+      sum += ds;
+    }
+    if (p.dc) {
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      const float md = sum / (float)win;
+      __syncwarp();
+      for (int n = lane; n < win; n += 32) d[n] -= md;
+    }
+    __syncwarp();
+  }
+}
+
+namespace {
+struct KaldiScratch {
+  size_t pre, g_energy, bad, spec, frames, total;
+};
+
+// The complex spectrum is composition-only (the fused kernel keeps X in registers).
+KaldiScratch kaldi_scratch_layout(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d, bool fused, int64_t rows,
+                                  int64_t frames) {
+  const size_t n = (size_t)rows * (size_t)frames, n_bins = fused ? 0 : d->n_fft / 2 + 1;
+  KaldiScratch s{};
+  s.pre = 0;
+  s.g_energy = align_up(sizeof(float) * n * kd->out_width, 256);
+  s.bad = s.g_energy + align_up(sizeof(float) * n, 256);
+  s.spec = s.bad + align_up(sizeof(int) * n, 256);
+  s.frames = s.spec + align_up(sizeof(float2) * n * n_bins, 256);
+  s.total = s.frames + align_up(sizeof(float) * n * d->n_fft, 256);
+  return s;
+}
+}  // namespace
+
+size_t kaldi_backward_scratch(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d, int stage, int64_t rows,
+                              int64_t length, int64_t frames) {
+  return kaldi_scratch_layout(kd, d, kaldi_backward_fused_applicable(d, kd, stage, length), rows, frames).total;
+}
+
+int kaldi_backward_impl(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d, const void* ws, int stage,
+                        const float* wave, int64_t rows, int64_t length, int64_t row_stride, int64_t frames,
+                        const float* grad, int64_t gs_row, int64_t gs_frame, int64_t gs_col, void* scratch,
+                        float* grad_wave, int64_t grad_row_stride, cudaStream_t stream) {
+  const bool fused = kaldi_backward_fused_applicable(d, kd, stage, length);
+  const KaldiScratch s = kaldi_scratch_layout(kd, d, fused, rows, frames);
+  unsigned char* sc = static_cast<unsigned char*>(scratch);
+  float* pre = reinterpret_cast<float*>(sc + s.pre);
+  float* g_energy = reinterpret_cast<float*>(sc + s.g_energy);
+  int* bad = reinterpret_cast<int*>(sc + s.bad);
+  float2* spec = reinterpret_cast<float2*>(sc + s.spec);
+  float* frame_buf = reinterpret_cast<float*>(sc + s.frames);
+  const int64_t n = rows * frames;
+  const int energy_mode = kd->energy_col >= 0 ? kd->energy_mode : 0;
+  // the forward's own kernel with the log and floor off: the values it took the log of, bit for bit
+  int rc = frontend_run_impl(d, ws, stage, wave, rows, length, row_stride, frames, pre, nullptr, 1, stream, kd, true);
+  if (rc != B200A_OK) return rc;
+  const int64_t elems = n * kd->out_width;
+  int64_t grid = sm_capped_grid((elems + 255) / 256, 8);
+  if (grid < 0) return B200A_ECUDA;
+  kaldi_log_vjp_kernel<<<(unsigned)grid, 256, 0, stream>>>(grad, gs_row, gs_frame, gs_col, pre, g_energy, frames, n,
+                                                           kd->out_width, kd->energy_col, energy_mode != 0, kd->use_log,
+                                                           kd->energy_floor);
+  rc = launch_status();
+  if (rc != B200A_OK) return rc;
+  const float* g_v = pre + kd->out_col0;
+  const int64_t gv_row = frames * kd->out_width, gv_frame = kd->out_width;
+  if (fused) {  // padded 256 / 512 / 1024: X recomputed in registers, G -> H -> inverse transform in one kernel
+    bad = nullptr;  // the kernel writes a NaN frame's gradient as NaN itself
+    rc = kaldi_backward_pow2(d, kd, ws, stage, wave, rows, length, row_stride, frames, g_v, gv_row, gv_frame, 1, frame_buf,
+                             stream);
+  } else {  // composition: the conditioned complex spectrum, its adjoint in place, the iSTFT frame stage
+    rc = frontend_run_impl(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames,
+                           reinterpret_cast<float*>(spec), nullptr, 1, stream, kd);
+    if (rc != B200A_OK) return rc;
+    rc = spec_vjp_frames(d, ws, stage, spec, g_v, gv_row, gv_frame, 1, bad, rows, frames, frame_buf, stream);
+  }
+  if (rc != B200A_OK) return rc;
+  KaldiCondParams cp{};
+  cp.frame_buf = frame_buf;
+  cp.g_energy = g_energy;
+  cp.wave = wave;
+  cp.window = reinterpret_cast<const float*>(static_cast<const unsigned char*>(ws) + ws_layout(*d).window);
+  cp.length = length;
+  cp.row_stride = row_stride;
+  cp.frames = frames;
+  cp.total = n;
+  cp.n_fft = d->n_fft;
+  cp.win = kd->window_size;
+  cp.hop = kd->window_shift;
+  cp.snip = kd->snip_edges;
+  cp.dc = kd->remove_dc_offset;
+  cp.energy_mode = energy_mode;
+  cp.preemph = kd->preemphasis;
+  rc = launch_kernel(kaldi_cond_vjp_kernel, sm_capped_grid((n + 7) / 8, 8), 256, 0, stream, cp);
+  if (rc != B200A_OK) return rc;
+  const int64_t bpr = (length + 255) / 256;
+  if (rows * bpr > 0x7fffffffLL) return B200A_EUNSUPPORTED;
+  const int lead = kd->snip_edges ? 0 : kd->window_size / 2 - kd->window_shift / 2;
+  frame_fold_kernel<<<(unsigned)(rows * bpr), 256, 0, stream>>>(frame_buf, bad, d->n_fft, kd->window_size, kd->window_shift,
+                                                                frames, length, 0, lead,
+                                                                kd->snip_edges ? B200A_PAD_CONSTANT : kPadSymmetric, bpr,
+                                                                grad_wave, grad_row_stride);
   return launch_status();
 }
 

@@ -35,7 +35,6 @@ namespace b200a {
 
 namespace {
 
-constexpr int kPadSymmetric = 4;  // internal pad mode: x[-1-j] = x[j], x[L+j] = x[L-1-j] (Kaldi snip_edges = false)
 constexpr int kWarps = 8;     // transform warps per CTA (n_fft = 2048 kernels)
 constexpr int kMelWarps = 4;  // contraction warps per CTA (n_fft = 2048 mel kernel)
 constexpr int kUniWarps = 16;  // warps per CTA of the 256 / 512 / 1024-point mel kernel, each transforms and contracts
@@ -206,6 +205,7 @@ struct Pow2Params {
   int out_width, out_col0, out_vec;  // out_vec: floats every row start is aligned to (1, 2 or 4)
   // Kaldi framing / per-frame conditioning (compliance/kaldi.py:44-83, :153-216); kaldi == 0: torch.stft framing
   int kaldi, k_off, k_win, k_dc, k_energy_mode, k_energy_col, k_log;
+  int k_prelog;  // the gradient's recompute: the energy column receives E itself, not its floored log
   float k_preemph, k_energy_floor;
   float power, db_mult, db_amin, db_offset;
   // iSTFT adjoint (kIstftGrad): frames [env_t_lo, env_t_hi] have the full window envelope at every sample
@@ -505,6 +505,8 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
     const float* fa = stage + 2 * gi * p.hop;
     const float* fb = fa + p.hop;
     const int win = p.k_win;
+    // the gradient kernel (kSpectra) forms no energy: its adjoint runs in kaldi_cond_vjp_kernel
+    const int energy_mode = POWER_MODE == kSpectra ? 0 : p.k_energy_mode;
     float ma = 0.f, mb = 0.f;
     if (p.k_dc) {
 #pragma unroll 4
@@ -521,7 +523,7 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       mb /= (float)win;
     }
     float ea = 0.f, eb = 0.f;
-    if (p.k_energy_mode == 1) {
+    if (energy_mode == 1) {
 #pragma unroll 4
       for (int n = l; n < win; n += G) {
         const float da = fa[n] - ma, db = fb[n] - mb;
@@ -541,12 +543,12 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
         vb = ((fb[n] - mb) - c * (fb[np] - mb)) * w;
       }
       a[brev5(j)] = make_float2(va, vb);
-      if (p.k_energy_mode == 2) {  // s_win carries the un-packing's 1/2
+      if (energy_mode == 2) {  // s_win carries the un-packing's 1/2
         ea = fmaf(2.f * va, 2.f * va, ea);
         eb = fmaf(2.f * vb, 2.f * vb, eb);
       }
     });
-    if (p.k_energy_mode != 0) {
+    if (energy_mode != 0) {
 #pragma unroll
       for (int o = G / 2; o > 0; o >>= 1) {
         ea += __shfl_xor_sync(0xffffffffu, ea, o);
@@ -555,8 +557,8 @@ __device__ __forceinline__ void transform_unit(const Pow2Params& p, const float*
       if (l == 0) {
         const float fl = p.k_energy_floor > 0.f ? logf(p.k_energy_floor) : -CUDART_INF_F;
         float* e_out = p.out + (row * p.frames + ta) * p.out_width + p.k_energy_col;
-        if (has_a) e_out[0] = fmaxf(logf(fmaxf(ea, kKaldiEps)), fl);
-        if (has_b) e_out[p.out_width] = fmaxf(logf(fmaxf(eb, kKaldiEps)), fl);
+        if (has_a) e_out[0] = p.k_prelog ? ea : fmaxf(logf(fmaxf(ea, kKaldiEps)), fl);
+        if (has_b) e_out[p.out_width] = p.k_prelog ? eb : fmaxf(logf(fmaxf(eb, kKaldiEps)), fl);
       }
     }
     __syncwarp();  // every lane has consumed the staging buffer
@@ -1307,7 +1309,9 @@ constexpr size_t bwd_smem_fixed() {  // twiddles, window, transpose tiles, per-b
   return sizeof(float2) * (32 * G + kBwWarps * Geo<G>::kTileF2) + sizeof(float) * Geo<G>::kNfft + sizeof(int2) * Geo<G>::kBins;
 }
 
-template <int G, int STAGE>
+// KALDI: the Kaldi variant (b200a_kaldi_backward): X is recomputed with transform_unit's Kaldi load stage (framing with
+// mirrored edges, DC removal, pre-emphasis, window), and `grad` holds dL/dv of the spectral values after the log adjoint.
+template <int G, int STAGE, bool KALDI>
 __global__ void __launch_bounds__(kBwWarps * 32, 1) stft_pow2_backward_kernel(const BwdParams bp) {
   using Ge = Geo<G>;
   constexpr int N = Ge::kNfft;
@@ -1338,7 +1342,7 @@ __global__ void __launch_bounds__(kBwWarps * 32, 1) stft_pow2_backward_kernel(co
   cur.init((int64_t)blockIdx.x * kBwWarps + warp, (int64_t)gridDim.x * kBwWarps, p.units_per_row);
   for (; cur.u < p.total_units; cur.advance()) {
     float2 xa[17], xb[17];
-    transform_unit<kSpectra, G, -1, false, false>(p, s_win, s_tw, tile, nullptr, parity, staged, cur, half, lane, xa, xb);
+    transform_unit<kSpectra, G, -1, KALDI, false>(p, s_win, s_tw, tile, nullptr, parity, staged, cur, half, lane, xa, xb);
     const int64_t t0 = cur.ub * Ge::kFrames, ta = t0 + 2 * gi, tb = ta + 1;
     const bool has_a = ta < p.frames, has_b = tb < p.frames;
     const float* ga = bp.grad + (cur.row * bp.gs_row + ta * bp.gs_frame) * (STAGE == B200A_STAGE_COMPLEX ? 2 : 1);
@@ -1658,7 +1662,7 @@ static Pow2Params pow2_geometry(const b200a_frontend_desc& d, const void* ws, co
 
 int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                       int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
-                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd) {
+                      int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd, bool kaldi_prelog) {
   if (!pow2_applicable(*d)) return kPathDeclined;
   if (stage == B200A_STAGE_COMPLEX && (d->n_fft > 1024 || kd != nullptr)) return kPathDeclined;
   // Kaldi features with a 256 / 512 / 1024-point FFT; every other size takes the generic kernel
@@ -1694,7 +1698,8 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
     p.k_energy_mode = kd->energy_col >= 0 ? kd->energy_mode : 0;
     p.k_energy_floor = kd->energy_floor;
     p.k_energy_col = kd->energy_col;
-    p.k_log = kd->use_log;
+    p.k_log = kaldi_prelog ? 0 : kd->use_log;
+    p.k_prelog = kaldi_prelog;
     p.out_width = kd->out_width;
     p.out_col0 = kd->out_col0;
     p.pad_mode = kPadSymmetric;  // only reached when snip_edges == 0 (frames never leave the signal otherwise)
@@ -1781,9 +1786,55 @@ int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int sta
   const int64_t grid = persistent_grid(bp.f.total_units, kBwWarps);
   return with_g(d->n_fft, [&](auto g) {
     constexpr int G = decltype(g)::value;
-    auto kern = stage == B200A_STAGE_COMPLEX ? stft_pow2_backward_kernel<G, B200A_STAGE_COMPLEX>
-                : stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<G, B200A_STAGE_POWER>
-                                             : stft_pow2_backward_kernel<G, B200A_STAGE_MEL>;
+    auto kern = stage == B200A_STAGE_COMPLEX ? stft_pow2_backward_kernel<G, B200A_STAGE_COMPLEX, false>
+                : stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<G, B200A_STAGE_POWER, false>
+                                             : stft_pow2_backward_kernel<G, B200A_STAGE_MEL, false>;
+    return launch_kernel(kern, grid, kBwWarps * 32, smem, stream, bp);
+  });
+}
+
+// The Kaldi gradient takes the fused kernel when the padded size is 256 / 512 / 1024, the staged g rows fit shared
+// memory (backward_smem) and a unit's span fits the transpose tile the Kaldi load stage conditions in -- all decided by
+// the descriptors and the signal length, never by the batch.
+bool kaldi_backward_fused_applicable(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, int stage, int64_t length) {
+  if (backward_smem(d, stage) == 0) return false;
+  const int64_t span = d->n_fft + (unit_frames(d->n_fft) - 1) * (int64_t)kd->window_shift;
+  return span <= stage_floats(d->n_fft, false) && length + d->n_fft < (int64_t)1 << 31;
+}
+
+// Frame gradients w * N * irfft(H) of the Kaldi features for padded 256 / 512 / 1024: `grad` is the log adjoint's dL/dv
+// (value k or filter m of frame t at grad[row gs_row + t gs_frame + (k | m) gs_col]).
+int kaldi_backward_pow2(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, const void* ws, int stage,
+                        const float* wave, int64_t rows, int64_t length, int64_t row_stride, int64_t frames,
+                        const float* grad, int64_t gs_row, int64_t gs_frame, int64_t gs_col, float* frame_buf,
+                        cudaStream_t stream) {
+  if (!kaldi_backward_fused_applicable(d, kd, stage, length)) return kPathDeclined;
+  const size_t smem = backward_smem(d, stage);
+  const WsLayout l = ws_layout(*d);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  BwdParams bp{};
+  bp.f = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, stage_floats(d->n_fft, false));
+  bp.f.n_mels = stage == B200A_STAGE_MEL ? d->n_mels : 0;
+  bp.f.stage = stage;
+  bp.f.kaldi = 1;
+  bp.f.k_off = kd->snip_edges ? 0 : kd->window_size / 2 - kd->window_shift / 2;
+  bp.f.k_win = kd->window_size;
+  bp.f.k_dc = kd->remove_dc_offset;
+  bp.f.k_preemph = kd->preemphasis;
+  bp.f.k_energy_mode = 0;  // the energy's adjoint is kaldi_cond_vjp_kernel's; nothing is written to an output row
+  bp.f.pad_mode = kPadSymmetric;
+  bp.grad = grad;
+  bp.gs_row = gs_row;
+  bp.gs_frame = gs_frame;
+  bp.gs_col = gs_col;
+  bp.frame_buf = frame_buf;
+  bp.fb = reinterpret_cast<const float*>(base + l.fb);
+  bp.bands = reinterpret_cast<const int2*>(base + l.bands);
+  const int64_t grid = persistent_grid(bp.f.total_units, kBwWarps);
+  return with_g(d->n_fft, [&](auto g) {
+    constexpr int G = decltype(g)::value;
+    auto kern = stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<G, B200A_STAGE_POWER, true>
+                                           : stft_pow2_backward_kernel<G, B200A_STAGE_MEL, true>;
     return launch_kernel(kern, grid, kBwWarps * 32, smem, stream, bp);
   });
 }

@@ -12,8 +12,8 @@ spectrum through HBM) -- they read the sub-modules' buffers and launch the fused
 
 Gradients are opt-in, per thread: Spectrogram and MelSpectrogram inside ``audio_b200.differentiable()``,
 InverseSpectrogram with ``inverse=True``, Resample / Speed / SpeedPerturbation with ``resample=True``, and MFCC,
-LFCC, AmplitudeToDB, MelScale and SpectralCentroid with ``features=True``.  GriffinLim, TimeStretch, PitchShift and
-the Kaldi features are forward-only.
+LFCC, AmplitudeToDB, MelScale and SpectralCentroid with ``features=True``, and the Kaldi features
+(``audio_b200.compliance.kaldi``) with ``kaldi=True``.  GriffinLim, TimeStretch and PitchShift are forward-only.
 """
 from __future__ import annotations
 

@@ -364,6 +364,25 @@ int b200a_kaldi_run(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* de
                     int32_t stage, const float* wave, int64_t rows, int64_t length, int64_t row_stride,
                     float* out, b200a_stream stream);
 
+/*
+ * Waveform gradient of b200a_kaldi_run (stage POWER or MEL): torch's autograd of the reference op sequence, ties
+ * included -- log(max(v, FLT_EPSILON)) gives 1/v above, half of 1/FLT_EPSILON on the tie and 0 below, and the energy
+ * floor splits the same way; the decisions are taken from the pre-log values recomputed by the forward's own kernel.
+ *   grad_out  : [rows][m][out_width] at element strides g_stride_* (0 allowed: an expanded gradient)
+ *   grad_wave : [rows][length] at row stride grad_row_stride >= length; every sample is written
+ *   scratch   : b200a_kaldi_backward_scratch_bytes(...) bytes
+ * Status codes as b200a_kaldi_run; B200A_EINVAL also for a null grad_out, scratch or grad_wave.  No atomics: reruns
+ * are bit-identical and a row's gradient does not depend on the other rows.
+ */
+int b200a_kaldi_backward(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* desc, const void* workspace,
+                         int32_t stage, const float* wave, int64_t rows, int64_t length, int64_t row_stride,
+                         const float* grad_out, int64_t g_stride_row, int64_t g_stride_frame, int64_t g_stride_col,
+                         void* scratch, float* grad_wave, int64_t grad_row_stride, b200a_stream stream);
+/* Scratch bytes of b200a_kaldi_backward: the recomputed pre-log rows, the per-frame energy gradient and NaN flag, the
+ * complex spectrum and the frame gradients (rows * m * padded_size floats).  0 for an invalid request. */
+size_t b200a_kaldi_backward_scratch_bytes(const b200a_kaldi_desc* kaldi, const b200a_frontend_desc* desc, int32_t stage,
+                                          int64_t rows, int64_t length);
+
 /* x[r][t][c] -= mean_t x[r][t][c], in place, for each of `rows` feature matrices (_subtract_column_mean, :219-226). */
 int b200a_subtract_column_mean(float* x, int64_t rows, int64_t frames, int64_t width, b200a_stream stream);
 

@@ -51,6 +51,10 @@ for kw in (dict(num_mel_bins=40, snip_edges=False, use_energy=True), dict(num_me
     K.fbank_batch(x * 1000, **kw)
 K.mfcc_batch(x * 1000, subtract_mean=True)
 K.spectrogram_batch(x * 1000)
+with audio_b200.differentiable(kaldi=True):  # Kaldi waveform gradients: 512-point frames with mirrored edges, 400-point
+    for fn, kw in ((K.fbank_batch, dict(num_mel_bins=40, snip_edges=False, use_energy=True)),
+                   (K.mfcc_batch, dict(round_to_power_of_two=False, use_energy=True, subtract_mean=True))):
+        fn((x * 1000).requires_grad_(), **kw).sum().backward()
 T.Resample(44100, 16000).cuda()(x)
 T.Resample(16000, 22050, resampling_method="sinc_interp_kaiser").cuda()(x)
 with audio_b200.differentiable(resample=True):  # resampler waveform gradients: the mma kernel, the direct kernel
