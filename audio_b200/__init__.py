@@ -13,7 +13,7 @@ from . import _lib  # noqa: F401  (does not load the .so until first use)
 from . import compliance, functional, transforms  # noqa: F401
 from ._plans import (differentiable, is_differentiable, is_feature_differentiable,  # noqa: F401
                      is_inverse_differentiable, is_kaldi_differentiable, is_resample_differentiable,
-                     set_differentiable)
+                     is_vocoder_differentiable, set_differentiable)
 
 __version__ = "0.1.0"
 

@@ -137,6 +137,11 @@ _SIGNATURES = {
         ctypes.c_int,
         [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_double, c_void_p, c_void_p, c_int64, c_void_p],
     ),
+    "b200a_phase_vocoder_backward": (
+        ctypes.c_int,
+        [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_double, c_void_p, c_void_p, c_int64, c_int64,
+         c_int64, c_void_p, c_int64, c_void_p],
+    ),
     "b200a_kaldi_num_frames": (c_int64, [c_int64, c_int32, c_int32, c_int32]),
     "b200a_kaldi_run": (
         ctypes.c_int,

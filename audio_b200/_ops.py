@@ -1,7 +1,7 @@
 """``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
-``resample_backward`` / ``kaldi_run`` / ``kaldi_backward``.
+``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -63,6 +63,9 @@ _LIB.define(
 _LIB.define(
     "kaldi_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int[] kaldi_i, float[] kaldi_f, "
     "int stage, int row_stride, Tensor grad_out) -> Tensor"
+)
+_LIB.define(
+    "phase_vocoder_backward(Tensor spec, Tensor out, Tensor grad, float rate) -> Tensor"
 )
 
 _KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
@@ -368,6 +371,29 @@ def _kaldi_backward_meta(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stag
     return wave.new_empty(wave.shape, dtype=torch.float32)
 
 
+# ---- phase_vocoder_backward --------------------------------------------------------------------------------------
+def _phase_vocoder_backward_cuda(spec, out, grad, rate):
+    """(rows, bins, frames_in) complex64 input of the forward, its (rows, frames_out, bins, 2) frame-major output and
+    the (rows, bins, frames_out) complex upstream gradient at any strides (0 included) -> (rows, frames_in, bins, 2)
+    frame-major spectrogram gradient."""
+    rows, bins, frames_in = spec.shape
+    frames_out = out.shape[1]
+    spec_r, ss = _complex_strides(torch.view_as_real(spec.resolve_conj()))
+    grad_r, gs = _complex_strides(torch.view_as_real(grad.resolve_conj()))
+    dev = spec.device
+    with torch.cuda.device(dev):
+        gx = torch.empty((rows, frames_in, bins, 2), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_phase_vocoder_backward(
+            spec_r.data_ptr(), ss[0], ss[1], ss[2], rows, bins, frames_in, float(rate), out.data_ptr(), grad_r.data_ptr(),
+            gs[0], gs[1], gs[2], gx.data_ptr(), frames_out, _stream(dev))
+    _lib.check(rc, "phase_vocoder_backward")
+    return gx
+
+
+def _phase_vocoder_backward_meta(spec, out, grad, rate):
+    return spec.new_empty((spec.shape[0], spec.shape[2], spec.shape[1], 2), dtype=torch.float32)
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
@@ -379,7 +405,8 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("resample_run", _resample_run_cuda, _resample_run_meta),
                             ("resample_backward", _resample_backward_cuda, _resample_backward_meta),
                             ("kaldi_run", _kaldi_run_cuda, _kaldi_run_meta),
-                            ("kaldi_backward", _kaldi_backward_cuda, _kaldi_backward_meta)):
+                            ("kaldi_backward", _kaldi_backward_cuda, _kaldi_backward_meta),
+                            ("phase_vocoder_backward", _phase_vocoder_backward_cuda, _phase_vocoder_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -395,3 +422,4 @@ resample_run = torch.ops.b200audio.resample_run
 resample_backward = torch.ops.b200audio.resample_backward
 kaldi_run = torch.ops.b200audio.kaldi_run
 kaldi_backward = torch.ops.b200audio.kaldi_backward
+phase_vocoder_backward = torch.ops.b200audio.phase_vocoder_backward

@@ -59,34 +59,66 @@ def is_kaldi_differentiable() -> bool:
     return getattr(_GRAD_STATE, "kaldi", False)
 
 
+def is_vocoder_differentiable() -> bool:
+    """Whether F.phase_vocoder and TimeStretch accept spectrograms, and F.pitch_shift and PitchShift waveforms, that
+    require grad (in this thread)."""
+    return getattr(_GRAD_STATE, "vocoder", False)
+
+
 def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = False, features: bool = False,
-                       kaldi: bool = False) -> None:
+                       kaldi: bool = False, vocoder: bool = False) -> None:
     """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
     ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT, ``resample=True``
     (with ``mode``) the waveform gradients of the resampler, ``features=True`` (with ``mode``) the input gradients of
     MFCC, LFCC, AmplitudeToDB, MelScale and SpectralCentroid, ``kaldi=True`` (with ``mode``) the waveform gradients of
-    the Kaldi spectrogram, fbank and mfcc.  They are separate switches so that vocoder inference, augmentation code
-    (Speed, SpeedPerturbation) and Kaldi feature preprocessing in data pipelines do not build graphs when loss
-    gradients are on, and so that the top_db clamp's gradient -- every clamped element's share goes to the group
-    maximum -- is opted into knowingly."""
+    the Kaldi spectrogram, fbank and mfcc, ``vocoder=True`` (with ``mode``) the spectrogram gradients of the phase
+    vocoder and TimeStretch and the waveform gradients of PitchShift.  They are separate switches so that vocoder
+    inference, augmentation code (Speed, SpeedPerturbation, TimeStretch, PitchShift) and Kaldi feature preprocessing in
+    data pipelines do not build graphs when loss gradients are on, and so that the top_db clamp's gradient -- every
+    clamped element's share goes to the group maximum -- is opted into knowingly."""
     _GRAD_STATE.on = bool(mode)
     _GRAD_STATE.inverse = bool(mode) and bool(inverse)
     _GRAD_STATE.resample = bool(mode) and bool(resample)
     _GRAD_STATE.features = bool(mode) and bool(features)
     _GRAD_STATE.kaldi = bool(mode) and bool(kaldi)
+    _GRAD_STATE.vocoder = bool(mode) and bool(vocoder)
+
+
+def _switches():
+    return (is_differentiable(), is_inverse_differentiable(), is_resample_differentiable(), is_feature_differentiable(),
+            is_kaldi_differentiable(), is_vocoder_differentiable())
+
+
+def _restore(prev) -> None:
+    set_differentiable(prev[0], inverse=prev[1], resample=prev[2], features=prev[3], kaldi=prev[4], vocoder=prev[5])
 
 
 @contextlib.contextmanager
 def differentiable(mode: bool = True, *, inverse: bool = False, resample: bool = False, features: bool = False,
-                   kaldi: bool = False):
+                   kaldi: bool = False, vocoder: bool = False):
     """Context manager form of :func:`set_differentiable`; restores the previous settings on exit."""
-    prev = (is_differentiable(), is_inverse_differentiable(), is_resample_differentiable(), is_feature_differentiable(),
-            is_kaldi_differentiable())
-    set_differentiable(mode, inverse=inverse, resample=resample, features=features, kaldi=kaldi)
+    prev = _switches()
+    set_differentiable(mode, inverse=inverse, resample=resample, features=features, kaldi=kaldi, vocoder=vocoder)
     try:
         yield
     finally:
-        set_differentiable(prev[0], inverse=prev[1], resample=prev[2], features=prev[3], kaldi=prev[4])
+        _restore(prev)
+
+
+@contextlib.contextmanager
+def vocoder_chain(waveform: torch.Tensor):
+    """PitchShift's stages (STFT, phase vocoder, inverse STFT, resampler) for one call: with ``vocoder=True`` on and a
+    waveform that requires grad, the front-end, inverse and resampler gradients are on too for the duration of the call,
+    and the caller's switches are restored on exit.  Otherwise the switches stay as they are."""
+    if not (is_vocoder_differentiable() and torch.is_grad_enabled() and waveform.requires_grad):
+        yield
+        return
+    prev = _switches()
+    set_differentiable(True, inverse=True, resample=True, features=prev[3], kaldi=prev[4], vocoder=True)
+    try:
+        yield
+    finally:
+        _restore(prev)
 
 
 def _no_autograd(t: torch.Tensor) -> None:
@@ -99,7 +131,8 @@ def _no_autograd(t: torch.Tensor) -> None:
             "and SpeedPerturbation compute waveform gradients inside audio_b200.differentiable(resample=True); MFCC, LFCC, "
             "AmplitudeToDB, MelScale and SpectralCentroid compute input gradients inside "
             "audio_b200.differentiable(features=True); compliance.kaldi spectrogram, fbank and mfcc compute waveform "
-            "gradients inside audio_b200.differentiable(kaldi=True).)"
+            "gradients inside audio_b200.differentiable(kaldi=True); F.phase_vocoder and TimeStretch compute spectrogram "
+            "gradients, F.pitch_shift and PitchShift waveform gradients, inside audio_b200.differentiable(vocoder=True).)"
         )
 
 

@@ -288,6 +288,19 @@ int b200a_phase_vocoder(const float* spec, int64_t stride_row, int64_t stride_bi
                             frames_out, static_cast<cudaStream_t>(stream));
 }
 
+int b200a_phase_vocoder_backward(const float* spec, int64_t stride_row, int64_t stride_bin, int64_t stride_frame,
+                                 int64_t rows, int64_t bins, int64_t frames_in, double rate, const float* out,
+                                 const float* grad, int64_t g_stride_row, int64_t g_stride_bin, int64_t g_stride_frame,
+                                 float* grad_spec, int64_t frames_out, b200a_stream stream) {
+  if (rows < 0 || bins < 1 || frames_in < 1 || frames_out < 1 || !(rate > 0.0)) return B200A_EINVAL;
+  if (g_stride_row < 0 || g_stride_bin < 0 || g_stride_frame < 0) return B200A_EINVAL;
+  if (rows == 0) return B200A_OK;
+  if (spec == nullptr || out == nullptr || grad == nullptr || grad_spec == nullptr) return B200A_EINVAL;
+  return phase_vocoder_backward_impl(spec, stride_row, stride_bin, stride_frame, rows, bins, frames_in, rate, out, grad,
+                                     g_stride_row, g_stride_bin, g_stride_frame, grad_spec, frames_out,
+                                     static_cast<cudaStream_t>(stream));
+}
+
 int64_t b200a_kaldi_num_frames(int64_t length, int32_t window_size, int32_t window_shift, int32_t snip_edges) {
   if (length < 0 || window_size < 1 || window_shift < 1) return -1;
   if (snip_edges) return length < window_size ? 0 : 1 + (length - window_size) / window_shift;

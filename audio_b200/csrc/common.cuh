@@ -157,6 +157,10 @@ int griffinlim_update_impl(const float* mag, int64_t ms_row, int64_t ms_bin, int
 int phase_vocoder_impl(const float* spec, int64_t s_row, int64_t s_bin, int64_t s_frame, int64_t rows, int64_t bins,
                        int64_t frames_in, double rate, const float* phase_advance, float* out, int64_t frames_out,
                        cudaStream_t stream);
+int phase_vocoder_backward_impl(const float* spec, int64_t s_row, int64_t s_bin, int64_t s_frame, int64_t rows,
+                                int64_t bins, int64_t frames_in, double rate, const float* out, const float* grad,
+                                int64_t g_row, int64_t g_bin, int64_t g_frame, float* grad_spec, int64_t frames_out,
+                                cudaStream_t stream);
 
 // feature_backward.cu: input gradients of MFCC / LFCC after the mel stage, AmplitudeToDB, MelScale, SpectralCentroid
 size_t mfcc_backward_scratch(int64_t rows, int64_t frames, int64_t rows_per_group);

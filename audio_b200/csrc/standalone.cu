@@ -176,10 +176,27 @@ int griffinlim_update_impl(const float* mag, int64_t ms_row, int64_t ms_bin, int
   return launch_status();
 }
 
+// The time grid of F.phase_vocoder (torch.arange(0, frames_in, rate, dtype=float32)): step t sits at ts = float(rate * t)
+// of the input; its neighbours are frames trunc(ts) and trunc(ts + 1), the latter computed in float (so not always
+// i0 + 1: it is i0 + 2 when ts + 1 rounds up to the next integer); alpha = ts mod 1.  The forward and its adjoint both
+// take their neighbours from here, so they make the same decisions bit for bit.
+struct VocoderStep {
+  int64_t i0, i1;
+  float alpha;
+};
+
+__device__ __forceinline__ VocoderStep vocoder_step(double rate, int64_t t) {
+  const float ts = (float)(rate * (double)t);
+  VocoderStep s;
+  s.alpha = fmodf(ts, 1.0f);
+  s.i0 = (int64_t)ts;
+  s.i1 = (int64_t)(ts + 1.0f);
+  return s;
+}
+
 // F.phase_vocoder (functional.py:713-803): one thread per (row, bin) walks the output frames in order, carrying the
 // accumulated phase (the reference's cumsum); consecutive threads are consecutive bins of the frame-major output.
-//   time step t' sits at ts = float(rate * t') of the input; its neighbours are frames trunc(ts) and trunc(ts + 1)
-//   (frames >= frames_in are the two zero frames the reference pads); alpha = ts mod 1.
+// Step t' interpolates frames vocoder_step(t').i0 / .i1 (frames >= frames_in are the two zero frames the reference pads).
 __global__ void __launch_bounds__(128) phase_vocoder_kernel(const float2* __restrict__ spec, int64_t s_row, int64_t s_bin,
                                                             int64_t s_frame, int64_t bins, int64_t frames_in, double rate,
                                                             const float* __restrict__ phase_advance,
@@ -197,11 +214,10 @@ __global__ void __launch_bounds__(128) phase_vocoder_kernel(const float2* __rest
   // the neighbours of step t + 1 are fetched before step t's arithmetic, so the global-load latency of the walk hides
   // behind the transcendental chain instead of adding to it
   auto fetch = [&](int64_t t, float& alpha, float2& z0, float2& z1) {
-    const float ts = (float)(rate * (double)t);
-    alpha = fmodf(ts, 1.0f);
-    const int64_t i0 = (int64_t)ts, i1 = (int64_t)(ts + 1.0f);
-    z0 = (t < frames_out && i0 < frames_in) ? sp[i0 * s_frame] : make_float2(0.f, 0.f);
-    z1 = (t < frames_out && i1 < frames_in) ? sp[i1 * s_frame] : make_float2(0.f, 0.f);
+    const VocoderStep s = vocoder_step(rate, t);
+    alpha = s.alpha;
+    z0 = (t < frames_out && s.i0 < frames_in) ? sp[s.i0 * s_frame] : make_float2(0.f, 0.f);
+    z1 = (t < frames_out && s.i1 < frames_in) ? sp[s.i1 * s_frame] : make_float2(0.f, 0.f);
   };
   float alpha, alpha_n;
   float2 z0, z1, z0n, z1n;
@@ -230,6 +246,106 @@ int phase_vocoder_impl(const float* spec, int64_t s_row, int64_t s_bin, int64_t 
   phase_vocoder_kernel<<<dim3((unsigned)((bins + 127) / 128), (unsigned)rows), 128, 0, stream>>>(
       reinterpret_cast<const float2*>(spec), s_row, s_bin, s_frame, bins, frames_in, rate, phase_advance,
       reinterpret_cast<float2*>(out), frames_out);
+  return launch_status();
+}
+
+// Adjoint of phase_vocoder_kernel (include/b200audio.h has the formula).  One thread per (row, bin), as the forward,
+// walks the output frames backwards, t = frames_out - 1 ... 0, carrying the suffix sum S of a_t = dL/dphi_t (the
+// adjoint of the phase cumsum) and the pending accumulators M (magnitude) and P (phase) of the input frames the walk
+// can still reach: frames top, top - 1, top - 2 with top = min(frames_in - 1, i1(t)), since i1 - i0 is 1 or 2 and both
+// only decrease along the walk.  A frame is written once, when the walk passes below it; frames no step touches are
+// written as 0.  S, M and P are double: S sums frames_out terms, and the forward carries its phase in double too.
+__global__ void __launch_bounds__(128) phase_vocoder_backward_kernel(
+    const float2* __restrict__ spec, int64_t s_row, int64_t s_bin, int64_t s_frame, int64_t bins, int64_t frames_in,
+    double rate, const float2* __restrict__ out, const float2* __restrict__ grad, int64_t g_row, int64_t g_bin,
+    int64_t g_frame, float2* __restrict__ grad_spec, int64_t frames_out) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t r = blockIdx.y;
+  if (k >= bins) return;
+  const float2* sp = spec + r * s_row + k * s_bin;
+  const float2* o = out + r * frames_out * bins + k;
+  const float2* g = grad + r * g_row + k * g_bin;
+  float2* gx = grad_spec + r * frames_in * bins + k;
+  // grad_X = sgn(X) M + i X / |X|^2 P = (X / |X|) (M + i P / |X|); exactly 0 at X = 0 (torch's abs / angle backward)
+  auto flush = [&](int64_t i, double m, double p) {
+    const float2 x = sp[i * s_frame];
+    const double n2 = (double)x.x * x.x + (double)x.y * x.y;
+    float2 v = make_float2(0.f, 0.f);
+    if (n2 > 0.0) {
+      const double inv = 1.0 / sqrt(n2), cr = x.x * inv, ci = x.y * inv, q = p * inv;
+      v = make_float2((float)(cr * m - ci * q), (float)(ci * m + cr * q));
+    }
+    gx[i * bins] = v;
+  };
+  double S = 0.0;
+  double m0 = 0.0, p0 = 0.0, m1 = 0.0, p1 = 0.0, m2 = 0.0, p2 = 0.0;  // pending frames top, top - 1, top - 2
+  int64_t top = frames_in - 1;
+  auto add = [&](int64_t i, double dm, double dp) {  // contributions to the pad frames (i > top) are dropped
+    const int64_t d = top - i;
+    if (d == 0) {
+      m0 += dm;
+      p0 += dp;
+    } else if (d == 1) {
+      m1 += dm;
+      p1 += dp;
+    } else if (d == 2) {
+      m2 += dm;
+      p2 += dp;
+    }
+  };
+  // g_t and o_t of the next step are fetched before this step's arithmetic, as the forward prefetches its neighbours
+  float2 gn = g[(frames_out - 1) * g_frame], on = o[(frames_out - 1) * bins];
+  for (int64_t t = frames_out - 1; t >= 0; --t) {
+    const float2 gt = gn, ot = on;
+    if (t > 0) {
+      gn = g[(t - 1) * g_frame];
+      on = o[(t - 1) * bins];
+    }
+    const VocoderStep st = vocoder_step(rate, t);
+    while (top > st.i1) {  // no step t' <= t reaches these frames any more
+      flush(top, m0, p0);
+      m0 = m1;
+      p0 = p1;
+      m1 = m2;
+      p1 = p2;
+      m2 = 0.0;
+      p2 = 0.0;
+      --top;
+    }
+    // torch's polar_backward on the result: a = Re(conj(g) i o), m = Re(conj(g) sgn(o))
+    const double a = (double)gt.y * ot.x - (double)gt.x * ot.y;
+    const double on2 = (double)ot.x * ot.x + (double)ot.y * ot.y;
+    const double m = on2 > 0.0 ? ((double)gt.x * ot.x + (double)gt.y * ot.y) / sqrt(on2) : 0.0;
+    const double al = (double)st.alpha;
+    // mag_t = alpha n(i1) + (1 - alpha) n(i0); psi_t (which reaches phi_u for u > t, so it sees S_{t+1}) adds
+    // angle(i1) - angle(i0)
+    add(st.i1, al * m, S);
+    add(st.i0, (1.0 - al) * m, -S);
+    S += a;
+  }
+  p0 += top == 0 ? S : 0.0;  // phi_0 = angle(X_0): frame 0 gets S_0
+  p1 += top == 1 ? S : 0.0;
+  while (top >= 0) {
+    flush(top, m0, p0);
+    m0 = m1;
+    p0 = p1;
+    m1 = m2;
+    p1 = p2;
+    m2 = 0.0;
+    p2 = 0.0;
+    --top;
+  }
+}
+
+int phase_vocoder_backward_impl(const float* spec, int64_t s_row, int64_t s_bin, int64_t s_frame, int64_t rows,
+                                int64_t bins, int64_t frames_in, double rate, const float* out, const float* grad,
+                                int64_t g_row, int64_t g_bin, int64_t g_frame, float* grad_spec, int64_t frames_out,
+                                cudaStream_t stream) {
+  if (rows > 65535) return B200A_EUNSUPPORTED;
+  phase_vocoder_backward_kernel<<<dim3((unsigned)((bins + 127) / 128), (unsigned)rows), 128, 0, stream>>>(
+      reinterpret_cast<const float2*>(spec), s_row, s_bin, s_frame, bins, frames_in, rate,
+      reinterpret_cast<const float2*>(out), reinterpret_cast<const float2*>(grad), g_row, g_bin, g_frame,
+      reinterpret_cast<float2*>(grad_spec), frames_out);
   return launch_status();
 }
 

@@ -12,7 +12,8 @@ gradient of ``spectrogram`` (and of the MelSpectrogram path) inside ``audio_b200
 gradient of ``inverse_spectrogram`` inside ``audio_b200.differentiable(inverse=True)``, the waveform gradient of
 ``resample`` / ``speed`` inside ``audio_b200.differentiable(resample=True)``, and the input gradients of
 ``amplitude_to_DB``, ``spectral_centroid`` and the MFCC / LFCC / MelScale paths inside
-``audio_b200.differentiable(features=True)``.
+``audio_b200.differentiable(features=True)``, and the spectrogram gradient of ``phase_vocoder`` and the waveform
+gradient of ``pitch_shift`` inside ``audio_b200.differentiable(vocoder=True)``.  ``griffinlim`` is forward-only.
 """
 from __future__ import annotations
 
@@ -30,7 +31,8 @@ from . import _lib, _ops
 from ._bookkeeping import resample_ratio
 from ._constants import create_dct, linear_fbanks, melscale_fbanks, sinc_resample_kernel
 from ._plans import (FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad,
-                     is_feature_differentiable, is_inverse_differentiable, new_group_max)
+                     is_feature_differentiable, is_inverse_differentiable, is_vocoder_differentiable, new_group_max,
+                     vocoder_chain)
 
 __all__ = [
     "spectrogram",
@@ -327,25 +329,56 @@ def phase_vocoder(complex_specgrams: Tensor, rate: float, phase_advance: Tensor)
         )
     if complex_specgrams.dtype != torch.complex64:
         raise TypeError(f"audio_b200: complex_specgrams must be complex64 (got {complex_specgrams.dtype})")
-    _no_autograd(complex_specgrams)
+    grad = _wants_grad(complex_specgrams, (("phase_advance", phase_advance),), is_vocoder_differentiable, "spectrogram")
+    if not grad:
+        _no_autograd(complex_specgrams)
     _require_cuda_f32(phase_advance, "phase_advance")
     shape = complex_specgrams.size()
     n_bins, frames = shape[-2], shape[-1]
     spec3 = complex_specgrams.reshape(-1, n_bins, frames)
-    rows = spec3.shape[0]
     pa = phase_advance.reshape(-1).contiguous()
     if pa.numel() != n_bins:
         raise RuntimeError(f"phase_advance must have one entry per frequency bin ({n_bins}), got {pa.numel()}")
+    if grad:
+        res = _PhaseVocoderFunction.apply(spec3, float(rate), pa)
+    else:
+        res = _phase_vocoder_run(spec3, rate, pa)[1]
+    return res.reshape(shape[:-2] + res.shape[1:])
+
+
+def _phase_vocoder_run(spec3: Tensor, rate: float, pa: Tensor):
+    """b200a_phase_vocoder on the packed (rows, bins, frames) spectrogram: the (rows, frames_out, bins, 2) frame-major
+    buffer and the logical (rows, bins, frames_out) complex view of it."""
+    rows, n_bins, frames = spec3.shape
     frames_out = int(math.ceil(frames / rate))  # len(torch.arange(0, frames, rate))
-    dev = complex_specgrams.device
+    dev = spec3.device
     with torch.cuda.device(dev):
         out = torch.empty((rows, frames_out, n_bins, 2), dtype=torch.float32, device=dev)
         rc = _lib.lib().b200a_phase_vocoder(
             torch.view_as_real(spec3).data_ptr(), spec3.stride(0), spec3.stride(1), spec3.stride(2), rows, n_bins, frames,
             float(rate), pa.data_ptr(), out.data_ptr(), frames_out, _stream_ptr(dev))
     _lib.check(rc, "phase_vocoder")
-    res = torch.view_as_complex(out).transpose(-1, -2)  # logical (rows, freq, frames_out) over the frame-major buffer
-    return res.reshape(shape[:-2] + res.shape[1:])
+    return out, torch.view_as_complex(out).transpose(-1, -2)  # logical (rows, freq, frames_out) over the buffer
+
+
+class _PhaseVocoderFunction(torch.autograd.Function):
+    """_phase_vocoder_run with b200audio::phase_vocoder_backward as its backward.  The backward needs the forward's input
+    and output and nothing else (no angles, no phase_advance, no recompute); both go through save_for_backward, so an
+    in-place edit of either before backward is an error."""
+
+    @staticmethod
+    def forward(ctx, spec3, rate, pa):
+        out, res = _phase_vocoder_run(spec3, rate, pa)
+        ctx.save_for_backward(spec3, out)
+        ctx.rate = rate
+        return res
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        spec3, out = ctx.saved_tensors
+        gx = _ops.phase_vocoder_backward(spec3, out, g, ctx.rate)  # (rows, frames_in, bins, 2)
+        return torch.view_as_complex(gx).transpose(1, 2), None, None
 
 
 def pitch_shift(
@@ -360,7 +393,8 @@ def pitch_shift(
 ) -> Tensor:
     """Shift the pitch of a waveform by ``n_steps`` steps (reference functional.py:1579-1719): STFT -> phase vocoder
     (rate 2^(-n_steps / bins_per_octave)) -> inverse STFT -> resample back to the original duration -> crop / zero-pad
-    to the input length.  Five kernels of this library, no host round trip."""
+    to the input length.  Five kernels of this library, no host round trip.  Inside
+    ``audio_b200.differentiable(vocoder=True)`` the waveform gradient runs their five adjoints."""
     _require_cuda_f32(waveform, "waveform")
     if hop_length is None:
         hop_length = n_fft // 4
@@ -368,6 +402,11 @@ def pitch_shift(
         win_length = n_fft
     if window is None:
         window = torch.hann_window(window_length=win_length, device=waveform.device)
+    with vocoder_chain(waveform):
+        return _pitch_shift(waveform, sample_rate, n_steps, bins_per_octave, n_fft, win_length, hop_length, window)
+
+
+def _pitch_shift(waveform, sample_rate, n_steps, bins_per_octave, n_fft, win_length, hop_length, window) -> Tensor:
     shape = waveform.size()
     flat = waveform.reshape(-1, shape[-1])
     ori_len = shape[-1]

@@ -12,8 +12,9 @@ spectrum through HBM) -- they read the sub-modules' buffers and launch the fused
 
 Gradients are opt-in, per thread: Spectrogram and MelSpectrogram inside ``audio_b200.differentiable()``,
 InverseSpectrogram with ``inverse=True``, Resample / Speed / SpeedPerturbation with ``resample=True``, and MFCC,
-LFCC, AmplitudeToDB, MelScale and SpectralCentroid with ``features=True``, and the Kaldi features
-(``audio_b200.compliance.kaldi``) with ``kaldi=True``.  GriffinLim, TimeStretch and PitchShift are forward-only.
+LFCC, AmplitudeToDB, MelScale and SpectralCentroid with ``features=True``, the Kaldi features
+(``audio_b200.compliance.kaldi``) with ``kaldi=True``, and TimeStretch (spectrogram gradient) and PitchShift
+(waveform gradient) with ``vocoder=True``.  GriffinLim is forward-only.
 """
 from __future__ import annotations
 
@@ -26,7 +27,7 @@ from torch import Tensor
 
 from . import _lib
 from . import functional as F
-from ._plans import FrontendPlan, ResamplePlan
+from ._plans import FrontendPlan, ResamplePlan, vocoder_chain
 
 __all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "MelSpectrogram", "MFCC", "LFCC", "SpectralCentroid", "Resample",
            "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift"]
@@ -609,6 +610,10 @@ class PitchShift(torch.nn.Module):
         super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs)
 
     def forward(self, waveform: Tensor) -> Tensor:
+        with vocoder_chain(waveform):
+            return self._shift(waveform)
+
+    def _shift(self, waveform: Tensor) -> Tensor:
         shape = waveform.size()
         flat = waveform.reshape(-1, shape[-1])
         ori_len = shape[-1]

@@ -326,6 +326,27 @@ int b200a_griffinlim_update(const float* mag, int64_t stride_row, int64_t stride
 int b200a_phase_vocoder(const float* spec, int64_t stride_row, int64_t stride_bin, int64_t stride_frame, int64_t rows,
                         int64_t bins, int64_t frames_in, double rate, const float* phase_advance, float* out,
                         int64_t frames_out, b200a_stream stream);
+/*
+ * Spectrogram gradient of b200a_phase_vocoder: grad_spec = dL/dRe X + i dL/dIm X for the upstream gradient g of `out`,
+ * torch's complex autograd convention.  With the forward's time grid (i0(t), i1(t), alpha_t) and o_t its output:
+ *   a_t = Im g_t Re o_t - Re g_t Im o_t              (dL/dphi_t)
+ *   m_t = Re(conj(g_t) sgn(o_t)), sgn(0) = 0         (dL/dmag_t)
+ *   S_t = sum_{u >= t} a_u,  S_{frames_out} = 0      (adjoint of the phase cumsum; the last phase step is dropped)
+ *   M_i = sum_{i0(t)=i} (1 - alpha_t) m_t + sum_{i1(t)=i} alpha_t m_t
+ *   P_i = sum_{i1(t)=i} S_{t+1} - sum_{i0(t)=i} S_{t+1} + [i = 0] S_0
+ *   grad_spec[i] = sgn(X_i) M_i + (i X_i / |X_i|^2) P_i,  exactly 0 at X_i = 0 (no NaN)
+ * The phase wrap and phase_advance have zero gradient; contributions to the two zero pad frames are dropped, and frames
+ * no step touches (rate > 2) get 0.
+ *   spec      : the forward's input, logical [rows][bins][frames_in], strides in complex elements
+ *   out       : the forward's output, complex64 frame-major [rows][frames_out][bins]
+ *   grad      : logical [rows][bins][frames_out], strides in complex elements (0 allowed: expanded gradients)
+ *   grad_spec : complex64 frame-major [rows][frames_in][bins] (every element written)
+ * Deterministic: no atomics, every element written once by the thread of its (row, bin).  rows <= 65535.
+ */
+int b200a_phase_vocoder_backward(const float* spec, int64_t stride_row, int64_t stride_bin, int64_t stride_frame,
+                                 int64_t rows, int64_t bins, int64_t frames_in, double rate, const float* out,
+                                 const float* grad, int64_t g_stride_row, int64_t g_stride_bin, int64_t g_stride_frame,
+                                 float* grad_spec, int64_t frames_out, b200a_stream stream);
 
 /* ---- Kaldi-compatible features (compliance/kaldi.py: spectrogram :229-316, fbank :514-645, mfcc :669-813) -------- */
 /*

@@ -64,5 +64,9 @@ T.GriffinLim(n_fft=512, hop_length=128, n_iter=3, length=12000, rand_init=False)
     T.Spectrogram(n_fft=512, hop_length=128).cuda()(x))
 T.PitchShift(16000, 12).cuda()(x)
 T.TimeStretch(hop_length=128, n_freq=257, fixed_rate=1.3).cuda()(T.Spectrogram(n_fft=512, hop_length=128, power=None).cuda()(x))
+with audio_b200.differentiable(vocoder=True):  # phase-vocoder adjoint: TimeStretch alone, then the whole PitchShift chain
+    spec = T.Spectrogram(n_fft=512, hop_length=128, power=None).cuda()(x).requires_grad_()
+    T.TimeStretch(hop_length=128, n_freq=257, fixed_rate=0.8).cuda()(spec).abs().sum().backward()
+    T.PitchShift(16000, -3).cuda()(x.clone().requires_grad_()).sum().backward()
 torch.cuda.synchronize()
 print("done")
