@@ -89,6 +89,15 @@ _SIGNATURES = {
          c_void_p, c_void_p, c_int64, c_void_p],
     ),
     "b200a_frontend_backward_scratch_bytes": (c_size_t, [POINTER(FrontendDesc), c_int32, c_int64, c_int64]),
+    "b200a_rnnt_features_run": (
+        ctypes.c_int,
+        [POINTER(FrontendDesc), c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_float, c_int64,
+         c_void_p, c_void_p, c_void_p],
+    ),
+    "b200a_rnnt_features_backward": (
+        ctypes.c_int,
+        [c_void_p, c_float, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int32, c_void_p, c_void_p],
+    ),
     "b200a_mfcc_finish": (
         ctypes.c_int,
         [POINTER(FrontendDesc), c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float, c_void_p, c_void_p],

@@ -1,7 +1,8 @@
 """``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
-``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward``.
+``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward`` / ``rnnt_features`` /
+``rnnt_features_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -67,6 +68,11 @@ _LIB.define(
 _LIB.define(
     "phase_vocoder_backward(Tensor spec, Tensor out, Tensor grad, float rate) -> Tensor"
 )
+_LIB.define(
+    "rnnt_features(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? lengths, Tensor stats, float gain, "
+    "int out_frames, int pad_frames, int row_stride, bool with_mel) -> (Tensor, Tensor)"
+)
+_LIB.define("rnnt_features_backward(Tensor stats, float gain, Tensor mel, Tensor grad) -> Tensor")
 
 _KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
                "out_width", "out_col0", "use_log")
@@ -394,6 +400,63 @@ def _phase_vocoder_backward_meta(spec, out, grad, rate):
     return spec.new_empty((spec.shape[0], spec.shape[2], spec.shape[1], 2), dtype=torch.float32)
 
 
+# ---- rnnt_features / rnnt_features_backward ----------------------------------------------------------------------
+def _rnnt_shapes(wave, desc_i, out_frames, pad_frames):
+    n_mels = int(desc_i[DESC_N_MELS])
+    return (wave.shape[0], out_frames + pad_frames, n_mels), (wave.shape[0], out_frames, n_mels)
+
+
+def _rnnt_features_cuda(wave, workspace, desc_i, desc_f, lengths, stats, gain, out_frames, pad_frames, row_stride, with_mel):
+    """(rows, L) waveform -> ((rows, out_frames + pad_frames, n_mels) features, (rows, out_frames, n_mels) mel values
+    or an empty tensor).  ``pad_frames`` zero rows after the features (one row only) are written by b200a_fill_f32."""
+    d = _unpack_desc(desc_i, desc_f)
+    rows, length = wave.shape
+    if pad_frames > 0 and rows != 1:
+        raise RuntimeError("audio_b200: rnnt_features pads a single row only")
+    out_shape, mel_shape = _rnnt_shapes(wave, desc_i, out_frames, pad_frames)
+    dev = wave.device
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        out = torch.empty(out_shape, dtype=torch.float32, device=dev)
+        mel = torch.empty(mel_shape if with_mel else (0,), dtype=torch.float32, device=dev)
+        rc = lib.b200a_rnnt_features_run(
+            d, workspace.data_ptr(), wave.data_ptr(), rows, length, row_stride,
+            None if lengths is None else lengths.data_ptr(), stats.data_ptr(), float(gain), out_frames, out.data_ptr(),
+            mel.data_ptr() if with_mel else None, _stream(dev))
+        if rc == _lib.OK and pad_frames > 0:
+            n = pad_frames * d.n_mels
+            rc = lib.b200a_fill_f32(out.data_ptr() + 4 * out_frames * d.n_mels, n, 0.0, _stream(dev))
+    if rc == _lib.ESHORT:
+        raise RuntimeError(
+            f"audio_b200: padding size n_fft//2={d.n_fft // 2} should be less than the input length "
+            f"{length + 2 * d.pad} for pad_mode reflect/circular (torch.stft raises the same way)")
+    _lib.check(rc, "rnnt_features")
+    return out, mel
+
+
+def _rnnt_features_meta(wave, workspace, desc_i, desc_f, lengths, stats, gain, out_frames, pad_frames, row_stride, with_mel):
+    out_shape, mel_shape = _rnnt_shapes(wave, desc_i, out_frames, pad_frames)
+    return wave.new_empty(out_shape, dtype=torch.float32), wave.new_empty(mel_shape if with_mel else (0,),
+                                                                           dtype=torch.float32)
+
+
+def _rnnt_features_backward_cuda(stats, gain, mel, grad):
+    """(rows, T, n_mels) feature gradient at any element strides (0 included) -> (rows, T, n_mels) mel gradient."""
+    rows, frames, n_mels = mel.shape
+    dev = mel.device
+    gs = grad.stride()
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, n_mels), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_rnnt_features_backward(stats.data_ptr(), float(gain), mel.data_ptr(), grad.data_ptr(), gs[0],
+                                                     gs[1], gs[2], rows, frames, n_mels, out.data_ptr(), _stream(dev))
+    _lib.check(rc, "rnnt_features_backward")
+    return out
+
+
+def _rnnt_features_backward_meta(stats, gain, mel, grad):
+    return mel.new_empty(mel.shape)
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
@@ -406,7 +469,9 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("resample_backward", _resample_backward_cuda, _resample_backward_meta),
                             ("kaldi_run", _kaldi_run_cuda, _kaldi_run_meta),
                             ("kaldi_backward", _kaldi_backward_cuda, _kaldi_backward_meta),
-                            ("phase_vocoder_backward", _phase_vocoder_backward_cuda, _phase_vocoder_backward_meta)):
+                            ("phase_vocoder_backward", _phase_vocoder_backward_cuda, _phase_vocoder_backward_meta),
+                            ("rnnt_features", _rnnt_features_cuda, _rnnt_features_meta),
+                            ("rnnt_features_backward", _rnnt_features_backward_cuda, _rnnt_features_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -423,3 +488,5 @@ resample_backward = torch.ops.b200audio.resample_backward
 kaldi_run = torch.ops.b200audio.kaldi_run
 kaldi_backward = torch.ops.b200audio.kaldi_backward
 phase_vocoder_backward = torch.ops.b200audio.phase_vocoder_backward
+rnnt_features = torch.ops.b200audio.rnnt_features
+rnnt_features_backward = torch.ops.b200audio.rnnt_features_backward

@@ -48,8 +48,8 @@ def is_resample_differentiable() -> bool:
 
 
 def is_feature_differentiable() -> bool:
-    """Whether MFCC, LFCC, AmplitudeToDB, MelScale and SpectralCentroid accept inputs that require grad (in this
-    thread)."""
+    """Whether MFCC, LFCC, AmplitudeToDB, MelScale, SpectralCentroid and pipelines.RNNTFeatureExtractor accept inputs
+    that require grad (in this thread)."""
     return getattr(_GRAD_STATE, "features", False)
 
 
@@ -70,7 +70,7 @@ def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = Fa
     """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
     ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT, ``resample=True``
     (with ``mode``) the waveform gradients of the resampler, ``features=True`` (with ``mode``) the input gradients of
-    MFCC, LFCC, AmplitudeToDB, MelScale and SpectralCentroid, ``kaldi=True`` (with ``mode``) the waveform gradients of
+    MFCC, LFCC, AmplitudeToDB, MelScale, SpectralCentroid and the RNN-T feature extractor, ``kaldi=True`` (with ``mode``) the waveform gradients of
     the Kaldi spectrogram, fbank and mfcc, ``vocoder=True`` (with ``mode``) the spectrogram gradients of the phase
     vocoder and TimeStretch and the waveform gradients of PitchShift.  They are separate switches so that vocoder
     inference, augmentation code (Speed, SpeedPerturbation, TimeStretch, PitchShift) and Kaldi feature preprocessing in
@@ -129,7 +129,7 @@ def _no_autograd(t: torch.Tensor) -> None:
             "waveform gradients inside audio_b200.differentiable(); InverseSpectrogram and F.inverse_spectrogram "
             "compute spectrogram gradients inside audio_b200.differentiable(inverse=True); Resample, F.resample, Speed "
             "and SpeedPerturbation compute waveform gradients inside audio_b200.differentiable(resample=True); MFCC, LFCC, "
-            "AmplitudeToDB, MelScale and SpectralCentroid compute input gradients inside "
+            "AmplitudeToDB, MelScale, SpectralCentroid and pipelines.RNNTFeatureExtractor compute input gradients inside "
             "audio_b200.differentiable(features=True); compliance.kaldi spectrogram, fbank and mfcc compute waveform "
             "gradients inside audio_b200.differentiable(kaldi=True); F.phase_vocoder and TimeStretch compute spectrogram "
             "gradients, F.pitch_shift and PitchShift waveform gradients, inside audio_b200.differentiable(vocoder=True).)"
@@ -198,6 +198,32 @@ class _MfccFunction(torch.autograd.Function):
         g_mel = _ops.mfcc_backward(grad_out, ctx.feat, mel, ctx.gmax, ctx.ws, desc_i, desc_f, rows_per_group, top_db)
         grad = _ops.frontend_backward(flat, ctx.ws, desc_i, desc_f, _lib.STAGE_MEL, stride, g_mel)
         return grad, None, None, None, None, None, None, None, None
+
+
+class _RNNTFunction(torch.autograd.Function):
+    """The RNN-T features of the packed (rows, L) waveform: the same b200audio::rnnt_features launch as the no-grad path
+    plus the mel values before the chain, so the features are bit-identical to it.  Saved: the waveform and the
+    statistics buffers ``mean`` / ``invstddev`` (save_for_backward: an in-place edit of either raises in backward), the
+    mel values, the packed statistics the forward read and its workspace.  Backward: the chain's VJP
+    (b200audio::rnnt_features_backward) on the first ``frames`` rows, then the mel-stage waveform gradient
+    (b200audio::frontend_backward)."""
+
+    @staticmethod
+    def forward(ctx, flat, ws, desc_i, desc_f, stats, mean, invstd, gain, frames, pad_frames, stride):
+        out, mel = _ops.rnnt_features(flat, ws, desc_i, desc_f, None, stats, gain, frames, pad_frames, stride, True)
+        ctx.save_for_backward(flat, mean, invstd)
+        ctx.mel, ctx.stats, ctx.ws = mel, stats, ws
+        ctx.args = desc_i, desc_f, gain, frames, stride
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        flat, _, _ = ctx.saved_tensors
+        desc_i, desc_f, gain, frames, stride = ctx.args
+        g_mel = _ops.rnnt_features_backward(ctx.stats, gain, ctx.mel, grad_out[:, :frames])
+        grad = _ops.frontend_backward(flat, ctx.ws, desc_i, desc_f, _lib.STAGE_MEL, stride, g_mel)
+        return grad, None, None, None, None, None, None, None, None, None, None
 
 
 def _version_of(t: torch.Tensor) -> int:

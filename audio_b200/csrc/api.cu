@@ -150,6 +150,34 @@ int b200a_frontend_backward(const b200a_frontend_desc* desc, const void* workspa
                                 static_cast<cudaStream_t>(stream));
 }
 
+int b200a_rnnt_features_run(const b200a_frontend_desc* desc, const void* workspace, const float* wave, int64_t rows,
+                            int64_t length, int64_t row_stride, const int64_t* lengths, const float* stats, float gain,
+                            int64_t out_frames, float* out, float* mel_out, b200a_stream stream) {
+  const int rc = validate_desc(desc);
+  if (rc != B200A_OK) return rc;
+  if (desc->n_mels <= 0 || !(desc->power > 0.f) || !std::isfinite(gain)) return B200A_EINVAL;
+  if (rows < 0 || length < 0 || out_frames < 0 || row_stride < length) return B200A_EINVAL;
+  if (rows == 0 || out_frames == 0) return B200A_OK;  // nothing to enqueue (pointers may be null)
+  if (workspace == nullptr || wave == nullptr || stats == nullptr || out == nullptr) return B200A_EINVAL;
+  if (lengths == nullptr) {  // one length for every row: torch.stft's padding rules hold for it
+    const int64_t frames = frontend_frames(desc, B200A_STAGE_MEL, rows, length);
+    if (frames < 1) return (int)frames;
+  }
+  return rnnt_features_impl(desc, workspace, wave, rows, length, row_stride, lengths, stats, gain, out_frames, out, mel_out,
+                            static_cast<cudaStream_t>(stream));
+}
+
+int b200a_rnnt_features_backward(const float* stats, float gain, const float* mel, const float* grad, int64_t g_stride_row,
+                                 int64_t g_stride_frame, int64_t g_stride_col, int64_t rows, int64_t frames, int32_t n_mels,
+                                 float* grad_mel, b200a_stream stream) {
+  if (rows < 0 || frames < 0 || n_mels < 1 || !std::isfinite(gain)) return B200A_EINVAL;
+  if (g_stride_row < 0 || g_stride_frame < 0 || g_stride_col < 0) return B200A_EINVAL;
+  if (rows == 0 || frames == 0) return B200A_OK;
+  if (stats == nullptr || mel == nullptr || grad == nullptr || grad_mel == nullptr) return B200A_EINVAL;
+  return rnnt_backward_impl(stats, gain, mel, grad, g_stride_row, g_stride_frame, g_stride_col, rows, frames, n_mels,
+                            grad_mel, static_cast<cudaStream_t>(stream));
+}
+
 int b200a_mfcc_finish(const b200a_frontend_desc* desc, const void* workspace, const float* feat, int64_t rows,
                       int64_t frames, const float* group_max, int64_t rows_per_group, float top_db, float* out,
                       b200a_stream stream) {

@@ -113,6 +113,13 @@ int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const floa
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);
 int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* feat, int64_t rows, int64_t frames,
                      const float* group_max, int64_t rows_per_group, float top_db, float* out, cudaStream_t stream);
+// The RNN-T feature chain in the epilogue of the Stockham kernel (every n_fft), per-row lengths, fill frames past T(L_r)
+int rnnt_features_impl(const b200a_frontend_desc* d, const void* ws, const float* wave, int64_t rows, int64_t length,
+                       int64_t row_stride, const int64_t* lengths, const float* stats, float gain, int64_t out_frames,
+                       float* out, float* mel_out, cudaStream_t stream);
+int rnnt_backward_impl(const float* stats, float gain, const float* mel, const float* grad, int64_t gs_row,
+                       int64_t gs_frame, int64_t gs_col, int64_t rows, int64_t frames, int n_mels, float* grad_mel,
+                       cudaStream_t stream);
 size_t kaldi_backward_scratch(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d, int stage, int64_t rows,
                               int64_t length, int64_t frames);
 int kaldi_backward_impl(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d, const void* ws, int stage,
@@ -256,6 +263,28 @@ __device__ __forceinline__ int2 filter_range(const int2* bands, int n_mels, int 
 // are exact.
 __device__ __forceinline__ float db_value(float x, float mult, float amin, float offset) {
   return mult * log10f(fmaxf(x, amin)) - offset;
+}
+
+// The RNN-T feature chain of one mel value m (pipelines/rnnt_pipeline.py:20-23, :43-44, :322-324):
+//   x = m * gain;  x[x > e] = log(x);  x[x <= e] /= e;  y = (x - mean) * invstddev
+// with the reference's two in-place statements taken literally: the second mask is read after the first write, so
+// there are three pieces -- x / e (x <= e), log(x) / e (e < x <= e^e) and log(x) (x > e^e) -- and a NaN stays NaN
+// (piece 0).  Returns y; `x` receives m * gain and `piece` the branch.  The forward epilogue, its fill frames and
+// rnnt_vjp_kernel all call this one expression, so the gradient's branch decisions are the forward's, bit for bit.
+constexpr float kRnntE = 2.71828182845904523536f;
+__device__ __forceinline__ float rnnt_value(float m, float gain, float mean, float invstd, float& x, int& piece) {
+  x = m * gain;
+  float y = x;
+  piece = 0;
+  if (x > kRnntE) {
+    y = logf(x);
+    piece = 3;
+  }
+  if (y <= kRnntE) {
+    y = y / kRnntE;
+    piece = piece == 3 ? 2 : 1;
+  }
+  return (y - mean) * invstd;
 }
 
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {

@@ -112,6 +112,12 @@ struct GenericParams {
   int kaldi, k_win, k_snip, k_dc, k_energy_mode, k_energy_col, k_log;
   int k_prelog;  // the gradient's recompute: the energy column receives E itself, not its floored log
   float k_preemph, k_energy_floor;
+  // RNN-T chain (stft_rnnt_kernel only): `frames` is the output frame count; row r holds T(L_r) frames of features,
+  // L_r = clamp(lengths[r], 0, length) (lengths may be null: L_r = length), and chain(0) after them
+  const int64_t* lengths;
+  const float* stats;  // [2][n_mels]: mean, invstddev
+  float* mel_out;      // null, or [rows][frames][n_mels]: the mel value before the chain (0 on fill frames)
+  float gain;
 };
 
 // Sample n of Kaldi frame t (kaldi.py:_get_strided).  snip_edges: frames lie inside the signal.  Otherwise the
@@ -238,7 +244,11 @@ __device__ __forceinline__ float spectral_power(float re, float im, float power)
   return powf(mag, power);
 }
 
-__global__ void __launch_bounds__(256) stft_generic_kernel(const GenericParams p) {
+// The body of stft_generic_kernel and, with kRnnt, of stft_rnnt_kernel: the RNN-T variant reads per-row lengths,
+// lets CTAs whose tile lies wholly past T(L_r) write fill frames without an FFT, and ends the mel projection with
+// rnnt_value.  A compile-time switch, so the other stages keep their code and register count.
+template <bool kRnnt>
+__device__ __forceinline__ void stft_generic_body(const GenericParams& p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int N = p.n_fft;
   const int pairs = p.pairs;
@@ -253,10 +263,34 @@ __global__ void __launch_bounds__(256) stft_generic_kernel(const GenericParams p
   const int64_t t0 = tile * (2 * pairs);
   const float* __restrict__ x = p.wave + row * p.row_stride;
   const int half = p.center ? N / 2 : 0;
+  // the samples this row may read, [0, length), and the frames that hold features, [0, valid)
+  int64_t length = p.length, valid = p.frames;
+  if constexpr (kRnnt) {
+    if (p.lengths != nullptr) {
+      const int64_t lr = p.lengths[row];
+      length = lr < 0 ? 0 : (lr < p.length ? lr : p.length);
+    }
+    const int64_t span = length + 2 * (int64_t)p.pad + 2 * (int64_t)half;  // b200a_num_frames
+    valid = span < N ? 0 : 1 + (span - N) / p.hop;
+    if (length == 0) valid = 0;  // no sample to read: every frame is a fill frame
+    if (valid > p.frames) valid = p.frames;
+    if (t0 >= valid) {  // fill frames only: chain(0), no FFT
+      const int64_t nf = min((int64_t)(2 * pairs), p.frames - t0);
+      for (int o = tid; o < nf * p.n_mels; o += nthr) {
+        const int f = o / p.n_mels, m = o - f * p.n_mels;
+        const int64_t at = (row * p.frames + t0 + f) * p.n_mels + m;
+        float xg;
+        int piece;
+        p.out[at] = rnnt_value(0.f, p.gain, __ldg(p.stats + m), __ldg(p.stats + p.n_mels + m), xg, piece);
+        if (p.mel_out != nullptr) p.mel_out[at] = 0.f;
+      }
+      return;
+    }
+  }
 
   for (int i = tid; i < N; i += nthr) tw[i] = p.twiddle[i];
 
-  if (p.kaldi) {
+  if (!kRnnt && p.kaldi) {
     // ---- Kaldi conditioning: raw frames -> (DC removal) -> [raw energy] -> pre-emphasis -> window -> [energy] ----
     float* raw = reinterpret_cast<float*>(buf1);   // [pair][n][2]
     float* cond = reinterpret_cast<float*>(buf0);  // same layout: z[n] = frame_a[n] + i frame_b[n]
@@ -317,12 +351,12 @@ __global__ void __launch_bounds__(256) stft_generic_kernel(const GenericParams p
     const int64_t ta = t0 + 2 * pr, tb = ta + 1;
     const float w = p.window[n];
     float a = 0.f, b = 0.f;
-    if (ta < p.frames) {
-      const int64_t s = source_index(ta * p.hop + n, p.length, p.pad, half, p.pad_mode);
+    if (ta < valid) {
+      const int64_t s = source_index(ta * p.hop + n, length, p.pad, half, p.pad_mode);
       if (s >= 0) a = x[s] * w;
     }
-    if (tb < p.frames) {
-      const int64_t s = source_index(tb * p.hop + n, p.length, p.pad, half, p.pad_mode);
+    if (tb < valid) {
+      const int64_t s = source_index(tb * p.hop + n, length, p.pad, half, p.pad_mode);
       if (s >= 0) b = x[s] * w;
     }
     buf0[o] = make_float2(a, b);
@@ -383,6 +417,14 @@ __global__ void __launch_bounds__(256) stft_generic_kernel(const GenericParams p
       const int2 band = p.bands[m];
       float acc = 0.f;
       for (int k = band.x; k < band.y; ++k) acc = fmaf(pw[k], p.fb[(size_t)k * p.n_mels + m], acc);
+      if constexpr (kRnnt) {  // the RNN-T chain; frames past T(L_r) are fill frames, chain(0)
+        const float mv = t < valid ? acc : 0.f;
+        if (p.mel_out != nullptr) p.mel_out[(row * p.frames + t) * p.n_mels + m] = mv;
+        float xg;
+        int piece;
+        orow[m] = rnnt_value(mv, p.gain, __ldg(p.stats + m), __ldg(p.stats + p.n_mels + m), xg, piece);
+        continue;
+      }
       if (p.stage == B200A_STAGE_FEAT) {
         acc = p.log_mels ? logf(acc + 1e-6f) : p.db_mult * log10f(fmaxf(acc, p.db_amin)) - p.db_offset;
         local_max = fmaxf(local_max, acc);
@@ -391,11 +433,14 @@ __global__ void __launch_bounds__(256) stft_generic_kernel(const GenericParams p
       orow[m] = acc;
     }
   }
-  if (p.stage == B200A_STAGE_FEAT && p.group_max != nullptr) {
+  if (!kRnnt && p.stage == B200A_STAGE_FEAT && p.group_max != nullptr) {
     local_max = warp_max(local_max);
     if (lane == 0 && local_max > -CUDART_INF_F) atomic_max_f32(p.group_max + row / p.rows_per_group, local_max);
   }
 }
+
+__global__ void __launch_bounds__(256) stft_generic_kernel(const GenericParams p) { stft_generic_body<false>(p); }
+__global__ void __launch_bounds__(256) stft_rnnt_kernel(const GenericParams p) { stft_generic_body<true>(p); }
 
 // ------------------------------------------------------------------------------------------
 // MFCC second stage: clamp at (group max - top_db), multiply by the DCT matrix
@@ -744,6 +789,75 @@ static int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, in
     p.out_col0 = kd->out_col0;
   }
   return launch_stockham(stft_generic_kernel, p, rows, frames, stream);
+}
+
+// The RNN-T features: the Stockham kernel for every n_fft (powers of two included), MEL stage, chain epilogue.
+int rnnt_features_impl(const b200a_frontend_desc* d, const void* ws, const float* wave, int64_t rows, int64_t length,
+                       int64_t row_stride, const int64_t* lengths, const float* stats, float gain, int64_t out_frames,
+                       float* out, float* mel_out, cudaStream_t stream) {
+  const WsLayout l = ws_layout(*d);
+  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  GenericParams p{};
+  p.n_stages = factorize(d->n_fft, p.radix);
+  if (p.n_stages < 0) return B200A_EUNSUPPORTED;
+  p.wave = wave;
+  p.length = length;
+  p.row_stride = row_stride;
+  p.frames = out_frames;
+  p.out = out;
+  p.rows_per_group = 1;
+  p.window = reinterpret_cast<const float*>(base + l.window);
+  p.twiddle = reinterpret_cast<const float2*>(base + l.twiddle);
+  p.bands = reinterpret_cast<const int2*>(base + l.bands);
+  p.fb = reinterpret_cast<const float*>(base + l.fb);
+  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.n_fft = d->n_fft;
+  p.hop = d->hop;
+  p.pad = d->pad;
+  p.center = d->center;
+  p.pad_mode = d->pad_mode;
+  p.n_bins = d->n_fft / 2 + 1;
+  p.n_mels = d->n_mels;
+  p.stage = B200A_STAGE_MEL;
+  p.power = d->power;
+  p.out_width = d->n_mels;
+  p.k_energy_col = -1;
+  p.lengths = lengths;
+  p.stats = stats;
+  p.mel_out = mel_out;
+  p.gain = gain;
+  return launch_stockham(stft_rnnt_kernel, p, rows, out_frames, stream);
+}
+
+// Elementwise VJP of the chain in torch's order: g * invstd, / e on pieces 1-2, / x on pieces 2-3, * gain.  The piece
+// and x come from rnnt_value on the forward's mel values, so the decisions are the forward's.
+__global__ void __launch_bounds__(256) rnnt_vjp_kernel(const float* __restrict__ stats, float gain,
+                                                       const float* __restrict__ mel, const float* __restrict__ grad,
+                                                       int64_t gs_row, int64_t gs_frame, int64_t gs_col, int64_t frames,
+                                                       int n_mels, int64_t total, float* __restrict__ grad_mel) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t f = i / n_mels, row = f / frames, t = f - row * frames;
+    const int m = (int)(i - f * n_mels);
+    const float invstd = __ldg(stats + n_mels + m);
+    float x;
+    int piece;
+    rnnt_value(mel[i], gain, __ldg(stats + m), invstd, x, piece);
+    float g = grad[row * gs_row + t * gs_frame + m * gs_col] * invstd;
+    if (piece == 1 || piece == 2) g = g / kRnntE;
+    if (piece >= 2) g = g / x;
+    grad_mel[i] = g * gain;
+  }
+}
+
+int rnnt_backward_impl(const float* stats, float gain, const float* mel, const float* grad, int64_t gs_row,
+                       int64_t gs_frame, int64_t gs_col, int64_t rows, int64_t frames, int n_mels, float* grad_mel,
+                       cudaStream_t stream) {
+  const int64_t total = rows * frames * n_mels;
+  const int64_t grid = sm_capped_grid((total + 255) / 256, 8);
+  if (grid < 0) return B200A_ECUDA;
+  rnnt_vjp_kernel<<<(unsigned)grid, 256, 0, stream>>>(stats, gain, mel, grad, gs_row, gs_frame, gs_col, frames, n_mels,
+                                                      total, grad_mel);
+  return launch_status();
 }
 
 int frontend_run_impl(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,

@@ -171,6 +171,40 @@ int b200a_mfcc_finish(const b200a_frontend_desc* desc, const void* workspace, co
                       int64_t rows, int64_t frames, const float* group_max, int64_t rows_per_group,
                       float top_db, float* out, b200a_stream stream);
 
+/* ---- RNN-T feature chain (pipelines/rnnt_pipeline.py:20-47, :310-343) ------------------------- */
+/*
+ * MelSpectrogram -> x = m * gain -> piecewise log -> (x - mean) * invstddev in one launch, with the workspace
+ * b200a_frontend_prepare built for a MEL descriptor (window and filterbank).  The piecewise log is the reference's two
+ * in-place statements, so it has three pieces, decided in float32:
+ *   y = x / e (x <= e),  log(x) / e (e < x, log(x) <= e),  log(x) (log(x) > e);  a NaN stays NaN.
+ * Row r has L_r = clamp(lengths[r], 0, length) samples (lengths NULL: L_r = length for every row) and
+ * T(L_r) = b200a_num_frames(L_r, ...) frames of features; frames T(L_r) <= t < out_frames get chain(0) =
+ * (0 - mean) * invstddev, the features of zero mel values (the recipes pad the mel batch with zeros).  The kernel never
+ * reads outside [0, L_r) of row r.  With lengths, torch.stft's per-row rules (reflect needs L_r > n_fft/2) are the
+ * caller's to check; without, they are checked here as in b200a_frontend_run (B200A_ESHORT).
+ *   lengths  : NULL, or a DEVICE array of rows int64 lengths
+ *   stats    : [2][n_mels]: mean, then invstddev
+ *   gain     : the float32 multiplier (the reference's 32767^2 rounds to 1073676288)
+ *   out      : [rows][out_frames][n_mels], every element written
+ *   mel_out  : NULL, or [rows][out_frames][n_mels]: m before the chain (0 on fill frames), for the gradient
+ * Every n_fft, powers of two included, runs the shared-memory Stockham kernel.  Bit-identical reruns; a row's output
+ * does not depend on the other rows or on out_frames.
+ */
+int b200a_rnnt_features_run(const b200a_frontend_desc* desc, const void* workspace, const float* wave, int64_t rows,
+                            int64_t length, int64_t row_stride, const int64_t* lengths, const float* stats, float gain,
+                            int64_t out_frames, float* out, float* mel_out, b200a_stream stream);
+/*
+ * Mel gradient of the chain, elementwise, in torch's order: g * invstddev, then / e on the first two pieces, then / x
+ * on the last two, then * gain (a NaN's piece passes g * invstddev * gain).  The pieces are decided from `mel` by the
+ * forward's own expression.
+ *   mel      : [rows][frames][n_mels], the forward's mel_out
+ *   grad     : [rows][frames][n_mels] at element strides (0 allowed: expanded gradients)
+ *   grad_mel : [rows][frames][n_mels], every element written; feed it to b200a_frontend_backward(B200A_STAGE_MEL)
+ */
+int b200a_rnnt_features_backward(const float* stats, float gain, const float* mel, const float* grad, int64_t g_stride_row,
+                                 int64_t g_stride_frame, int64_t g_stride_col, int64_t rows, int64_t frames, int32_t n_mels,
+                                 float* grad_mel, b200a_stream stream);
+
 /* ---- stand-alone stages (MelScale / AmplitudeToDB modules used on their own) ---------------- */
 /*
  * out[r][t][m] = sum_k spec[r][k][t] * fb[k][m] for a spectrogram given in the reference's LOGICAL
