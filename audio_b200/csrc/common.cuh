@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <math_constants.h>
 #include <stdint.h>
+#include <type_traits>
 
 #include "../../include/b200audio.h"
 
@@ -51,6 +52,51 @@ inline WsLayout ws_layout(const b200a_frontend_desc& d) {
   off = align_up(off + sizeof(float) * (size_t)(d.n_mels > 0 ? d.n_mels : 0) * (d.n_mfcc > 0 ? d.n_mfcc : 0), 256);
   l.total = off;
   return l;
+}
+
+// A T* into a workspace, const when the workspace pointer W* is: prepare functions write their tables through a view
+// made from `void*`, launchers read them through one made from `const void*`.
+template <typename W, typename T>
+using WsPtr = std::conditional_t<std::is_const<W>::value, const T, T>*;
+
+template <typename T, typename W>
+WsPtr<W, T> ws_at(W* ws, size_t off) {
+  return reinterpret_cast<WsPtr<W, T>>(static_cast<WsPtr<W, unsigned char>>(ws) + off);
+}
+
+// The tables of a front-end workspace (WsLayout).
+template <typename W>
+struct FrontendWs {
+  WsPtr<W, WsHeader> header;
+  WsPtr<W, float> window;
+  WsPtr<W, float2> twiddle;
+  WsPtr<W, int2> bands;
+  WsPtr<W, float> fb, dct;
+};
+
+template <typename W>
+FrontendWs<W> frontend_ws(const b200a_frontend_desc& d, W* ws) {
+  const WsLayout l = ws_layout(d);
+  return {ws_at<WsHeader>(ws, l.header), ws_at<float>(ws, l.window), ws_at<float2>(ws, l.twiddle),
+          ws_at<int2>(ws, l.bands),      ws_at<float>(ws, l.fb),     ws_at<float>(ws, l.dct)};
+}
+
+// Samples Kaldi frame t starts before t * window_shift: 0 with snip_edges, else win/2 - shift/2 (kaldi.py:_get_strided)
+inline int kaldi_lead(const b200a_kaldi_desc& kd) { return kd.snip_edges ? 0 : kd.window_size / 2 - kd.window_shift / 2; }
+
+// The Kaldi fields GenericParams and Pow2Params share; output = false (the gradient writes no feature rows) skips the
+// energy column and output row geometry.  Energy mode, k_log / k_prelog, pad mode and lead (k_snip / k_off): the caller's.
+template <typename Params>
+void fill_kaldi(Params& p, const b200a_kaldi_desc& kd, bool output) {
+  p.kaldi = 1;
+  p.k_win = kd.window_size;
+  p.k_dc = kd.remove_dc_offset;
+  p.k_preemph = kd.preemphasis;
+  if (!output) return;
+  p.k_energy_floor = kd.energy_floor;
+  p.k_energy_col = kd.energy_col;
+  p.out_width = kd.out_width;
+  p.out_col0 = kd.out_col0;
 }
 
 constexpr int kSmemLimit = 227 * 1024;  // dynamic shared memory per CTA on sm_90
@@ -137,14 +183,12 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
 int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
                       int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, cudaStream_t stream);
 bool backward_fused_applicable(const b200a_frontend_desc* d, int stage);
+bool kaldi_backward_fused_applicable(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, int stage, int64_t length);
+// kd: the Kaldi gradient, or null; taken only where backward_fused_applicable / kaldi_backward_fused_applicable hold.
 int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
                            int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
-                           int64_t gs_frame, int64_t gs_col, float* frame_buf, cudaStream_t stream);
-bool kaldi_backward_fused_applicable(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, int stage, int64_t length);
-int kaldi_backward_pow2(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, const void* ws, int stage,
-                        const float* wave, int64_t rows, int64_t length, int64_t row_stride, int64_t frames,
-                        const float* grad, int64_t gs_row, int64_t gs_frame, int64_t gs_col, float* frame_buf,
-                        cudaStream_t stream);
+                           int64_t gs_frame, int64_t gs_col, float* frame_buf, cudaStream_t stream,
+                           const b200a_kaldi_desc* kd);
 bool istft_backward_fused_applicable(const b200a_frontend_desc* d, int64_t frames);
 int istft_backward_pow2(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, float* grad_spec, cudaStream_t stream);

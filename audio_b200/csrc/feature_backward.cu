@@ -267,7 +267,7 @@ int mfcc_backward_impl(const b200a_frontend_desc* d, const void* ws, const float
   p.gs_row = gs_row;
   p.gs_frame = gs_frame;
   p.gs_col = gs_col;
-  p.dct = reinterpret_cast<const float*>(static_cast<const unsigned char*>(ws) + ws_layout(*d).dct);
+  p.dct = frontend_ws(*d, ws).dct;
   p.n = d->n_mels;
   p.n_c = d->n_mfcc;
   p.frames = frames;

@@ -698,23 +698,16 @@ int frontend_prepare_impl(const b200a_frontend_desc* d, const float* window, con
   if (window == nullptr || ws == nullptr) return B200A_EINVAL;
   if (d->n_mels > 0 && fb == nullptr) return B200A_EINVAL;
   if (d->n_mfcc > 0 && dct == nullptr) return B200A_EINVAL;
-  const WsLayout l = ws_layout(*d);
-  if (ws_bytes < l.total) return B200A_EWORKSPACE;
-  unsigned char* base = static_cast<unsigned char*>(ws);
+  if (ws_bytes < ws_layout(*d).total) return B200A_EWORKSPACE;  // pow2_prepare checks the tables after these
+  const FrontendWs<void> t = frontend_ws(*d, ws);
   const int n_bins = d->onesided ? d->n_fft / 2 + 1 : d->n_fft;
   prepare_window_kernel<<<1, 256, 0, stream>>>(window, d->win_length, d->n_fft, n_bins, d->n_mels, d->n_mfcc,
-                                               d->frame_length_norm, d->window_norm,
-                                               reinterpret_cast<WsHeader*>(base + l.header),
-                                               reinterpret_cast<float*>(base + l.window));
-  prepare_twiddle_kernel<<<(d->n_fft + 255) / 256, 256, 0, stream>>>(d->n_fft, reinterpret_cast<float2*>(base + l.twiddle));
-  if (d->n_mels > 0) {
-    prepare_fbank_kernel<<<(d->n_mels + 63) / 64, 64, 0, stream>>>(fb, n_bins, d->n_mels,
-                                                                  reinterpret_cast<float*>(base + l.fb),
-                                                                  reinterpret_cast<int2*>(base + l.bands));
-  }
+                                               d->frame_length_norm, d->window_norm, t.header, t.window);
+  prepare_twiddle_kernel<<<(d->n_fft + 255) / 256, 256, 0, stream>>>(d->n_fft, t.twiddle);
+  if (d->n_mels > 0) prepare_fbank_kernel<<<(d->n_mels + 63) / 64, 64, 0, stream>>>(fb, n_bins, d->n_mels, t.fb, t.bands);
   if (d->n_mfcc > 0) {
     const int64_t n = (int64_t)d->n_mels * d->n_mfcc;
-    copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(dct, reinterpret_cast<float*>(base + l.dct), n);
+    copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(dct, t.dct, n);
   }
   return launch_status();
 }
@@ -736,92 +729,69 @@ static int launch_stockham(void (*kern)(Params), Params p, int64_t rows, int64_t
   return launch_kernel(kern, grid, 256, smem, stream, p);
 }
 
-static int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
-                                int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
-                                int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd,
-                                bool kaldi_prelog) {
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
+// The GenericParams fields every Stockham front-end launch fills alike: the transform and the stage from the descriptor,
+// the workspace tables, and the waveform and its framing into `frames` frames of `out`.  n_stages < 0: n_fft has no
+// Stockham factorisation.
+static GenericParams generic_params(const b200a_frontend_desc& d, const void* ws, int stage, const float* wave,
+                                    int64_t length, int64_t row_stride, int64_t frames, float* out) {
+  const FrontendWs<const void> t = frontend_ws(d, ws);
   GenericParams p{};
-  p.n_stages = factorize(d->n_fft, p.radix);
-  if (p.n_stages < 0) return B200A_EUNSUPPORTED;
+  p.n_stages = factorize(d.n_fft, p.radix);
   p.wave = wave;
   p.length = length;
   p.row_stride = row_stride;
   p.frames = frames;
   p.out = out;
+  p.window = t.window;
+  p.twiddle = t.twiddle;
+  p.bands = t.bands;
+  p.fb = t.fb;
+  p.hdr = t.header;
+  p.n_fft = d.n_fft;
+  p.hop = d.hop;
+  p.pad = d.pad;
+  p.center = d.center;
+  p.pad_mode = d.pad_mode;
+  p.n_bins = d.onesided ? d.n_fft / 2 + 1 : d.n_fft;
+  p.n_mels = d.n_mels;
+  p.stage = stage;
+  p.power = d.power;
+  p.out_width = stage >= B200A_STAGE_MEL ? p.n_mels : p.n_bins;
+  p.k_energy_col = -1;
+  return p;
+}
+
+static int frontend_run_generic(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                                int64_t length, int64_t row_stride, int64_t frames, float* out, float* group_max,
+                                int64_t rows_per_group, cudaStream_t stream, const b200a_kaldi_desc* kd,
+                                bool kaldi_prelog) {
+  GenericParams p = generic_params(*d, ws, stage, wave, length, row_stride, frames, out);
+  if (p.n_stages < 0) return B200A_EUNSUPPORTED;
   p.group_max = group_max;
   p.rows_per_group = rows_per_group;
-  p.window = reinterpret_cast<const float*>(base + l.window);
-  p.twiddle = reinterpret_cast<const float2*>(base + l.twiddle);
-  p.bands = reinterpret_cast<const int2*>(base + l.bands);
-  p.fb = reinterpret_cast<const float*>(base + l.fb);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
-  p.n_fft = d->n_fft;
-  p.hop = d->hop;
-  p.pad = d->pad;
-  p.center = d->center;
-  p.pad_mode = d->pad_mode;
-  p.n_bins = d->onesided ? d->n_fft / 2 + 1 : d->n_fft;
-  p.n_mels = d->n_mels;
-  p.stage = stage;
   p.log_mels = d->log_mels;
-  p.power = d->power;
   p.db_mult = d->db_multiplier;
   p.db_amin = d->db_amin;
   p.db_offset = d->db_offset;
-  p.out_width = stage >= B200A_STAGE_MEL ? p.n_mels : p.n_bins;
-  p.out_col0 = 0;
-  p.k_energy_col = -1;
   if (kd != nullptr) {
-    p.kaldi = 1;
-    p.k_win = kd->window_size;
+    fill_kaldi(p, *kd, true);
     p.k_snip = kd->snip_edges;
-    p.k_dc = kd->remove_dc_offset;
-    p.k_preemph = kd->preemphasis;
     // the COMPLEX stage's output is the spectrum alone: no energy column to write into
     p.k_energy_mode = kd->energy_col >= 0 && stage != B200A_STAGE_COMPLEX ? kd->energy_mode : 0;
-    p.k_energy_floor = kd->energy_floor;
-    p.k_energy_col = kd->energy_col;
     p.k_log = kaldi_prelog ? 0 : kd->use_log;
     p.k_prelog = kaldi_prelog;
-    p.out_width = kd->out_width;
-    p.out_col0 = kd->out_col0;
   }
   return launch_stockham(stft_generic_kernel, p, rows, frames, stream);
 }
 
-// The RNN-T features: the Stockham kernel for every n_fft (powers of two included), MEL stage, chain epilogue.
+// The RNN-T features: the Stockham kernel for every n_fft (powers of two included), MEL stage, chain epilogue.  The
+// descriptor is one-sided (validate_desc: n_mels > 0); log_mels and the dB fields stay 0.
 int rnnt_features_impl(const b200a_frontend_desc* d, const void* ws, const float* wave, int64_t rows, int64_t length,
                        int64_t row_stride, const int64_t* lengths, const float* stats, float gain, int64_t out_frames,
                        float* out, float* mel_out, cudaStream_t stream) {
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
-  GenericParams p{};
-  p.n_stages = factorize(d->n_fft, p.radix);
+  GenericParams p = generic_params(*d, ws, B200A_STAGE_MEL, wave, length, row_stride, out_frames, out);
   if (p.n_stages < 0) return B200A_EUNSUPPORTED;
-  p.wave = wave;
-  p.length = length;
-  p.row_stride = row_stride;
-  p.frames = out_frames;
-  p.out = out;
   p.rows_per_group = 1;
-  p.window = reinterpret_cast<const float*>(base + l.window);
-  p.twiddle = reinterpret_cast<const float2*>(base + l.twiddle);
-  p.bands = reinterpret_cast<const int2*>(base + l.bands);
-  p.fb = reinterpret_cast<const float*>(base + l.fb);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
-  p.n_fft = d->n_fft;
-  p.hop = d->hop;
-  p.pad = d->pad;
-  p.center = d->center;
-  p.pad_mode = d->pad_mode;
-  p.n_bins = d->n_fft / 2 + 1;
-  p.n_mels = d->n_mels;
-  p.stage = B200A_STAGE_MEL;
-  p.power = d->power;
-  p.out_width = d->n_mels;
-  p.k_energy_col = -1;
   p.lengths = lengths;
   p.stats = stats;
   p.mel_out = mel_out;
@@ -963,8 +933,7 @@ static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const
   const int rc = istft_frames_pow2(d, ws, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, stream);
   if (rc != kPathDeclined) return rc;
   // any other size: shared-memory Stockham
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const FrontendWs<const void> t = frontend_ws(*d, ws);
   IstftParams p{};
   p.n_stages = factorize(d->n_fft, p.radix);
   if (p.n_stages < 0) return B200A_EUNSUPPORTED;
@@ -974,9 +943,9 @@ static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const
   p.stride_frame = stride_frame;
   p.frames = frames;
   p.frame_buf = frame_buf;
-  p.window = reinterpret_cast<const float*>(base + l.window);
-  p.twiddle = reinterpret_cast<const float2*>(base + l.twiddle);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.window = t.window;
+  p.twiddle = t.twiddle;
+  p.hdr = t.header;
   p.n_fft = d->n_fft;
   return launch_stockham(istft_frames_kernel, p, rows, frames, stream);
 }
@@ -987,11 +956,10 @@ int istft_run_impl(const b200a_frontend_desc* d, const void* ws, const float* sp
   if (rows > 65535) return B200A_EUNSUPPORTED;  // the overlap-add grid keeps rows in blockIdx.y
   int rc = istft_frames_impl(d, ws, spec, rows, frames, stride_row, stride_bin, stride_frame, frame_buf, stream);
   if (rc != B200A_OK) return rc;
-  const float* window = reinterpret_cast<const float*>(static_cast<const unsigned char*>(ws) + ws_layout(*d).window);
   const int64_t blocks = (out_len + 255) / 256;
   if (blocks > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  istft_ola_kernel<<<dim3((unsigned)blocks, (unsigned)rows), 256, 0, stream>>>(frame_buf, window, d->n_fft, d->hop, frames,
-                                                                               start, out_len, out, out_row_stride);
+  istft_ola_kernel<<<dim3((unsigned)blocks, (unsigned)rows), 256, 0, stream>>>(
+      frame_buf, frontend_ws(*d, ws).window, d->n_fft, d->hop, frames, start, out_len, out, out_row_stride);
   return launch_status();
 }
 
@@ -1138,8 +1106,7 @@ size_t frontend_backward_scratch(const b200a_frontend_desc* d, int stage, int64_
 static int spec_vjp_frames(const b200a_frontend_desc* d, const void* ws, int stage, float2* spec, const float* grad,
                            int64_t gs_row, int64_t gs_frame, int64_t gs_col, int* bad, int64_t rows, int64_t frames,
                            float* frame_buf, cudaStream_t stream) {
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const FrontendWs<const void> t = frontend_ws(*d, ws);
   const int64_t n = rows * frames;
   const int n_bins = d->onesided ? d->n_fft / 2 + 1 : d->n_fft;
   SpecVjpParams p{};
@@ -1149,9 +1116,9 @@ static int spec_vjp_frames(const b200a_frontend_desc* d, const void* ws, int sta
   p.gs_frame = gs_frame;
   p.gs_col = gs_col;
   p.bad = bad;
-  p.fb = reinterpret_cast<const float*>(base + l.fb);
-  p.bands = reinterpret_cast<const int2*>(base + l.bands);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.fb = t.fb;
+  p.bands = t.bands;
+  p.hdr = t.header;
   p.frames = frames;
   p.total = n;
   p.n_fft = d->n_fft;
@@ -1178,7 +1145,7 @@ int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int sta
   if (backward_fused_applicable(d, stage)) {
     frame_buf = reinterpret_cast<float*>(sc);
     rc = frontend_backward_pow2(d, ws, stage, wave, rows, length, row_stride, frames, grad, gs_row, gs_frame, gs_col, frame_buf,
-                                stream);
+                                stream, nullptr);
   } else {
     // composition: forward complex spectrum -> H * N * scale^2 in place -> the iSTFT frame stage -> fold
     const int n_bins = d->onesided ? d->n_fft / 2 + 1 : d->n_fft;
@@ -1244,15 +1211,13 @@ int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const floa
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream) {
   const int rc = istft_backward_pow2(d, ws, grad, rows, g_row_stride, start, g_len, frames, grad_spec, stream);
   if (rc != kPathDeclined) return rc;
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const FrontendWs<const void> t = frontend_ws(*d, ws);
   const int64_t expected = d->n_fft + (int64_t)d->hop * (frames - 1);
   float* g_hat = static_cast<float*>(scratch);
   const int64_t bpr = (expected + 255) / 256;
   if (rows * bpr > 0x7fffffffLL) return B200A_EUNSUPPORTED;
   istft_grad_prescale_kernel<<<(unsigned)(rows * bpr), 256, 0, stream>>>(
-      grad, g_row_stride, start, g_len, reinterpret_cast<const float*>(base + l.window), d->n_fft, d->hop, frames, expected,
-      bpr, g_hat);
+      grad, g_row_stride, start, g_len, t.window, d->n_fft, d->hop, frames, expected, bpr, g_hat);
   int r = launch_status();
   if (r != B200A_OK) return r;
   b200a_frontend_desc plain = *d;  // frames of g_hat from sample 0: no centre or constant padding
@@ -1265,8 +1230,8 @@ int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const floa
   const int64_t n = rows * frames * n_bins;
   const int64_t grid = sm_capped_grid((n + 255) / 256, 8);
   if (grid < 0) return B200A_ECUDA;
-  istft_grad_scale_kernel<<<(unsigned)grid, 256, 0, stream>>>(
-      reinterpret_cast<float2*>(grad_spec), n, d->n_fft, n_bins, reinterpret_cast<const WsHeader*>(base + l.header));
+  istft_grad_scale_kernel<<<(unsigned)grid, 256, 0, stream>>>(reinterpret_cast<float2*>(grad_spec), n, d->n_fft, n_bins,
+                                                              t.header);
   return launch_status();
 }
 
@@ -1430,8 +1395,8 @@ int kaldi_backward_impl(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d
   const int64_t gv_row = frames * kd->out_width, gv_frame = kd->out_width;
   if (fused) {  // padded 256 / 512 / 1024: X recomputed in registers, G -> H -> inverse transform in one kernel
     bad = nullptr;  // the kernel writes a NaN frame's gradient as NaN itself
-    rc = kaldi_backward_pow2(d, kd, ws, stage, wave, rows, length, row_stride, frames, g_v, gv_row, gv_frame, 1, frame_buf,
-                             stream);
+    rc = frontend_backward_pow2(d, ws, stage, wave, rows, length, row_stride, frames, g_v, gv_row, gv_frame, 1, frame_buf,
+                                stream, kd);
   } else {  // composition: the conditioned complex spectrum, its adjoint in place, the iSTFT frame stage
     rc = frontend_run_impl(d, ws, B200A_STAGE_COMPLEX, wave, rows, length, row_stride, frames,
                            reinterpret_cast<float*>(spec), nullptr, 1, stream, kd);
@@ -1443,7 +1408,7 @@ int kaldi_backward_impl(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d
   cp.frame_buf = frame_buf;
   cp.g_energy = g_energy;
   cp.wave = wave;
-  cp.window = reinterpret_cast<const float*>(static_cast<const unsigned char*>(ws) + ws_layout(*d).window);
+  cp.window = frontend_ws(*d, ws).window;
   cp.length = length;
   cp.row_stride = row_stride;
   cp.frames = frames;
@@ -1459,9 +1424,8 @@ int kaldi_backward_impl(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d
   if (rc != B200A_OK) return rc;
   const int64_t bpr = (length + 255) / 256;
   if (rows * bpr > 0x7fffffffLL) return B200A_EUNSUPPORTED;
-  const int lead = kd->snip_edges ? 0 : kd->window_size / 2 - kd->window_shift / 2;
   frame_fold_kernel<<<(unsigned)(rows * bpr), 256, 0, stream>>>(frame_buf, bad, d->n_fft, kd->window_size, kd->window_shift,
-                                                                frames, length, 0, lead,
+                                                                frames, length, 0, kaldi_lead(*kd),
                                                                 kd->snip_edges ? B200A_PAD_CONSTANT : kPadSymmetric, bpr,
                                                                 grad_wave, grad_row_stride);
   return launch_status();
@@ -1470,8 +1434,7 @@ int kaldi_backward_impl(const b200a_kaldi_desc* kd, const b200a_frontend_desc* d
 int mfcc_finish_impl(const b200a_frontend_desc* d, const void* ws, const float* feat, int64_t rows,
                      int64_t frames, const float* group_max, int64_t rows_per_group, float top_db,
                      float* out, cudaStream_t stream) {
-  const WsLayout l = ws_layout(*d);
-  const float* dct = reinterpret_cast<const float*>(static_cast<const unsigned char*>(ws) + l.dct);
+  const float* dct = frontend_ws(*d, ws).dct;
   const int64_t total = rows * frames;
   if (total == 0) return B200A_OK;
   if (rows_per_group < 1) rows_per_group = 1;

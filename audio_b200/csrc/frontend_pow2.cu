@@ -107,6 +107,20 @@ inline Pow2Extra pow2_layout(const b200a_frontend_desc& d, size_t base) {
   return e;
 }
 
+// The register-FFT tables of a front-end workspace (Pow2Extra), after its front-end tables.
+template <typename W>
+struct Pow2Ws {
+  WsPtr<W, float2> tw2d, tw_eo;
+  WsPtr<W, MelPlan> plan;
+  WsPtr<W, float4> frags;
+};
+
+template <typename W>
+Pow2Ws<W> pow2_ws(const b200a_frontend_desc& d, W* ws) {
+  const Pow2Extra e = pow2_layout(d, ws_layout(d).total);
+  return {ws_at<float2>(ws, e.tw2d), ws_at<float2>(ws, e.tw_eo), ws_at<MelPlan>(ws, e.plan), ws_at<float4>(ws, e.frags)};
+}
+
 bool pow2_applicable(const b200a_frontend_desc& d) {
   return (d.n_fft == 2048 || d.n_fft == 1024 || d.n_fft == 512 || d.n_fft == 256) && d.onesided != 0;
 }
@@ -1551,19 +1565,16 @@ size_t pow2_workspace_extra(const b200a_frontend_desc* d) {
 
 int pow2_prepare(const b200a_frontend_desc* d, void* ws, size_t ws_bytes, cudaStream_t stream) {
   if (!pow2_applicable(*d)) return B200A_OK;
-  const WsLayout l = ws_layout(*d);
-  const Pow2Extra e = pow2_layout(*d, l.total);
-  if (ws_bytes < e.total) return B200A_EWORKSPACE;
-  unsigned char* base = static_cast<unsigned char*>(ws);
+  if (ws_bytes < b200a_frontend_workspace_bytes(d)) return B200A_EWORKSPACE;
+  const FrontendWs<void> t = frontend_ws(*d, ws);
+  const Pow2Ws<void> x = pow2_ws(*d, ws);
   const int G = fft_g(d->n_fft);
-  prepare_tw2d_kernel<<<(32 * G + 255) / 256, 256, 0, stream>>>(reinterpret_cast<float2*>(base + e.tw2d), G);
-  if (d->n_fft == 2048) prepare_tw_eo_kernel<<<3, 256, 0, stream>>>(reinterpret_cast<float2*>(base + e.tw_eo));
+  prepare_tw2d_kernel<<<(32 * G + 255) / 256, 256, 0, stream>>>(x.tw2d, G);
+  if (d->n_fft == 2048) prepare_tw_eo_kernel<<<3, 256, 0, stream>>>(x.tw_eo);
   if (d->n_mels > 0 && mel_tiles(d->n_mels) <= kMaxItems) {
     const int n_mtiles = d->n_fft == 2048 ? 0 : kUniWarps * unit_frames(d->n_fft) / 16;  // Geo<G>::kMTiles
-    prepare_mma_kernel<<<1, 256, 0, stream>>>(reinterpret_cast<const float*>(base + l.fb),
-                                              reinterpret_cast<const int2*>(base + l.bands), d->n_fft / 2 + 1, d->n_mels,
-                                              mel_tiles(d->n_mels), n_mtiles, reinterpret_cast<MelPlan*>(base + e.plan),
-                                              reinterpret_cast<float4*>(base + e.frags));
+    prepare_mma_kernel<<<1, 256, 0, stream>>>(t.fb, t.bands, d->n_fft / 2 + 1, d->n_mels, mel_tiles(d->n_mels), n_mtiles,
+                                              x.plan, x.frags);
   }
   return launch_status();
 }
@@ -1636,9 +1647,7 @@ static int stage_floats(int n_fft, bool mel) {
 // `staging` floats, and its gather can index with 32 bits.
 static Pow2Params pow2_geometry(const b200a_frontend_desc& d, const void* ws, const float* wave, int64_t rows,
                                 int64_t length, int64_t row_stride, int64_t frames, int staging) {
-  const WsLayout l = ws_layout(d);
-  const Pow2Extra e = pow2_layout(d, l.total);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const FrontendWs<const void> t = frontend_ws(d, ws);
   const int frames_per_unit = unit_frames(d.n_fft);
   Pow2Params p{};
   p.wave = wave;
@@ -1647,9 +1656,9 @@ static Pow2Params pow2_geometry(const b200a_frontend_desc& d, const void* ws, co
   p.frames = frames;
   p.units_per_row = (frames + frames_per_unit - 1) / frames_per_unit;
   p.total_units = rows * p.units_per_row;
-  p.window = reinterpret_cast<const float*>(base + l.window);
-  p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.window = t.window;
+  p.tw2d = pow2_ws(d, ws).tw2d;
+  p.hdr = t.header;
   p.hop = d.hop;
   p.pad = d.pad;
   p.center = d.center;
@@ -1668,8 +1677,7 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   // Kaldi features with a 256 / 512 / 1024-point FFT; every other size takes the generic kernel
   if (kd != nullptr && d->n_fft > 1024) return kPathDeclined;
   if (stage >= B200A_STAGE_MEL && mel_tiles(d->n_mels) > kMaxItems) return kPathDeclined;  // > 512 filters
-  const Pow2Extra e = pow2_layout(*d, ws_layout(*d).total);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const Pow2Ws<const void> x = pow2_ws(*d, ws);
   const bool eo = d->n_fft == 2048;
   const bool mel = stage >= B200A_STAGE_MEL;
   const int staging = stage_floats(d->n_fft, mel);
@@ -1677,8 +1685,8 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   p.out = out;
   p.group_max = group_max;
   p.rows_per_group = rows_per_group;
-  p.plan = reinterpret_cast<const MelPlan*>(base + e.plan);
-  p.frags = reinterpret_cast<const float4*>(base + e.frags);
+  p.plan = x.plan;
+  p.frags = x.frags;
   p.n_mels = d->n_mels;
   p.stage = stage;
   p.log_mels = d->log_mels;
@@ -1686,22 +1694,14 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   p.db_amin = d->db_amin;
   p.db_offset = d->db_offset;
   p.out_width = stage >= B200A_STAGE_MEL ? d->n_mels : d->n_fft / 2 + 1;
-  p.out_col0 = 0;
   p.k_energy_col = -1;
   int64_t lead = (d->center ? d->n_fft / 2 : 0) + d->pad;
   if (kd != nullptr) {
-    p.kaldi = 1;
-    p.k_off = kd->snip_edges ? 0 : kd->window_size / 2 - kd->window_shift / 2;
-    p.k_win = kd->window_size;
-    p.k_dc = kd->remove_dc_offset;
-    p.k_preemph = kd->preemphasis;
+    fill_kaldi(p, *kd, true);
+    p.k_off = kaldi_lead(*kd);
     p.k_energy_mode = kd->energy_col >= 0 ? kd->energy_mode : 0;
-    p.k_energy_floor = kd->energy_floor;
-    p.k_energy_col = kd->energy_col;
     p.k_log = kaldi_prelog ? 0 : kd->use_log;
     p.k_prelog = kaldi_prelog;
-    p.out_width = kd->out_width;
-    p.out_col0 = kd->out_col0;
     p.pad_mode = kPadSymmetric;  // only reached when snip_edges == 0 (frames never leave the signal otherwise)
     lead = p.k_off;
     if (!p.stage_ok) return kPathDeclined;  // the conditioning reads the staged span
@@ -1713,10 +1713,7 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
   p.out_vec = (p.out_width % 4 == 0 && p.out_col0 % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0)   ? 4
               : (p.out_width % 2 == 0 && p.out_col0 % 2 == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0) ? 2
                                                                                                               : 1;
-  if (eo) {
-    const float2* tw_eo = reinterpret_cast<const float2*>(base + e.tw_eo);
-    return d->power == 2.f ? launch_eo<2>(p, tw_eo, mel, stream) : launch_eo<0>(p, tw_eo, mel, stream);
-  }
+  if (eo) return d->power == 2.f ? launch_eo<2>(p, x.tw_eo, mel, stream) : launch_eo<0>(p, x.tw_eo, mel, stream);
   return with_g(d->n_fft, [&](auto g) {
     constexpr int G = decltype(g)::value;
     if (stage == B200A_STAGE_COMPLEX) return launch_g<kComplexOut, G>(p, false, stream);
@@ -1728,22 +1725,19 @@ int frontend_run_pow2(const b200a_frontend_desc* d, const void* ws, int stage, c
 int istft_frames_pow2(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
                       int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf, cudaStream_t stream) {
   if (!pow2_applicable(*d) || d->n_fft > 1024) return kPathDeclined;
-  const WsLayout l = ws_layout(*d);
-  const Pow2Extra e = pow2_layout(*d, l.total);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
-  const int frames_per_unit = unit_frames(d->n_fft);
+  const Pow2Params g = pow2_geometry(*d, ws, nullptr, rows, 0, 0, frames, 0);  // the unit grid and the FFT tables
   IstftPow2Params p{};
   p.spec = reinterpret_cast<const float2*>(spec);
   p.stride_row = stride_row;
   p.stride_bin = stride_bin;
   p.stride_frame = stride_frame;
   p.frames = frames;
-  p.units_per_row = (frames + frames_per_unit - 1) / frames_per_unit;
-  p.total_units = rows * p.units_per_row;
+  p.units_per_row = g.units_per_row;
+  p.total_units = g.total_units;
   p.frame_buf = frame_buf;
-  p.window = reinterpret_cast<const float*>(base + l.window);
-  p.tw2d = reinterpret_cast<const float2*>(base + e.tw2d);
-  p.hdr = reinterpret_cast<const WsHeader*>(base + l.header);
+  p.window = g.window;
+  p.tw2d = g.tw2d;
+  p.hdr = g.hdr;
   const int64_t grid = persistent_grid(p.total_units, kIsWarps);
   return with_g(d->n_fft, [&](auto g) {
     constexpr int G = decltype(g)::value;
@@ -1762,37 +1756,6 @@ static size_t backward_smem(const b200a_frontend_desc* d, int stage) {
 
 bool backward_fused_applicable(const b200a_frontend_desc* d, int stage) { return backward_smem(d, stage) != 0; }
 
-// First half of b200a_frontend_backward for n_fft = 256 / 512 / 1024: frame gradients into frame_buf.
-int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
-                           int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
-                           int64_t gs_frame, int64_t gs_col, float* frame_buf, cudaStream_t stream) {
-  const size_t smem = backward_smem(d, stage);
-  if (smem == 0) return B200A_EUNSUPPORTED;
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
-  BwdParams bp{};
-  // edge units gather their span into the Spectrogram kernel's float2 transpose tile; bulk_ok stays 0: the tile doubles
-  // as the inverse transform's, so nothing is staged into it ahead
-  bp.f = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, stage_floats(d->n_fft, false));
-  bp.f.n_mels = stage == B200A_STAGE_MEL ? d->n_mels : 0;
-  bp.f.stage = stage;
-  bp.grad = grad;
-  bp.gs_row = gs_row;
-  bp.gs_frame = gs_frame;
-  bp.gs_col = gs_col;
-  bp.frame_buf = frame_buf;
-  bp.fb = reinterpret_cast<const float*>(base + l.fb);
-  bp.bands = reinterpret_cast<const int2*>(base + l.bands);
-  const int64_t grid = persistent_grid(bp.f.total_units, kBwWarps);
-  return with_g(d->n_fft, [&](auto g) {
-    constexpr int G = decltype(g)::value;
-    auto kern = stage == B200A_STAGE_COMPLEX ? stft_pow2_backward_kernel<G, B200A_STAGE_COMPLEX, false>
-                : stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<G, B200A_STAGE_POWER, false>
-                                             : stft_pow2_backward_kernel<G, B200A_STAGE_MEL, false>;
-    return launch_kernel(kern, grid, kBwWarps * 32, smem, stream, bp);
-  });
-}
-
 // The Kaldi gradient takes the fused kernel when the padded size is 256 / 512 / 1024, the staged g rows fit shared
 // memory (backward_smem) and a unit's span fits the transpose tile the Kaldi load stage conditions in -- all decided by
 // the descriptors and the signal length, never by the batch.
@@ -1802,36 +1765,46 @@ bool kaldi_backward_fused_applicable(const b200a_frontend_desc* d, const b200a_k
   return span <= stage_floats(d->n_fft, false) && length + d->n_fft < (int64_t)1 << 31;
 }
 
-// Frame gradients w * N * irfft(H) of the Kaldi features for padded 256 / 512 / 1024: `grad` is the log adjoint's dL/dv
-// (value k or filter m of frame t at grad[row gs_row + t gs_frame + (k | m) gs_col]).
-int kaldi_backward_pow2(const b200a_frontend_desc* d, const b200a_kaldi_desc* kd, const void* ws, int stage,
-                        const float* wave, int64_t rows, int64_t length, int64_t row_stride, int64_t frames,
-                        const float* grad, int64_t gs_row, int64_t gs_frame, int64_t gs_col, float* frame_buf,
-                        cudaStream_t stream) {
-  if (!kaldi_backward_fused_applicable(d, kd, stage, length)) return kPathDeclined;
+// First half of b200a_frontend_backward and b200a_kaldi_backward for n_fft = 256 / 512 / 1024: frame gradients
+// w * N * irfft(H) into frame_buf.  With kd, `grad` is the log adjoint's dL/dv (value k or filter m of frame t at
+// grad[row gs_row + t gs_frame + (k | m) gs_col]).
+int frontend_backward_pow2(const b200a_frontend_desc* d, const void* ws, int stage, const float* wave, int64_t rows,
+                           int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
+                           int64_t gs_frame, int64_t gs_col, float* frame_buf, cudaStream_t stream,
+                           const b200a_kaldi_desc* kd) {
+  if (kd != nullptr ? !kaldi_backward_fused_applicable(d, kd, stage, length) : !backward_fused_applicable(d, stage))
+    return B200A_EUNSUPPORTED;
   const size_t smem = backward_smem(d, stage);
-  const WsLayout l = ws_layout(*d);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
   BwdParams bp{};
+  // edge units gather their span into the Spectrogram kernel's float2 transpose tile; bulk_ok stays 0: the tile doubles
+  // as the inverse transform's, so nothing is staged into it ahead
   bp.f = pow2_geometry(*d, ws, wave, rows, length, row_stride, frames, stage_floats(d->n_fft, false));
   bp.f.n_mels = stage == B200A_STAGE_MEL ? d->n_mels : 0;
   bp.f.stage = stage;
-  bp.f.kaldi = 1;
-  bp.f.k_off = kd->snip_edges ? 0 : kd->window_size / 2 - kd->window_shift / 2;
-  bp.f.k_win = kd->window_size;
-  bp.f.k_dc = kd->remove_dc_offset;
-  bp.f.k_preemph = kd->preemphasis;
-  bp.f.k_energy_mode = 0;  // the energy's adjoint is kaldi_cond_vjp_kernel's; nothing is written to an output row
-  bp.f.pad_mode = kPadSymmetric;
+  if (kd != nullptr) {
+    // k_energy_mode stays 0: the energy's adjoint is kaldi_cond_vjp_kernel's; nothing is written to an output row
+    fill_kaldi(bp.f, *kd, false);
+    bp.f.k_off = kaldi_lead(*kd);
+    bp.f.pad_mode = kPadSymmetric;
+  }
   bp.grad = grad;
   bp.gs_row = gs_row;
   bp.gs_frame = gs_frame;
   bp.gs_col = gs_col;
   bp.frame_buf = frame_buf;
-  bp.fb = reinterpret_cast<const float*>(base + l.fb);
-  bp.bands = reinterpret_cast<const int2*>(base + l.bands);
+  const FrontendWs<const void> t = frontend_ws(*d, ws);
+  bp.fb = t.fb;
+  bp.bands = t.bands;
   const int64_t grid = persistent_grid(bp.f.total_units, kBwWarps);
-  return with_g(d->n_fft, [&](auto g) {
+  if (kd == nullptr)
+    return with_g(d->n_fft, [&](auto g) {
+      constexpr int G = decltype(g)::value;
+      auto kern = stage == B200A_STAGE_COMPLEX ? stft_pow2_backward_kernel<G, B200A_STAGE_COMPLEX, false>
+                  : stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<G, B200A_STAGE_POWER, false>
+                                               : stft_pow2_backward_kernel<G, B200A_STAGE_MEL, false>;
+      return launch_kernel(kern, grid, kBwWarps * 32, smem, stream, bp);
+    });
+  return with_g(d->n_fft, [&](auto g) {  // the Kaldi stages are POWER and MEL
     constexpr int G = decltype(g)::value;
     auto kern = stage == B200A_STAGE_POWER ? stft_pow2_backward_kernel<G, B200A_STAGE_POWER, true>
                                            : stft_pow2_backward_kernel<G, B200A_STAGE_MEL, true>;

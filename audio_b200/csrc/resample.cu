@@ -87,6 +87,22 @@ inline RsLayout rs_layout(int new_r, int taps) {
   return l;
 }
 
+// The tables of a resampler workspace (RsLayout).
+template <typename W>
+struct RsWs {
+  WsPtr<W, RsHeader> header;
+  WsPtr<W, int2> support;
+  WsPtr<W, BandTile> tiles;
+  WsPtr<W, float4> frags;
+};
+
+template <typename W>
+RsWs<W> rs_ws(int new_r, int taps, W* ws) {
+  const RsLayout l = rs_layout(new_r, taps);
+  return {ws_at<RsHeader>(ws, l.header), ws_at<int2>(ws, l.support), ws_at<BandTile>(ws, l.tiles),
+          ws_at<float4>(ws, l.frags)};
+}
+
 // One warp per phase: [first, last] index of taps with |k| > 1e-12 * max|k| of that row.
 __global__ void resample_support_kernel(const float* __restrict__ kernel, int new_r, int taps, int orig_r,
                                         int width, RsHeader* hdr, int2* support) {
@@ -403,6 +419,23 @@ inline RbLayout rb_layout(int orig_r, int new_r, int width) {
   return l;
 }
 
+// The tables of a resampler adjoint workspace (RbLayout).
+template <typename W>
+struct RbWs {
+  WsPtr<W, RsHeader> header;
+  WsPtr<W, int2> support, tap_range;
+  WsPtr<W, float> kt;
+  WsPtr<W, BandTile> cols;
+  WsPtr<W, float4> frags;
+};
+
+template <typename W>
+RbWs<W> rb_ws(int orig_r, int new_r, int width, W* ws) {
+  const RbLayout l = rb_layout(orig_r, new_r, width);
+  return {ws_at<RsHeader>(ws, l.header), ws_at<int2>(ws, l.support), ws_at<int2>(ws, l.tap_range),
+          ws_at<float>(ws, l.kt),        ws_at<BandTile>(ws, l.cols), ws_at<float4>(ws, l.frags)};
+}
+
 // One thread per tap: the hull of the phases for which it is live; and kt, the masked transpose of the kernel.
 __global__ void resample_adjoint_table_kernel(const float* __restrict__ kernel, const int2* __restrict__ support,
                                               int new_r, int taps, int2* tap_range, float* kt) {
@@ -576,23 +609,16 @@ int resample_backward_prepare_impl(const float* kernel, int orig_r, int new_r, i
                                    cudaStream_t stream) {
   if (kernel == nullptr || ws == nullptr || orig_r < 1 || new_r < 1 || width < 0) return B200A_EINVAL;
   const int taps = 2 * width + orig_r;
-  const RbLayout l = rb_layout(orig_r, new_r, width);
-  if (ws_bytes < l.total) return B200A_EWORKSPACE;
+  if (ws_bytes < resample_backward_workspace_bytes_impl(orig_r, new_r, width)) return B200A_EWORKSPACE;
   const RbConfig c = rb_config(orig_r, new_r, width);
-  unsigned char* base = static_cast<unsigned char*>(ws);
-  if (cudaMemsetAsync(base + l.header, 0, sizeof(RsHeader), stream) != cudaSuccess) return B200A_ECUDA;
-  RsHeader* hdr = reinterpret_cast<RsHeader*>(base + l.header);
-  int2* support = reinterpret_cast<int2*>(base + l.support);
-  int2* tap_range = reinterpret_cast<int2*>(base + l.tap_range);
-  float* kt = reinterpret_cast<float*>(base + l.kt);
-  resample_support_kernel<<<(new_r + 7) / 8, 256, 0, stream>>>(kernel, new_r, taps, orig_r, width, hdr, support);
+  const RbWs<void> t = rb_ws(orig_r, new_r, width, ws);
+  if (cudaMemsetAsync(t.header, 0, sizeof(RsHeader), stream) != cudaSuccess) return B200A_ECUDA;
+  resample_support_kernel<<<(new_r + 7) / 8, 256, 0, stream>>>(kernel, new_r, taps, orig_r, width, t.header, t.support);
   const int64_t elems = (int64_t)taps * new_r;
   const unsigned grid = (unsigned)std::min<int64_t>(std::max<int64_t>((elems + 255) / 256, (taps + 255) / 256), 4096);
-  resample_adjoint_table_kernel<<<grid, 256, 0, stream>>>(kernel, support, new_r, taps, tap_range, kt);
+  resample_adjoint_table_kernel<<<grid, 256, 0, stream>>>(kernel, t.support, new_r, taps, t.tap_range, t.kt);
   if (c.mma)
-    resample_plan_kernel<<<1, 256, 0, stream>>>(kt, tap_range, taps, new_r, c.n_cols, hdr,
-                                                reinterpret_cast<BandTile*>(base + l.cols),
-                                                reinterpret_cast<float4*>(base + l.frags));
+    resample_plan_kernel<<<1, 256, 0, stream>>>(t.kt, t.tap_range, taps, new_r, c.n_cols, t.header, t.cols, t.frags);
   return launch_status();
 }
 
@@ -600,9 +626,8 @@ int resample_backward_impl(const void* ws, int orig_r, int new_r, int width, con
                            int64_t g_row_stride, int64_t out_len, float* grad_wave, int64_t length,
                            int64_t grad_row_stride, cudaStream_t stream) {
   const int taps = 2 * width + orig_r;
-  const RbLayout l = rb_layout(orig_r, new_r, width);
+  const RbWs<const void> t = rb_ws(orig_r, new_r, width, ws);
   const RbConfig c = rb_config(orig_r, new_r, width);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
   if (c.mma) {
     RbParams p{};
     p.grad = grad;
@@ -611,9 +636,9 @@ int resample_backward_impl(const void* ws, int orig_r, int new_r, int width, con
     p.out = grad_wave;
     p.length = length;
     p.out_row_stride = grad_row_stride;
-    p.hdr = reinterpret_cast<const RsHeader*>(base + l.header);
-    p.cols = reinterpret_cast<const BandTile*>(base + l.cols);
-    p.frags = reinterpret_cast<const float4*>(base + l.frags);
+    p.hdr = t.header;
+    p.cols = t.cols;
+    p.frags = t.frags;
     p.orig_r = orig_r;
     p.new_r = new_r;
     p.width = width;
@@ -634,9 +659,8 @@ int resample_backward_impl(const void* ws, int orig_r, int new_r, int width, con
   }
   unsigned bx = (unsigned)std::min<int64_t>((length + 255) / 256, 4096);
   dim3 grid(bx, (unsigned)std::min<int64_t>(rows, 65535));
-  resample_backward_direct_kernel<<<grid, 256, 0, stream>>>(
-      grad, rows, g_row_stride, out_len, reinterpret_cast<const int2*>(base + l.tap_range),
-      reinterpret_cast<const float*>(base + l.kt), orig_r, new_r, width, taps, grad_wave, length, grad_row_stride);
+  resample_backward_direct_kernel<<<grid, 256, 0, stream>>>(grad, rows, g_row_stride, out_len, t.tap_range, t.kt, orig_r,
+                                                            new_r, width, taps, grad_wave, length, grad_row_stride);
   return launch_status();
 }
 
@@ -644,17 +668,12 @@ int resample_prepare_impl(const float* kernel, int orig_r, int new_r, int width,
                           cudaStream_t stream) {
   if (kernel == nullptr || ws == nullptr || orig_r < 1 || new_r < 1 || width < 0) return B200A_EINVAL;
   const int taps = 2 * width + orig_r;
-  const RsLayout l = rs_layout(new_r, taps);
-  if (ws_bytes < l.total) return B200A_EWORKSPACE;
-  unsigned char* base = static_cast<unsigned char*>(ws);
-  if (cudaMemsetAsync(base + l.header, 0, sizeof(RsHeader), stream) != cudaSuccess) return B200A_ECUDA;
-  RsHeader* hdr = reinterpret_cast<RsHeader*>(base + l.header);
-  int2* support = reinterpret_cast<int2*>(base + l.support);
-  resample_support_kernel<<<(new_r + 7) / 8, 256, 0, stream>>>(kernel, new_r, taps, orig_r, width, hdr, support);
+  if (ws_bytes < resample_workspace_bytes_impl(new_r, taps)) return B200A_EWORKSPACE;
+  const RsWs<void> t = rs_ws(new_r, taps, ws);
+  if (cudaMemsetAsync(t.header, 0, sizeof(RsHeader), stream) != cudaSuccess) return B200A_ECUDA;
+  resample_support_kernel<<<(new_r + 7) / 8, 256, 0, stream>>>(kernel, new_r, taps, orig_r, width, t.header, t.support);
   if (rs_tiles(new_r) <= kRsMaxTiles)
-    resample_plan_kernel<<<1, 256, 0, stream>>>(kernel, support, new_r, taps, rs_tiles(new_r), hdr,
-                                                reinterpret_cast<BandTile*>(base + l.tiles),
-                                                reinterpret_cast<float4*>(base + l.frags));
+    resample_plan_kernel<<<1, 256, 0, stream>>>(kernel, t.support, new_r, taps, rs_tiles(new_r), t.header, t.tiles, t.frags);
   return launch_status();
 }
 
@@ -665,8 +684,7 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
   if (rows == 0 || out_len == 0) return B200A_OK;  // empty batch: pointers may be null
   if (ws == nullptr || kernel == nullptr || wave == nullptr || out == nullptr) return B200A_EINVAL;
   const int taps = 2 * width + orig_r;
-  const RsLayout l = rs_layout(new_r, taps);
-  const unsigned char* base = static_cast<const unsigned char*>(ws);
+  const RsWs<const void> t = rs_ws(new_r, taps, ws);
 
   // ---- tensor-pipe path -------------------------------------------------------------------------
   const int n_tiles = rs_tiles(new_r);
@@ -682,9 +700,9 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
     p.out = out;
     p.out_row_stride = out_row_stride;
     p.out_len = out_len;
-    p.hdr = reinterpret_cast<const RsHeader*>(base + l.header);
-    p.tiles = reinterpret_cast<const BandTile*>(base + l.tiles);
-    p.frags = reinterpret_cast<const float4*>(base + l.frags);
+    p.hdr = t.header;
+    p.tiles = t.tiles;
+    p.frags = t.frags;
     p.orig_r = orig_r;
     p.new_r = new_r;
     p.width = width;
@@ -719,9 +737,8 @@ int resample_run_impl(const void* ws, const float* kernel, int orig_r, int new_r
   unsigned bx = (unsigned)((out_len + 255) / 256);
   if (bx > 4096) bx = 4096;
   dim3 grid(bx, (unsigned)rows);
-  resample_direct_kernel<<<grid, 256, 0, stream>>>(wave, length, row_stride, kernel,
-                                                  reinterpret_cast<const int2*>(base + l.support), orig_r, new_r,
-                                                  width, taps, out, out_row_stride, out_len);
+  resample_direct_kernel<<<grid, 256, 0, stream>>>(wave, length, row_stride, kernel, t.support, orig_r, new_r, width, taps,
+                                                  out, out_row_stride, out_len);
   return launch_status();
 }
 
