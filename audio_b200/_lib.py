@@ -15,9 +15,11 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 # B200A_LIB: load another build of the same ABI (A/B timing of kernel changes); the default is the in-tree build
 LIB_PATH = os.environ.get("B200A_LIB") or os.path.join(_PKG, "lib", "libb200audio.so")
 
-OK, EINVAL, EUNSUPPORTED, ESHORT, EWORKSPACE, ECUDA = 0, -1, -2, -3, -4, -5
+OK, EINVAL, EUNSUPPORTED, ESHORT, EWORKSPACE, ECUDA, ESINGULAR = 0, -1, -2, -3, -4, -5, -6
 PAD_MODE = {"reflect": 0, "constant": 1, "replicate": 2, "circular": 3}
 STAGE_COMPLEX, STAGE_POWER, STAGE_MEL, STAGE_FEAT = 0, 1, 2, 3
+LSTSQ_DRIVER = {"gels": 0, "gelsy": 1, "gelsd": 2, "gelss": 3}
+INVERSE_MEL_MAX_BANDWIDTH, INVERSE_MEL_MAX_MELS = 4, 512  # B200A_INVERSE_MEL_MAX_BANDWIDTH / _MAX_MELS
 
 
 class FrontendDesc(ctypes.Structure):
@@ -177,6 +179,18 @@ _SIGNATURES = {
     "b200a_resample_backward": (
         ctypes.c_int,
         [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p],
+    ),
+    "b200a_inverse_mel_plan_bytes": (c_size_t, [c_int32, c_int32]),
+    "b200a_inverse_mel_plan": (
+        ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_size_t, POINTER(c_int32), POINTER(c_int32)]),
+    "b200a_inverse_mel_run": (
+        ctypes.c_int,
+        [c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p],
+    ),
+    "b200a_inverse_mel_backward": (
+        ctypes.c_int,
+        [c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64,
+         c_int64, c_void_p, c_void_p],
     ),
 }
 

@@ -2,7 +2,7 @@
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
 ``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward`` / ``rnnt_features`` /
-``rnnt_features_backward``.
+``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -73,6 +73,8 @@ _LIB.define(
     "int out_frames, int pad_frames, int row_stride, bool with_mel) -> (Tensor, Tensor)"
 )
 _LIB.define("rnnt_features_backward(Tensor stats, float gain, Tensor mel, Tensor grad) -> Tensor")
+_LIB.define("inverse_mel(Tensor mel, Tensor plan, int n_stft) -> Tensor")
+_LIB.define("inverse_mel_backward(Tensor grad, Tensor mel, Tensor plan, int n_stft) -> Tensor")
 
 _KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
                "out_width", "out_col0", "use_log")
@@ -457,6 +459,42 @@ def _rnnt_features_backward_meta(stats, gain, mel, grad):
     return mel.new_empty(mel.shape)
 
 
+# ---- inverse_mel / inverse_mel_backward ----------------------------------------------------------------------------
+def _inverse_mel_cuda(mel, plan, n_stft):
+    """(rows, n_mels, T) mel spectrogram at any element strides -> (rows, T, n_stft) frame-major linear spectrogram."""
+    rows, n_mels, frames = mel.shape
+    dev = mel.device
+    ms = mel.stride()
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, n_stft), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_inverse_mel_run(plan.data_ptr(), n_stft, n_mels, mel.data_ptr(), rows, frames, ms[0], ms[1],
+                                              ms[2], out.data_ptr(), _stream(dev))
+    _lib.check(rc, "inverse_mel")
+    return out
+
+
+def _inverse_mel_meta(mel, plan, n_stft):
+    return mel.new_empty((mel.shape[0], mel.shape[2], n_stft))
+
+
+def _inverse_mel_backward_cuda(grad, mel, plan, n_stft):
+    """(rows, T, n_stft) output gradient at any element strides (0 included) -> (rows, T, n_mels) frame-major."""
+    rows, n_mels, frames = mel.shape
+    dev = mel.device
+    ms, gs = mel.stride(), grad.stride()
+    with torch.cuda.device(dev):
+        out = torch.empty((rows, frames, n_mels), dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_inverse_mel_backward(plan.data_ptr(), n_stft, n_mels, mel.data_ptr(), rows, frames, ms[0],
+                                                   ms[1], ms[2], grad.data_ptr(), gs[0], gs[1], gs[2], out.data_ptr(),
+                                                   _stream(dev))
+    _lib.check(rc, "inverse_mel_backward")
+    return out
+
+
+def _inverse_mel_backward_meta(grad, mel, plan, n_stft):
+    return mel.new_empty((mel.shape[0], mel.shape[2], mel.shape[1]))
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
@@ -471,7 +509,9 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("kaldi_backward", _kaldi_backward_cuda, _kaldi_backward_meta),
                             ("phase_vocoder_backward", _phase_vocoder_backward_cuda, _phase_vocoder_backward_meta),
                             ("rnnt_features", _rnnt_features_cuda, _rnnt_features_meta),
-                            ("rnnt_features_backward", _rnnt_features_backward_cuda, _rnnt_features_backward_meta)):
+                            ("rnnt_features_backward", _rnnt_features_backward_cuda, _rnnt_features_backward_meta),
+                            ("inverse_mel", _inverse_mel_cuda, _inverse_mel_meta),
+                            ("inverse_mel_backward", _inverse_mel_backward_cuda, _inverse_mel_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -490,3 +530,5 @@ kaldi_backward = torch.ops.b200audio.kaldi_backward
 phase_vocoder_backward = torch.ops.b200audio.phase_vocoder_backward
 rnnt_features = torch.ops.b200audio.rnnt_features
 rnnt_features_backward = torch.ops.b200audio.rnnt_features_backward
+inverse_mel = torch.ops.b200audio.inverse_mel
+inverse_mel_backward = torch.ops.b200audio.inverse_mel_backward

@@ -48,8 +48,8 @@ def is_resample_differentiable() -> bool:
 
 
 def is_feature_differentiable() -> bool:
-    """Whether MFCC, LFCC, AmplitudeToDB, MelScale, SpectralCentroid and pipelines.RNNTFeatureExtractor accept inputs
-    that require grad (in this thread)."""
+    """Whether MFCC, LFCC, AmplitudeToDB, MelScale, InverseMelScale, SpectralCentroid and pipelines.RNNTFeatureExtractor
+    accept inputs that require grad (in this thread)."""
     return getattr(_GRAD_STATE, "features", False)
 
 
@@ -70,8 +70,8 @@ def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = Fa
     """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
     ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT, ``resample=True``
     (with ``mode``) the waveform gradients of the resampler, ``features=True`` (with ``mode``) the input gradients of
-    MFCC, LFCC, AmplitudeToDB, MelScale, SpectralCentroid and the RNN-T feature extractor, ``kaldi=True`` (with ``mode``) the waveform gradients of
-    the Kaldi spectrogram, fbank and mfcc, ``vocoder=True`` (with ``mode``) the spectrogram gradients of the phase
+    MFCC, LFCC, AmplitudeToDB, MelScale, InverseMelScale, SpectralCentroid and the RNN-T feature extractor,
+    ``kaldi=True`` (with ``mode``) the waveform gradients of the Kaldi spectrogram, fbank and mfcc, ``vocoder=True`` (with ``mode``) the spectrogram gradients of the phase
     vocoder and TimeStretch and the waveform gradients of PitchShift.  They are separate switches so that vocoder
     inference, augmentation code (Speed, SpeedPerturbation, TimeStretch, PitchShift) and Kaldi feature preprocessing in
     data pipelines do not build graphs when loss gradients are on, and so that the top_db clamp's gradient -- every
@@ -129,8 +129,8 @@ def _no_autograd(t: torch.Tensor) -> None:
             "waveform gradients inside audio_b200.differentiable(); InverseSpectrogram and F.inverse_spectrogram "
             "compute spectrogram gradients inside audio_b200.differentiable(inverse=True); Resample, F.resample, Speed "
             "and SpeedPerturbation compute waveform gradients inside audio_b200.differentiable(resample=True); MFCC, LFCC, "
-            "AmplitudeToDB, MelScale, SpectralCentroid and pipelines.RNNTFeatureExtractor compute input gradients inside "
-            "audio_b200.differentiable(features=True); compliance.kaldi spectrogram, fbank and mfcc compute waveform "
+            "AmplitudeToDB, MelScale, InverseMelScale, SpectralCentroid and pipelines.RNNTFeatureExtractor compute input "
+            "gradients inside audio_b200.differentiable(features=True); compliance.kaldi spectrogram, fbank and mfcc compute waveform "
             "gradients inside audio_b200.differentiable(kaldi=True); F.phase_vocoder and TimeStretch compute spectrogram "
             "gradients, F.pitch_shift and PitchShift waveform gradients, inside audio_b200.differentiable(vocoder=True).)"
         )
@@ -392,6 +392,70 @@ class FrontendPlan:
         if self._desc_lists is None:
             self._desc_lists = _ops.pack_desc(self.desc)
         return self._desc_lists
+
+
+_RANK_MESSAGE = ("torch.linalg.lstsq: The least squares solution could not be computed because the input matrix does not "
+                 "have full rank (error code: {}).")
+
+
+class InverseMelPlan:
+    """InverseMelScale's banded L D L^T factorisation of G = fb^T fb (b200a_inverse_mel_plan) on fb's device.  Built on
+    the host from one device-to-host copy of ``fb`` and uploaded once; rebuilt only when ``fb`` changes, by the stamp
+    rule of :meth:`FrontendPlan.workspace`.  The errors of the reference's ``lstsq`` are raised here, at ``forward``."""
+
+    def __init__(self, driver: str):
+        self.driver = driver
+        self._plan: Optional[torch.Tensor] = None
+        self._stamp = None
+        self._held = None  # the fb behind the stamp (see FrontendPlan._held)
+
+    def plan(self, fb: torch.Tensor) -> torch.Tensor:
+        stamp = (fb.data_ptr(), _version_of(fb), str(fb.device))
+        if self._plan is not None and stamp == self._stamp:
+            return self._plan
+        import ctypes
+
+        lib = _lib.lib()
+        n_stft, n_mels = fb.shape
+        nbytes = lib.b200a_inverse_mel_plan_bytes(n_stft, n_mels)
+        blob = torch.zeros(nbytes, dtype=torch.uint8)
+        fb_host = fb.detach().to("cpu").contiguous()
+        bw, pivot = ctypes.c_int32(), ctypes.c_int32()
+        rc = lib.b200a_inverse_mel_plan(fb_host.data_ptr(), n_stft, n_mels, _lib.LSTSQ_DRIVER[self.driver], blob.data_ptr(),
+                                        nbytes, ctypes.byref(bw), ctypes.byref(pivot))
+        if rc == _lib.ESINGULAR and self.driver == "gels":
+            raise torch.linalg.LinAlgError(_RANK_MESSAGE.format(pivot.value + 1))
+        if rc == _lib.ESINGULAR:
+            raise RuntimeError(
+                f"audio_b200: InverseMelScale(driver={self.driver!r}) on a rank-deficient filterbank (first zero pivot at "
+                f"filter {pivot.value} of fb{tuple(fb.shape)}) is not supported: the rank-revealing drivers return "
+                "different answers there; drop the empty filters or use driver='gels', which raises as the reference does")
+        if rc == _lib.EUNSUPPORTED:
+            raise RuntimeError(
+                f"audio_b200: InverseMelScale with fb{tuple(fb.shape)} is not supported: it needs n_mels <= n_stft "
+                f"(an underdetermined system), n_mels <= {_lib.INVERSE_MEL_MAX_MELS} and a Gram bandwidth <= "
+                f"{_lib.INVERSE_MEL_MAX_BANDWIDTH} (this bank: {bw.value})")
+        _lib.check(rc, "inverse_mel_plan")
+        self._plan, self._stamp, self._held = blob.to(fb.device), stamp, fb
+        return self._plan
+
+
+class _InverseMelFunction(torch.autograd.Function):
+    """b200audio::inverse_mel on the packed (rows, n_mels, T) mel spectrogram, with b200audio::inverse_mel_backward as its
+    backward.  The mel input goes through save_for_backward (in-place edits are detected); the forward's plan is kept,
+    so an fb changed before backward does not change the gradient."""
+
+    @staticmethod
+    def forward(ctx, m3, plan, n_stft):
+        ctx.save_for_backward(m3)
+        ctx.plan, ctx.n_stft = plan, n_stft
+        return _ops.inverse_mel(m3, plan, n_stft)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (m3,) = ctx.saved_tensors
+        return _ops.inverse_mel_backward(g, m3, ctx.plan, ctx.n_stft).transpose(1, 2), None, None
 
 
 def new_group_max(groups: int, device: torch.device) -> torch.Tensor:

@@ -18,6 +18,7 @@ const char* b200a_strerror(int status) {
     case B200A_ESHORT: return "signal too short for this n_fft / padding mode";
     case B200A_EWORKSPACE: return "workspace too small or not prepared";
     case B200A_ECUDA: return "CUDA launch failed";
+    case B200A_ESINGULAR: return "rank-deficient system (singular Gram matrix)";
     default: return "unknown status";
   }
 }
@@ -458,6 +459,27 @@ int b200a_resample_backward(const void* workspace, int32_t orig_r, int32_t new_r
   if (length == 0) return B200A_OK;
   return resample_backward_impl(workspace, orig_r, new_r, width, grad, rows, g_row_stride, out_len, grad_wave, length,
                                 grad_row_stride, static_cast<cudaStream_t>(stream));
+}
+
+size_t b200a_inverse_mel_plan_bytes(int32_t n_stft, int32_t n_mels) { return inverse_mel_plan_bytes_impl(n_stft, n_mels); }
+
+int b200a_inverse_mel_plan(const float* fb, int32_t n_stft, int32_t n_mels, int32_t driver, void* plan, size_t plan_bytes,
+                           int32_t* bandwidth, int32_t* pivot) {
+  return inverse_mel_plan_impl(fb, n_stft, n_mels, driver, plan, plan_bytes, bandwidth, pivot);
+}
+
+int b200a_inverse_mel_run(const void* plan, int32_t n_stft, int32_t n_mels, const float* mel, int64_t rows, int64_t frames,
+                          int64_t stride_row, int64_t stride_mel, int64_t stride_frame, float* out, b200a_stream stream) {
+  return inverse_mel_run_impl(plan, n_stft, n_mels, mel, rows, frames, stride_row, stride_mel, stride_frame, out,
+                              static_cast<cudaStream_t>(stream));
+}
+
+int b200a_inverse_mel_backward(const void* plan, int32_t n_stft, int32_t n_mels, const float* mel, int64_t rows,
+                               int64_t frames, int64_t stride_row, int64_t stride_mel, int64_t stride_frame,
+                               const float* grad, int64_t g_stride_row, int64_t g_stride_frame, int64_t g_stride_bin,
+                               float* grad_mel, b200a_stream stream) {
+  return inverse_mel_backward_impl(plan, n_stft, n_mels, mel, rows, frames, stride_row, stride_mel, stride_frame, grad,
+                                   g_stride_row, g_stride_frame, g_stride_bin, grad_mel, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

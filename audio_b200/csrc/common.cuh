@@ -154,6 +154,15 @@ int frontend_backward_impl(const b200a_frontend_desc* d, const void* ws, int sta
                            int64_t length, int64_t row_stride, int64_t frames, const float* grad, int64_t gs_row,
                            int64_t gs_frame, int64_t gs_col, void* scratch, float* grad_wave, int64_t grad_row_stride,
                            cudaStream_t stream);
+// inverse_mel.cu
+size_t inverse_mel_plan_bytes_impl(int64_t n_stft, int64_t n_mels);
+int inverse_mel_plan_impl(const float* fb, int32_t n_stft, int32_t n_mels, int32_t driver, void* plan, size_t plan_bytes,
+                          int32_t* bandwidth, int32_t* pivot);
+int inverse_mel_run_impl(const void* plan, int32_t n_stft, int32_t n_mels, const float* mel, int64_t rows, int64_t frames,
+                         int64_t s_row, int64_t s_mel, int64_t s_frame, float* out, cudaStream_t stream);
+int inverse_mel_backward_impl(const void* plan, int32_t n_stft, int32_t n_mels, const float* mel, int64_t rows,
+                              int64_t frames, int64_t s_row, int64_t s_mel, int64_t s_frame, const float* grad,
+                              int64_t g_row, int64_t g_frame, int64_t g_bin, float* grad_mel, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

@@ -2,8 +2,8 @@
 
 Class names, constructor signatures, attribute / buffer / sub-module names and error
 behaviour follow pytorch/audio/src/torchaudio/transforms/_transforms.py
-(Spectrogram 25-123, AmplitudeToDB 300-346, MelScale 349-415, MelSpectrogram 506-622,
-MFCC 625-709, Resample 899-980), so ``state_dict``s interchange with torchaudio's and
+(Spectrogram 25-123, AmplitudeToDB 300-346, MelScale 349-415, InverseMelScale 418-503,
+MelSpectrogram 506-622, MFCC 625-709, Resample 899-980), so ``state_dict``s interchange with torchaudio's and
 existing call sites keep working after ``import audio_b200.transforms as T``.
 
 ``forward`` launches hand-written sm_90a kernels through the C ABI; MelSpectrogram and MFCC
@@ -12,7 +12,7 @@ spectrum through HBM) -- they read the sub-modules' buffers and launch the fused
 
 Gradients are opt-in, per thread: Spectrogram and MelSpectrogram inside ``audio_b200.differentiable()``,
 InverseSpectrogram with ``inverse=True``, Resample / Speed / SpeedPerturbation with ``resample=True``, and MFCC,
-LFCC, AmplitudeToDB, MelScale and SpectralCentroid with ``features=True``, the Kaldi features
+LFCC, AmplitudeToDB, MelScale, InverseMelScale and SpectralCentroid with ``features=True``, the Kaldi features
 (``audio_b200.compliance.kaldi``) with ``kaldi=True``, and TimeStretch (spectrogram gradient) and PitchShift
 (waveform gradient) with ``vocoder=True``.  GriffinLim is forward-only.
 """
@@ -25,12 +25,13 @@ from typing import Callable, Optional, Union
 import torch
 from torch import Tensor
 
-from . import _lib
+from . import _lib, _ops
 from . import functional as F
-from ._plans import FrontendPlan, ResamplePlan, vocoder_chain
+from ._plans import (FrontendPlan, InverseMelPlan, ResamplePlan, _InverseMelFunction, _no_autograd, _require_cuda_f32,
+                     _wants_grad, is_feature_differentiable, vocoder_chain)
 
-__all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "MelSpectrogram", "MFCC", "LFCC", "SpectralCentroid", "Resample",
-           "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift"]
+__all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "InverseMelScale", "MelSpectrogram", "MFCC", "LFCC",
+           "SpectralCentroid", "Resample", "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift"]
 
 
 def _setup_framing(mod, n_fft, win_length, hop_length, window_fn=None, wkwargs=None, hop_div=2):
@@ -224,6 +225,63 @@ class MelScale(torch.nn.Module):
 
     def forward(self, specgram: Tensor) -> Tensor:
         return F._apply_fbank(specgram, self.fb)
+
+
+class InverseMelScale(torch.nn.Module):
+    r"""Estimate a linear-frequency spectrogram from a mel spectrogram (reference _transforms.py:418-503):
+    ``(..., n_mels, time) -> (..., n_stft, time)``; buffer ``fb``.
+
+    The reference returns ``relu(lstsq(fb^T, melspec, driver).solution)``.  For ``n_mels <= n_stft`` and a nonsingular
+    Gram matrix ``G = fb^T fb`` every driver gives the minimum-norm solution ``relu(fb G^-1 m)``; ``G`` of a mel bank is
+    banded (tridiagonal), so each frame is one banded solve (factored once per ``fb`` version, in double precision on
+    the host) and a <= 2-tap expansion, in one kernel.  The output is a transposed view of a frame-major tensor, the
+    strides the reference returns.  A singular ``G`` raises ``torch.linalg.LinAlgError`` with ``driver="gels"``, as the
+    reference does, and a "not supported" error with the rank-revealing drivers; so do ``n_mels > n_stft`` banks except
+    where gels fails.  Inside ``audio_b200.differentiable(features=True)`` the mel spectrogram gets its gradient.
+    """
+
+    __constants__ = ["n_stft", "n_mels", "sample_rate", "f_min", "f_max"]
+
+    def __init__(
+        self,
+        n_stft: int,
+        n_mels: int = 128,
+        sample_rate: int = 16000,
+        f_min: float = 0.0,
+        f_max: Optional[float] = None,
+        norm: Optional[str] = None,
+        mel_scale: str = "htk",
+        driver: str = "gels",
+    ) -> None:
+        super().__init__()
+        self.n_mels = n_mels
+        self.sample_rate = sample_rate
+        self.f_max = f_max or float(sample_rate // 2)
+        self.f_min = f_min
+        self.driver = driver
+        if f_min > self.f_max:
+            raise ValueError("Require f_min: {} <= f_max: {}".format(f_min, self.f_max))
+        if driver not in ["gels", "gelsy", "gelsd", "gelss"]:
+            raise ValueError(f'driver must be one of ["gels", "gelsy", "gelsd", "gelss"]. Found {driver}.')
+        fb = F.melscale_fbanks(n_stft, self.f_min, self.f_max, self.n_mels, self.sample_rate, norm, mel_scale)
+        self.register_buffer("fb", fb)
+        self._plan = InverseMelPlan(driver)
+
+    def forward(self, melspec: Tensor) -> Tensor:
+        shape = melspec.size()
+        n_mels, time = shape[-2], shape[-1]
+        if self.n_mels != n_mels:
+            raise ValueError("Expected an input with {} mel bins. Found: {}".format(self.n_mels, n_mels))
+        _require_cuda_f32(melspec, "melspec")
+        _require_cuda_f32(self.fb, "fb")
+        grad = _wants_grad(melspec, (("fb", self.fb),), is_feature_differentiable, "mel spectrogram")
+        if not grad:
+            _no_autograd(melspec)
+        n_stft = self.fb.shape[0]
+        plan = self._plan.plan(self.fb)
+        m3 = melspec.reshape(-1, n_mels, time)
+        out = _InverseMelFunction.apply(m3, plan, n_stft) if grad else _ops.inverse_mel(m3, plan, n_stft)
+        return out.reshape(shape[:-2] + (time, n_stft)).transpose(-1, -2)
 
 
 class MelSpectrogram(torch.nn.Module):

@@ -46,7 +46,8 @@ enum b200a_status {
   B200A_EUNSUPPORTED = -2, /* valid in the reference, not implemented here (documented) */
   B200A_ESHORT = -3,       /* signal too short: reflect/circular pad needs n_fft/2 < length, or < n_fft samples */
   B200A_EWORKSPACE = -4,   /* workspace too small / not prepared for this descriptor */
-  B200A_ECUDA = -5         /* CUDA runtime reported an error at launch (cudaGetLastError) */
+  B200A_ECUDA = -5,        /* CUDA runtime reported an error at launch (cudaGetLastError) */
+  B200A_ESINGULAR = -6     /* the system is rank-deficient (b200a_inverse_mel_plan: singular Gram matrix) */
 };
 
 enum b200a_pad_mode { /* torch.nn.functional.pad modes accepted by torch.stft(center=True) */
@@ -440,6 +441,55 @@ size_t b200a_kaldi_backward_scratch_bytes(const b200a_kaldi_desc* kaldi, const b
 
 /* x[r][t][c] -= mean_t x[r][t][c], in place, for each of `rows` feature matrices (_subtract_column_mean, :219-226). */
 int b200a_subtract_column_mean(float* x, int64_t rows, int64_t frames, int64_t width, b200a_stream stream);
+
+/* ---- InverseMelScale (transforms/_transforms.py:418-503) ------------------------------------------------------- */
+/*
+ * x = relu(lstsq(fb^T, m).solution) per frame.  For n_mels <= n_stft and a nonsingular Gram matrix G = fb^T fb every
+ * LAPACK driver returns the minimum-norm solution x = relu(fb G^-1 m).  A bin of a mel (or linear) bank overlaps at most
+ * two adjacent filters, so G is banded; the plan factors it as banded L D L^T.
+ */
+#define B200A_INVERSE_MEL_MAX_BANDWIDTH 4 /* Gram bandwidth cap (mel and LFCC linear banks have 1) */
+#define B200A_INVERSE_MEL_MAX_MELS 512    /* n_mels cap: the backward stages two 32-frame tiles in shared memory */
+enum b200a_lstsq_driver { B200A_GELS = 0, B200A_GELSY = 1, B200A_GELSD = 2, B200A_GELSS = 3 };
+
+/* Bytes of the plan blob for this size (its layout depends on n_stft and n_mels alone); 0 for non-positive sizes. */
+size_t b200a_inverse_mel_plan_bytes(int32_t n_stft, int32_t n_mels);
+/*
+ * HOST-only: build the plan from a HOST copy of fb ([n_stft][n_mels], row-major float32; the caller copies it from the
+ * device once per fb version and uploads the blob once).  In double precision: each bin's nonzero filter span and each
+ * filter's nonzero bin span (read from fb, any bank), the Gram bandwidth, then G = L D L^T; stored as float32 factors
+ * (L, 1/D), the per-bin table (first filter, count, fb values) and the per-filter table (first bin, count).
+ *   plan      : HOST buffer of b200a_inverse_mel_plan_bytes(n_stft, n_mels) bytes (B200A_EWORKSPACE if smaller)
+ *   bandwidth : out, the Gram bandwidth found (-1 if not reached)
+ *   pivot     : out, the first zero pivot (0-based filter) on B200A_ESINGULAR, or for an overdetermined bank with gels
+ *               the first empty bin; else -1
+ * Returns B200A_ESINGULAR for a singular G (n_mels <= n_stft; the gels driver fails there too) and for n_mels > n_stft
+ * with B200A_GELS and an all-zero bin; B200A_EUNSUPPORTED for any other n_mels > n_stft, a bandwidth above
+ * B200A_INVERSE_MEL_MAX_BANDWIDTH or n_mels above B200A_INVERSE_MEL_MAX_MELS; B200A_EINVAL for null pointers,
+ * non-positive sizes or a bad driver.
+ */
+int b200a_inverse_mel_plan(const float* fb, int32_t n_stft, int32_t n_mels, int32_t driver, void* plan, size_t plan_bytes,
+                           int32_t* bandwidth, int32_t* pivot);
+/*
+ * out[r][t][k] = relu(sum_m fb[k][m] z[r][t][m]),  G z[r][t] = mel[r][:, t]  (one banded solve per frame, FP32)
+ *   plan : the blob of b200a_inverse_mel_plan in DEVICE memory
+ *   mel  : logical [rows][n_mels][frames] at element strides (the frame-major view MelSpectrogram returns and a
+ *          contiguous tensor both load coalesced)
+ *   out  : FRAME-MAJOR [rows][frames][n_stft], every element written
+ */
+int b200a_inverse_mel_run(const void* plan, int32_t n_stft, int32_t n_mels, const float* mel, int64_t rows, int64_t frames,
+                          int64_t stride_row, int64_t stride_mel, int64_t stride_frame, float* out, b200a_stream stream);
+/*
+ * Mel gradient of b200a_inverse_mel_run: z and the pre-relu values are recomputed by the forward's code (the relu mask
+ * is bit-identical to the forward's), u[m] = sum_{k in filter m} fb[k][m] [x_k > 0] g[k] in a fixed order, then
+ * grad_mel = G^-1 u with the same factors.  No atomics: reruns are bit-identical.
+ *   grad     : logical [rows][frames][n_stft] at element strides (0 allowed: expanded gradients)
+ *   grad_mel : FRAME-MAJOR [rows][frames][n_mels], every element written
+ */
+int b200a_inverse_mel_backward(const void* plan, int32_t n_stft, int32_t n_mels, const float* mel, int64_t rows,
+                               int64_t frames, int64_t stride_row, int64_t stride_mel, int64_t stride_frame,
+                               const float* grad, int64_t g_stride_row, int64_t g_stride_frame, int64_t g_stride_bin,
+                               float* grad_mel, b200a_stream stream);
 
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */

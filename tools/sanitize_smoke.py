@@ -45,6 +45,10 @@ with audio_b200.differentiable(features=True):  # feature gradients: MFCC clamp 
         mod.cuda()(xin.clone().requires_grad_()).sum().backward()
     spec = T.Spectrogram(n_fft=400).cuda()(x).requires_grad_()
     T.AmplitudeToDB(top_db=0.0)(T.MelScale(40, 16000, n_stft=201).cuda()(spec)).sum().backward()
+    # InverseMelScale forward + backward: a frame-major input with a partial last tile, a contiguous 2-D one
+    mel = T.MelSpectrogram(16000, n_fft=512, hop_length=128, n_mels=40, power=1.0).cuda()(x).requires_grad_()
+    T.InverseMelScale(257, 40, 16000).cuda()(mel).sum().backward()
+    T.InverseMelScale(257, 40, 16000).cuda()(mel.detach()[0].contiguous().requires_grad_()).sum().backward()
 T.MFCC(16000, n_mfcc=13, melkwargs=dict(n_fft=512, hop_length=160, n_mels=40)).cuda()(x)
 T.MFCC(16000, n_mfcc=40, melkwargs=dict(n_fft=1024, hop_length=256, n_mels=80)).cuda()(x.reshape(1, 3, -1))
 for kw in (dict(num_mel_bins=40, snip_edges=False, use_energy=True), dict(num_mel_bins=23), dict(frame_length=20.0, round_to_power_of_two=False)):
