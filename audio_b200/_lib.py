@@ -20,6 +20,7 @@ PAD_MODE = {"reflect": 0, "constant": 1, "replicate": 2, "circular": 3}
 STAGE_COMPLEX, STAGE_POWER, STAGE_MEL, STAGE_FEAT = 0, 1, 2, 3
 LSTSQ_DRIVER = {"gels": 0, "gelsy": 1, "gelsd": 2, "gelss": 3}
 INVERSE_MEL_MAX_BANDWIDTH, INVERSE_MEL_MAX_MELS = 4, 512  # B200A_INVERSE_MEL_MAX_BANDWIDTH / _MAX_MELS
+LFILTER_MAX_ORDER = 16  # B200A_LFILTER_MAX_ORDER
 
 
 class FrontendDesc(ctypes.Structure):
@@ -191,6 +192,18 @@ _SIGNATURES = {
         ctypes.c_int,
         [c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64,
          c_int64, c_void_p, c_void_p],
+    ),
+    "b200a_lfilter_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32, c_int32]),
+    "b200a_lfilter_backward_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32, c_int32]),
+    "b200a_lfilter_run": (
+        ctypes.c_int,
+        [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int32, c_int32, c_void_p,
+         c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_lfilter_backward": (
+        ctypes.c_int,
+        [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32,
+         c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
     ),
 }
 

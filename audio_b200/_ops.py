@@ -2,7 +2,7 @@
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
 ``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward`` / ``rnnt_features`` /
-``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward``.
+``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward`` / ``lfilter`` / ``lfilter_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -75,6 +75,11 @@ _LIB.define(
 _LIB.define("rnnt_features_backward(Tensor stats, float gain, Tensor mel, Tensor grad) -> Tensor")
 _LIB.define("inverse_mel(Tensor mel, Tensor plan, int n_stft) -> Tensor")
 _LIB.define("inverse_mel_backward(Tensor grad, Tensor mel, Tensor plan, int n_stft) -> Tensor")
+_LIB.define("lfilter(Tensor x, Tensor a, Tensor b, bool clamp, bool reverse, bool with_raw) -> (Tensor, Tensor)")
+_LIB.define(
+    "lfilter_backward(Tensor grad, Tensor x, Tensor y_raw, Tensor a, Tensor b, bool clamp, bool reverse) "
+    "-> (Tensor, Tensor, Tensor)"
+)
 
 _KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
                "out_width", "out_col0", "use_log")
@@ -495,6 +500,61 @@ def _inverse_mel_backward_meta(grad, mel, plan, n_stft):
     return mel.new_empty((mel.shape[0], mel.shape[2], mel.shape[1]))
 
 
+# ---- lfilter / lfilter_backward ---------------------------------------------------------------------------------
+def _lfilter_strides(x):
+    """Batch and filter element strides of a (batch, n_filters, T) input with a unit (or irrelevant) time stride."""
+    return x.stride(0), x.stride(1)
+
+
+def _lfilter_cuda(x, a, b, clamp, reverse, with_raw):
+    """(batch, n_filters, T) waveform rows at any batch / filter strides (0 included), unit time stride, and
+    (n_filters, n_order) contiguous coefficients -> (y, unclamped y or an empty tensor), both contiguous."""
+    batch, n_filters, length = x.shape
+    n_order = a.shape[1]
+    dev = x.device
+    lib = _lib.lib()
+    sb, sf = _lfilter_strides(x)
+    with torch.cuda.device(dev):
+        y = torch.empty((batch, n_filters, length), dtype=torch.float32, device=dev)
+        raw = torch.empty((batch, n_filters, length) if with_raw else (0,), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_lfilter_workspace_bytes(batch * n_filters, length, n_order, n_filters)
+        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        rc = lib.b200a_lfilter_run(a.data_ptr(), b.data_ptr(), n_filters, n_order, x.data_ptr(), batch, length, sb, sf,
+                                   int(clamp), int(reverse), y.data_ptr(), raw.data_ptr() if with_raw else None,
+                                   ws.data_ptr(), nbytes, _stream(dev))
+    _lib.check(rc, "lfilter")
+    return y, raw
+
+
+def _lfilter_meta(x, a, b, clamp, reverse, with_raw):
+    return x.new_empty(x.shape), x.new_empty(x.shape if with_raw else (0,))
+
+
+def _lfilter_backward_cuda(grad, x, y_raw, a, b, clamp, reverse):
+    """Upstream gradient of the (batch, n_filters, T) output -> (grad_x (batch, n_filters, T), grad_a, grad_b)."""
+    batch, n_filters, length = x.shape
+    n_order = a.shape[1]
+    grad = grad.contiguous()
+    dev = x.device
+    lib = _lib.lib()
+    sb, sf = _lfilter_strides(x)
+    with torch.cuda.device(dev):
+        gx = torch.empty((batch, n_filters, length), dtype=torch.float32, device=dev)
+        ga = torch.empty((n_filters, n_order), dtype=torch.float32, device=dev)
+        gb = torch.empty((n_filters, n_order), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_lfilter_backward_workspace_bytes(batch * n_filters, length, n_order, n_filters)
+        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        rc = lib.b200a_lfilter_backward(a.data_ptr(), b.data_ptr(), n_filters, n_order, x.data_ptr(), batch, length, sb,
+                                        sf, y_raw.data_ptr(), grad.data_ptr(), int(clamp), int(reverse), gx.data_ptr(),
+                                        ga.data_ptr(), gb.data_ptr(), ws.data_ptr(), nbytes, _stream(dev))
+    _lib.check(rc, "lfilter_backward")
+    return gx, ga, gb
+
+
+def _lfilter_backward_meta(grad, x, y_raw, a, b, clamp, reverse):
+    return x.new_empty(x.shape), a.new_empty(a.shape), b.new_empty(b.shape)
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
@@ -511,7 +571,9 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("rnnt_features", _rnnt_features_cuda, _rnnt_features_meta),
                             ("rnnt_features_backward", _rnnt_features_backward_cuda, _rnnt_features_backward_meta),
                             ("inverse_mel", _inverse_mel_cuda, _inverse_mel_meta),
-                            ("inverse_mel_backward", _inverse_mel_backward_cuda, _inverse_mel_backward_meta)):
+                            ("inverse_mel_backward", _inverse_mel_backward_cuda, _inverse_mel_backward_meta),
+                            ("lfilter", _lfilter_cuda, _lfilter_meta),
+                            ("lfilter_backward", _lfilter_backward_cuda, _lfilter_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -532,3 +594,5 @@ rnnt_features = torch.ops.b200audio.rnnt_features
 rnnt_features_backward = torch.ops.b200audio.rnnt_features_backward
 inverse_mel = torch.ops.b200audio.inverse_mel
 inverse_mel_backward = torch.ops.b200audio.inverse_mel_backward
+lfilter = torch.ops.b200audio.lfilter
+lfilter_backward = torch.ops.b200audio.lfilter_backward

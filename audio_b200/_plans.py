@@ -65,14 +65,21 @@ def is_vocoder_differentiable() -> bool:
     return getattr(_GRAD_STATE, "vocoder", False)
 
 
+def is_filtering_differentiable() -> bool:
+    """Whether F.lfilter, F.filtfilt, the ``*_biquad`` filters, F.deemphasis, F.preemphasis, Preemphasis and
+    Deemphasis accept waveforms and coefficients that require grad (in this thread)."""
+    return getattr(_GRAD_STATE, "filtering", False)
+
+
 def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = False, features: bool = False,
-                       kaldi: bool = False, vocoder: bool = False) -> None:
+                       kaldi: bool = False, vocoder: bool = False, filtering: bool = False) -> None:
     """Turn waveform gradients on or off for the calling thread (off by default, like a fresh thread's grad mode).
     ``inverse=True`` (with ``mode``) also turns on the spectrogram gradients of the inverse STFT, ``resample=True``
     (with ``mode``) the waveform gradients of the resampler, ``features=True`` (with ``mode``) the input gradients of
     MFCC, LFCC, AmplitudeToDB, MelScale, InverseMelScale, SpectralCentroid and the RNN-T feature extractor,
     ``kaldi=True`` (with ``mode``) the waveform gradients of the Kaldi spectrogram, fbank and mfcc, ``vocoder=True`` (with ``mode``) the spectrogram gradients of the phase
-    vocoder and TimeStretch and the waveform gradients of PitchShift.  They are separate switches so that vocoder
+    vocoder and TimeStretch and the waveform gradients of PitchShift, ``filtering=True`` (with ``mode``) the waveform
+    and coefficient gradients of lfilter, filtfilt, the biquads and pre-/de-emphasis.  They are separate switches so that vocoder
     inference, augmentation code (Speed, SpeedPerturbation, TimeStretch, PitchShift) and Kaldi feature preprocessing in
     data pipelines do not build graphs when loss gradients are on, and so that the top_db clamp's gradient -- every
     clamped element's share goes to the group maximum -- is opted into knowingly."""
@@ -82,23 +89,26 @@ def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = Fa
     _GRAD_STATE.features = bool(mode) and bool(features)
     _GRAD_STATE.kaldi = bool(mode) and bool(kaldi)
     _GRAD_STATE.vocoder = bool(mode) and bool(vocoder)
+    _GRAD_STATE.filtering = bool(mode) and bool(filtering)
 
 
 def _switches():
     return (is_differentiable(), is_inverse_differentiable(), is_resample_differentiable(), is_feature_differentiable(),
-            is_kaldi_differentiable(), is_vocoder_differentiable())
+            is_kaldi_differentiable(), is_vocoder_differentiable(), is_filtering_differentiable())
 
 
 def _restore(prev) -> None:
-    set_differentiable(prev[0], inverse=prev[1], resample=prev[2], features=prev[3], kaldi=prev[4], vocoder=prev[5])
+    set_differentiable(prev[0], inverse=prev[1], resample=prev[2], features=prev[3], kaldi=prev[4], vocoder=prev[5],
+                       filtering=prev[6])
 
 
 @contextlib.contextmanager
 def differentiable(mode: bool = True, *, inverse: bool = False, resample: bool = False, features: bool = False,
-                   kaldi: bool = False, vocoder: bool = False):
+                   kaldi: bool = False, vocoder: bool = False, filtering: bool = False):
     """Context manager form of :func:`set_differentiable`; restores the previous settings on exit."""
     prev = _switches()
-    set_differentiable(mode, inverse=inverse, resample=resample, features=features, kaldi=kaldi, vocoder=vocoder)
+    set_differentiable(mode, inverse=inverse, resample=resample, features=features, kaldi=kaldi, vocoder=vocoder,
+                       filtering=filtering)
     try:
         yield
     finally:
@@ -114,7 +124,8 @@ def vocoder_chain(waveform: torch.Tensor):
         yield
         return
     prev = _switches()
-    set_differentiable(True, inverse=True, resample=True, features=prev[3], kaldi=prev[4], vocoder=True)
+    set_differentiable(True, inverse=True, resample=True, features=prev[3], kaldi=prev[4], vocoder=True,
+                       filtering=prev[6])
     try:
         yield
     finally:
@@ -132,7 +143,9 @@ def _no_autograd(t: torch.Tensor) -> None:
             "AmplitudeToDB, MelScale, InverseMelScale, SpectralCentroid and pipelines.RNNTFeatureExtractor compute input "
             "gradients inside audio_b200.differentiable(features=True); compliance.kaldi spectrogram, fbank and mfcc compute waveform "
             "gradients inside audio_b200.differentiable(kaldi=True); F.phase_vocoder and TimeStretch compute spectrogram "
-            "gradients, F.pitch_shift and PitchShift waveform gradients, inside audio_b200.differentiable(vocoder=True).)"
+            "gradients, F.pitch_shift and PitchShift waveform gradients, inside audio_b200.differentiable(vocoder=True); F.lfilter, "
+            "F.filtfilt, the *_biquad filters, F.preemphasis, F.deemphasis, Preemphasis and Deemphasis compute waveform and "
+            "coefficient gradients inside audio_b200.differentiable(filtering=True).)"
         )
 
 

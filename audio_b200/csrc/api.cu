@@ -482,5 +482,29 @@ int b200a_inverse_mel_backward(const void* plan, int32_t n_stft, int32_t n_mels,
                                    g_stride_row, g_stride_frame, g_stride_bin, grad_mel, static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_lfilter_workspace_bytes(int64_t rows, int64_t length, int32_t n_order, int32_t n_filters) {
+  return lfilter_workspace_bytes_impl(rows, length, n_order, n_filters, false);
+}
+
+size_t b200a_lfilter_backward_workspace_bytes(int64_t rows, int64_t length, int32_t n_order, int32_t n_filters) {
+  return lfilter_workspace_bytes_impl(rows, length, n_order, n_filters, true);
+}
+
+int b200a_lfilter_run(const float* a, const float* b, int32_t n_filters, int32_t n_order, const float* x, int64_t batch,
+                      int64_t length, int64_t stride_batch, int64_t stride_filter, int32_t clamp, int32_t reverse,
+                      float* y, float* y_unclamped, void* workspace, size_t workspace_bytes, b200a_stream stream) {
+  return lfilter_run_impl(a, b, n_filters, n_order, x, batch, length, stride_batch, stride_filter, clamp != 0,
+                          reverse != 0, y, y_unclamped, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int b200a_lfilter_backward(const float* a, const float* b, int32_t n_filters, int32_t n_order, const float* x,
+                           int64_t batch, int64_t length, int64_t stride_batch, int64_t stride_filter,
+                           const float* y_unclamped, const float* grad, int32_t clamp, int32_t reverse, float* grad_x,
+                           float* grad_a, float* grad_b, void* workspace, size_t workspace_bytes, b200a_stream stream) {
+  return lfilter_backward_impl(a, b, n_filters, n_order, x, batch, length, stride_batch, stride_filter, y_unclamped,
+                               grad, clamp != 0, reverse != 0, grad_x, grad_a, grad_b, workspace, workspace_bytes,
+                               static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

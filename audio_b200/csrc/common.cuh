@@ -163,6 +163,15 @@ int inverse_mel_run_impl(const void* plan, int32_t n_stft, int32_t n_mels, const
 int inverse_mel_backward_impl(const void* plan, int32_t n_stft, int32_t n_mels, const float* mel, int64_t rows,
                               int64_t frames, int64_t s_row, int64_t s_mel, int64_t s_frame, const float* grad,
                               int64_t g_row, int64_t g_frame, int64_t g_bin, float* grad_mel, cudaStream_t stream);
+// lfilter.cu
+size_t lfilter_workspace_bytes_impl(int64_t rows, int64_t length, int n_order, int n_filters, bool backward);
+int lfilter_run_impl(const float* a, const float* b, int n_filters, int n_order, const float* x, int64_t batch,
+                     int64_t length, int64_t s_batch, int64_t s_filter, bool clamp, bool reverse, float* y,
+                     float* y_raw, void* ws, size_t ws_bytes, cudaStream_t stream);
+int lfilter_backward_impl(const float* a, const float* b, int n_filters, int n_order, const float* x, int64_t batch,
+                          int64_t length, int64_t s_batch, int64_t s_filter, const float* y_raw, const float* grad,
+                          bool clamp, bool reverse, float* grad_x, float* grad_a, float* grad_b, void* ws,
+                          size_t ws_bytes, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

@@ -13,7 +13,14 @@ gradient of ``inverse_spectrogram`` inside ``audio_b200.differentiable(inverse=T
 ``resample`` / ``speed`` inside ``audio_b200.differentiable(resample=True)``, and the input gradients of
 ``amplitude_to_DB``, ``spectral_centroid`` and the MFCC / LFCC / MelScale paths inside
 ``audio_b200.differentiable(features=True)``, and the spectrogram gradient of ``phase_vocoder`` and the waveform
-gradient of ``pitch_shift`` inside ``audio_b200.differentiable(vocoder=True)``.  ``griffinlim`` is forward-only.
+gradient of ``pitch_shift`` inside ``audio_b200.differentiable(vocoder=True)``, and the waveform and coefficient
+gradients of ``lfilter``, ``filtfilt``, the ``*_biquad`` filters, ``preemphasis`` and ``deemphasis`` inside
+``audio_b200.differentiable(filtering=True)``.  ``griffinlim`` is forward-only.
+
+IIR filtering (reference functional/filtering.py): ``lfilter`` (1032-1099), ``filtfilt`` (672-710), ``biquad`` and the
+``allpass`` / ``band`` / ``bandpass`` / ``bandreject`` / ``bass`` / ``deemph`` / ``equalizer`` / ``highpass`` /
+``lowpass`` / ``riaa`` / ``treble`` ``_biquad`` designs, and ``preemphasis`` / ``deemphasis`` (functional.py:2426-2473),
+all on one chunked-scan kernel family; filter orders up to 16.
 """
 from __future__ import annotations
 
@@ -30,6 +37,9 @@ from torch.autograd.function import once_differentiable
 from . import _lib, _ops
 from ._bookkeeping import resample_ratio
 from ._constants import create_dct, linear_fbanks, melscale_fbanks, sinc_resample_kernel
+from ._filtering import (allpass_biquad, band_biquad, bandpass_biquad, bandreject_biquad, bass_biquad,  # noqa: F401
+                         biquad, deemph_biquad, deemphasis, equalizer_biquad, filtfilt, highpass_biquad, lfilter,
+                         lowpass_biquad, preemphasis, riaa_biquad, treble_biquad)
 from ._plans import (FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad,
                      is_feature_differentiable, is_inverse_differentiable, is_vocoder_differentiable, new_group_max,
                      vocoder_chain)
@@ -49,6 +59,22 @@ __all__ = [
     "spectral_centroid",
     "mel_spectrogram",
     "mfcc",
+    "lfilter",
+    "filtfilt",
+    "biquad",
+    "allpass_biquad",
+    "band_biquad",
+    "bandpass_biquad",
+    "bandreject_biquad",
+    "bass_biquad",
+    "deemph_biquad",
+    "equalizer_biquad",
+    "highpass_biquad",
+    "lowpass_biquad",
+    "riaa_biquad",
+    "treble_biquad",
+    "preemphasis",
+    "deemphasis",
 ]
 
 

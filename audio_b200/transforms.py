@@ -13,8 +13,9 @@ spectrum through HBM) -- they read the sub-modules' buffers and launch the fused
 Gradients are opt-in, per thread: Spectrogram and MelSpectrogram inside ``audio_b200.differentiable()``,
 InverseSpectrogram with ``inverse=True``, Resample / Speed / SpeedPerturbation with ``resample=True``, and MFCC,
 LFCC, AmplitudeToDB, MelScale, InverseMelScale and SpectralCentroid with ``features=True``, the Kaldi features
-(``audio_b200.compliance.kaldi``) with ``kaldi=True``, and TimeStretch (spectrogram gradient) and PitchShift
-(waveform gradient) with ``vocoder=True``.  GriffinLim is forward-only.
+(``audio_b200.compliance.kaldi``) with ``kaldi=True``, TimeStretch (spectrogram gradient) and PitchShift
+(waveform gradient) with ``vocoder=True``, and Preemphasis and Deemphasis (waveform gradient) with ``filtering=True``.
+GriffinLim is forward-only.
 """
 from __future__ import annotations
 
@@ -31,7 +32,8 @@ from ._plans import (FrontendPlan, InverseMelPlan, ResamplePlan, _InverseMelFunc
                      _wants_grad, is_feature_differentiable, vocoder_chain)
 
 __all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "InverseMelScale", "MelSpectrogram", "MFCC", "LFCC",
-           "SpectralCentroid", "Resample", "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift"]
+           "SpectralCentroid", "Resample", "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift", "Preemphasis",
+           "Deemphasis"]
 
 
 def _setup_framing(mod, n_fft, win_length, hop_length, window_fn=None, wkwargs=None, hop_div=2):
@@ -700,6 +702,28 @@ class PitchShift(torch.nn.Module):
         else:
             shifted = torch.nn.functional.pad(shifted, [0, ori_len - shift_len])
         return shifted.reshape(shape[:-1] + shifted.shape[-1:])
+
+
+class Preemphasis(torch.nn.Module):
+    """y[i] = x[i] - coeff * x[i - 1] along the last dimension (reference _transforms.py:2086-2112)."""
+
+    def __init__(self, coeff: float = 0.97) -> None:
+        super().__init__()
+        self.coeff = coeff
+
+    def forward(self, waveform: Tensor) -> Tensor:
+        return F.preemphasis(waveform, coeff=self.coeff)
+
+
+class Deemphasis(torch.nn.Module):
+    """y[i] = x[i] + coeff * y[i - 1], clamped to [-1, 1] as the reference's is (reference _transforms.py:2115-2140)."""
+
+    def __init__(self, coeff: float = 0.97) -> None:
+        super().__init__()
+        self.coeff = coeff
+
+    def forward(self, waveform: Tensor) -> Tensor:
+        return F.deemphasis(waveform, coeff=self.coeff)
 
 
 # ---- B200A_REFERENCE=1: A/B switch to the reference implementation (debugging only, never silent) -----------------

@@ -491,6 +491,54 @@ int b200a_inverse_mel_backward(const void* plan, int32_t n_stft, int32_t n_mels,
                                const float* grad, int64_t g_stride_row, int64_t g_stride_frame, int64_t g_stride_bin,
                                float* grad_mel, b200a_stream stream);
 
+/* ---- IIR filtering: lfilter (functional/filtering.py:1032-1099) ------------------------------------------------ */
+/*
+ * Rows are (batch, filter) pairs, row r = bi * n_filters + f uses filter f.  With n_order coefficients (filter order
+ * N = n_order - 1) and the float32-normalised coefficients a^ = a / a0, b^ = b / a0 (one float division each, as the
+ * reference normalises):
+ *   v[t] = sum_{k=0..N} b^_k x[t-k],   y[t] = v[t] - sum_{k=1..N} a^_k y[t-k],   zero history before t = 0;
+ * with `reverse` the recurrence runs from t = length-1 downward (x[t+k], y[t+k], zero history past the end), which is
+ * filtfilt's second pass without flip copies.  `clamp` applies clamp(y, -1, 1) once at the end.
+ * The recurrence is a chunked scan: every thread runs 32 samples serially from a zero history, chunk and tile carries
+ * are joined through the N-sample output history with the carry map M and its powers built from a^ in DOUBLE, and
+ * each chunk re-runs from its true starting history rounded to float32.  The scan order is fixed and the chunk length
+ * depends on N alone: reruns are bit-identical and a row's output does not depend on the other rows.  No atomics.
+ */
+#define B200A_LFILTER_MAX_ORDER 16 /* filter order cap N = n_order - 1 (B200A_EUNSUPPORTED above) */
+
+/* Workspace bytes of b200a_lfilter_run for `rows` = batch * n_filters rows of `length` samples; 0 for an invalid or
+ * unsupported request.  b200a_lfilter_backward needs b200a_lfilter_backward_workspace_bytes instead. */
+size_t b200a_lfilter_workspace_bytes(int64_t rows, int64_t length, int32_t n_order, int32_t n_filters);
+size_t b200a_lfilter_backward_workspace_bytes(int64_t rows, int64_t length, int32_t n_order, int32_t n_filters);
+/*
+ *   a, b        : DEVICE [n_filters][n_order] raw coefficients (read on the device: no host synchronisation)
+ *   x           : row (bi, f) at x + bi * stride_batch + f * stride_filter, unit element stride; stride_filter may be 0
+ *                 (one waveform row for every filter: batching=False without a stacked copy)
+ *   y           : [batch][n_filters][length] contiguous, every element written (clamped when `clamp`)
+ *   y_unclamped : the same before the clamp, or NULL
+ * B200A_EINVAL for null pointers, non-positive n_order / n_filters or negative sizes; B200A_EUNSUPPORTED for
+ * n_order - 1 > B200A_LFILTER_MAX_ORDER; B200A_EWORKSPACE when workspace_bytes is too small.  batch == 0 or
+ * length == 0 enqueues nothing.
+ */
+int b200a_lfilter_run(const float* a, const float* b, int32_t n_filters, int32_t n_order, const float* x, int64_t batch,
+                      int64_t length, int64_t stride_batch, int64_t stride_filter, int32_t clamp, int32_t reverse,
+                      float* y, float* y_unclamped, void* workspace, size_t workspace_bytes, b200a_stream stream);
+/*
+ * Gradients of b200a_lfilter_run.  g_y = grad * (-1 <= y_unclamped <= 1) when `clamp` (torch.clamp's inclusive rule),
+ * else grad; u = the IIR recurrence run in the opposite direction on g_y (the mask is fused into its input read);
+ *   grad_x[t] = sum_k b^_k u[t+k],  d a^_k = -sum_t u[t] y[t-k],  d b^_k = sum_t u[t] x[t-k]  (k toward the past of
+ * the forward's direction), the last two summed over the rows of each filter, then taken through a0 to the raw a, b.
+ *   y_unclamped : [batch][n_filters][length] contiguous (the forward's unclamped output)
+ *   grad        : [batch][n_filters][length] contiguous
+ *   grad_x      : [batch][n_filters][length] contiguous, or NULL;  grad_a, grad_b : [n_filters][n_order], or NULL
+ * The coefficient gradients are reduced over rows and tiles in a fixed order (double partial sums): reruns are
+ * bit-identical, and grad_x of a row does not depend on the other rows.  Statuses as b200a_lfilter_run.
+ */
+int b200a_lfilter_backward(const float* a, const float* b, int32_t n_filters, int32_t n_order, const float* x,
+                           int64_t batch, int64_t length, int64_t stride_batch, int64_t stride_filter,
+                           const float* y_unclamped, const float* grad, int32_t clamp, int32_t reverse, float* grad_x,
+                           float* grad_a, float* grad_b, void* workspace, size_t workspace_bytes, b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);

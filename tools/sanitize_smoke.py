@@ -72,5 +72,21 @@ with audio_b200.differentiable(vocoder=True):  # phase-vocoder adjoint: TimeStre
     spec = T.Spectrogram(n_fft=512, hop_length=128, power=None).cuda()(x).requires_grad_()
     T.TimeStretch(hop_length=128, n_freq=257, fixed_rate=0.8).cuda()(spec).abs().sum().backward()
     T.PitchShift(16000, -3).cuda()(x.clone().requires_grad_()).sum().backward()
+import audio_b200.functional as F  # noqa: E402
+
+# IIR filtering: lfilter forward + backward over several tiles, filtfilt, a pure gain (n_order = 1), a signal shorter
+# than one chunk, the order cap and batching=False (stride-0 rows)
+with audio_b200.differentiable(filtering=True):
+    xg = x.clone().requires_grad_()
+    a = torch.tensor([1.0, -1.8, 0.81], device="cuda", requires_grad=True)
+    b = torch.tensor([0.01, 0.02, 0.01], device="cuda", requires_grad=True)
+    F.lfilter(xg, a, b).sum().backward()
+    F.filtfilt(xg, a, b).sum().backward()
+    F.lfilter(xg, a[:1], b[:1]).sum().backward()
+    F.lfilter(xg[:, :20], a, b).sum().backward()
+a16 = 0.01 * torch.rand(3, 17, device="cuda")
+a16[:, 0] = 1.0
+F.lfilter(x, a16, torch.rand(3, 17, device="cuda"), batching=False)
+F.deemphasis(x)
 torch.cuda.synchronize()
 print("done")
