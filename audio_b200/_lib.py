@@ -21,6 +21,7 @@ STAGE_COMPLEX, STAGE_POWER, STAGE_MEL, STAGE_FEAT = 0, 1, 2, 3
 LSTSQ_DRIVER = {"gels": 0, "gelsy": 1, "gelsd": 2, "gelss": 3}
 INVERSE_MEL_MAX_BANDWIDTH, INVERSE_MEL_MAX_MELS = 4, 512  # B200A_INVERSE_MEL_MAX_BANDWIDTH / _MAX_MELS
 LFILTER_MAX_ORDER = 16  # B200A_LFILTER_MAX_ORDER
+FFTCONVOLVE_MAX_PARTITIONS, FFTCONVOLVE_MAX_BLOCK = 128, 2048  # B200A_FFTCONVOLVE_MAX_PARTITIONS; the largest block
 
 
 class FrontendDesc(ctypes.Structure):
@@ -65,6 +66,24 @@ class KaldiDesc(ctypes.Structure):
         ("out_width", c_int32),
         ("out_col0", c_int32),
         ("use_log", c_int32),
+    ]
+
+
+class FftconvolveDesc(ctypes.Structure):
+    """Mirror of ``b200a_fftconvolve_desc``."""
+
+    _fields_ = [
+        ("n", c_int64),
+        ("m", c_int64),
+        ("out_len", c_int64),
+        ("start", c_int64),
+        ("rows", c_int64),
+        ("x_rows", c_int64),
+        ("y_rows", c_int64),
+        ("x_index", c_void_p),
+        ("y_index", c_void_p),
+        ("x_stride", c_int64),
+        ("y_stride", c_int64),
     ]
 
 
@@ -204,6 +223,16 @@ _SIGNATURES = {
         ctypes.c_int,
         [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int32,
          c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_fftconvolve_workspace_bytes": (c_size_t, [POINTER(FftconvolveDesc)]),
+    "b200a_fftconvolve_backward_workspace_bytes": (c_size_t, [POINTER(FftconvolveDesc)]),
+    "b200a_fftconvolve_run": (
+        ctypes.c_int,
+        [POINTER(FftconvolveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_fftconvolve_backward": (
+        ctypes.c_int,
+        [POINTER(FftconvolveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
     ),
 }
 

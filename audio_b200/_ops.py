@@ -2,7 +2,8 @@
 capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
 ``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward`` / ``rnnt_features`` /
-``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward`` / ``lfilter`` / ``lfilter_backward``.
+``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward`` / ``lfilter`` / ``lfilter_backward`` /
+``fftconvolve`` / ``fftconvolve_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -14,6 +15,8 @@ deliberately NO CPU implementation: a CPU tensor fails in the dispatcher ("no ke
 The descriptor travels as a list of ints + a list of floats (``b200a_frontend_desc`` is plain old data).
 """
 from __future__ import annotations
+
+import ctypes
 
 from typing import List, Optional
 
@@ -79,6 +82,10 @@ _LIB.define("lfilter(Tensor x, Tensor a, Tensor b, bool clamp, bool reverse, boo
 _LIB.define(
     "lfilter_backward(Tensor grad, Tensor x, Tensor y_raw, Tensor a, Tensor b, bool clamp, bool reverse) "
     "-> (Tensor, Tensor, Tensor)"
+)
+_LIB.define("fftconvolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor")
+_LIB.define(
+    "fftconvolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)"
 )
 
 _KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
@@ -555,6 +562,58 @@ def _lfilter_backward_meta(grad, x, y_raw, a, b, clamp, reverse):
     return x.new_empty(x.shape), a.new_empty(a.shape), b.new_empty(b.shape)
 
 
+# ---- fftconvolve / fftconvolve_backward -------------------------------------------------------------------------
+def _fftconvolve_desc(x, y, x_index, y_index, start, out_len):
+    if not (x_index.is_contiguous() and y_index.is_contiguous() and x_index.dtype == y_index.dtype == torch.int64):
+        raise ValueError("fftconvolve: the row index vectors must be contiguous int64")
+    return _lib.FftconvolveDesc(n=x.shape[1], m=y.shape[1], out_len=out_len, start=start, rows=x_index.shape[0],
+                                x_rows=x.shape[0], y_rows=y.shape[0], x_index=x_index.data_ptr(),
+                                y_index=y_index.data_ptr(), x_stride=x.stride(0), y_stride=y.stride(0))
+
+
+def _fftconvolve_cuda(x, y, x_index, y_index, start, out_len):
+    """(x_rows, N) and (y_rows, M) operand rows with a unit time stride, and int64 (rows,) index vectors naming each
+    output row's operand rows -> the (rows, out_len) slice [start, start + out_len) of the full convolution."""
+    dev = x.device
+    lib = _lib.lib()
+    d = _fftconvolve_desc(x, y, x_index, y_index, start, out_len)
+    with torch.cuda.device(dev):
+        out = torch.empty((x_index.shape[0], out_len), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_fftconvolve_workspace_bytes(ctypes.byref(d))
+        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        rc = lib.b200a_fftconvolve_run(ctypes.byref(d), x.data_ptr(), y.data_ptr(), out.data_ptr(), ws.data_ptr(),
+                                       nbytes, _stream(dev))
+    _lib.check(rc, "fftconvolve")
+    return out
+
+
+def _fftconvolve_meta(x, y, x_index, y_index, start, out_len):
+    return x.new_empty((x_index.shape[0], out_len))
+
+
+def _fftconvolve_backward_cuda(grad, x, y, x_index, y_index, start):
+    """Upstream gradient of the (rows, L) output -> per-output-row (grad_x (rows, N), grad_y (rows, M))."""
+    dev = x.device
+    lib = _lib.lib()
+    grad = grad.contiguous()
+    d = _fftconvolve_desc(x, y, x_index, y_index, start, grad.shape[1])
+    rows = x_index.shape[0]
+    with torch.cuda.device(dev):
+        gx = torch.empty((rows, x.shape[1]), dtype=torch.float32, device=dev)
+        gy = torch.empty((rows, y.shape[1]), dtype=torch.float32, device=dev)
+        nbytes = lib.b200a_fftconvolve_backward_workspace_bytes(ctypes.byref(d))
+        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        rc = lib.b200a_fftconvolve_backward(ctypes.byref(d), x.data_ptr(), y.data_ptr(), grad.data_ptr(), gx.data_ptr(),
+                                            gy.data_ptr(), ws.data_ptr(), nbytes, _stream(dev))
+    _lib.check(rc, "fftconvolve_backward")
+    return gx, gy
+
+
+def _fftconvolve_backward_meta(grad, x, y, x_index, y_index, start):
+    rows = x_index.shape[0]
+    return x.new_empty((rows, x.shape[1])), y.new_empty((rows, y.shape[1]))
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
@@ -573,7 +632,9 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("inverse_mel", _inverse_mel_cuda, _inverse_mel_meta),
                             ("inverse_mel_backward", _inverse_mel_backward_cuda, _inverse_mel_backward_meta),
                             ("lfilter", _lfilter_cuda, _lfilter_meta),
-                            ("lfilter_backward", _lfilter_backward_cuda, _lfilter_backward_meta)):
+                            ("lfilter_backward", _lfilter_backward_cuda, _lfilter_backward_meta),
+                            ("fftconvolve", _fftconvolve_cuda, _fftconvolve_meta),
+                            ("fftconvolve_backward", _fftconvolve_backward_cuda, _fftconvolve_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -596,3 +657,5 @@ inverse_mel = torch.ops.b200audio.inverse_mel
 inverse_mel_backward = torch.ops.b200audio.inverse_mel_backward
 lfilter = torch.ops.b200audio.lfilter
 lfilter_backward = torch.ops.b200audio.lfilter_backward
+fftconvolve = torch.ops.b200audio.fftconvolve
+fftconvolve_backward = torch.ops.b200audio.fftconvolve_backward

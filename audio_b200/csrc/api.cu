@@ -506,5 +506,25 @@ int b200a_lfilter_backward(const float* a, const float* b, int32_t n_filters, in
                                static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_fftconvolve_workspace_bytes(const b200a_fftconvolve_desc* desc) {
+  return fftconvolve_workspace_bytes_impl(desc, false);
+}
+
+size_t b200a_fftconvolve_backward_workspace_bytes(const b200a_fftconvolve_desc* desc) {
+  return fftconvolve_workspace_bytes_impl(desc, true);
+}
+
+int b200a_fftconvolve_run(const b200a_fftconvolve_desc* desc, const float* x, const float* y, float* out,
+                          void* workspace, size_t workspace_bytes, b200a_stream stream) {
+  return fftconvolve_run_impl(desc, x, y, out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int b200a_fftconvolve_backward(const b200a_fftconvolve_desc* desc, const float* x, const float* y, const float* grad,
+                               float* grad_x, float* grad_y, void* workspace, size_t workspace_bytes,
+                               b200a_stream stream) {
+  return fftconvolve_backward_impl(desc, x, y, grad, grad_x, grad_y, workspace, workspace_bytes,
+                                   static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -14,13 +14,16 @@ gradient of ``inverse_spectrogram`` inside ``audio_b200.differentiable(inverse=T
 ``amplitude_to_DB``, ``spectral_centroid`` and the MFCC / LFCC / MelScale paths inside
 ``audio_b200.differentiable(features=True)``, and the spectrogram gradient of ``phase_vocoder`` and the waveform
 gradient of ``pitch_shift`` inside ``audio_b200.differentiable(vocoder=True)``, and the waveform and coefficient
-gradients of ``lfilter``, ``filtfilt``, the ``*_biquad`` filters, ``preemphasis`` and ``deemphasis`` inside
-``audio_b200.differentiable(filtering=True)``.  ``griffinlim`` is forward-only.
+gradients of ``lfilter``, ``filtfilt``, the ``*_biquad`` filters, ``preemphasis`` and ``deemphasis``, and the input
+gradients of ``fftconvolve``, inside ``audio_b200.differentiable(filtering=True)``.  ``griffinlim`` is forward-only.
 
 IIR filtering (reference functional/filtering.py): ``lfilter`` (1032-1099), ``filtfilt`` (672-710), ``biquad`` and the
 ``allpass`` / ``band`` / ``bandpass`` / ``bandreject`` / ``bass`` / ``deemph`` / ``equalizer`` / ``highpass`` /
 ``lowpass`` / ``riaa`` / ``treble`` ``_biquad`` designs, and ``preemphasis`` / ``deemphasis`` (functional.py:2426-2473),
 all on one chunked-scan kernel family; filter orders up to 16.
+
+FFT convolution: ``fftconvolve`` (functional.py:2222-2258), uniformly partitioned overlap-save on the kernels of
+``csrc/convolve.cu``.
 """
 from __future__ import annotations
 
@@ -41,8 +44,8 @@ from ._filtering import (allpass_biquad, band_biquad, bandpass_biquad, bandrejec
                          biquad, deemph_biquad, deemphasis, equalizer_biquad, filtfilt, highpass_biquad, lfilter,
                          lowpass_biquad, preemphasis, riaa_biquad, treble_biquad)
 from ._plans import (FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad,
-                     is_feature_differentiable, is_inverse_differentiable, is_vocoder_differentiable, new_group_max,
-                     vocoder_chain)
+                     is_feature_differentiable, is_filtering_differentiable, is_inverse_differentiable,
+                     is_vocoder_differentiable, new_group_max, pack_rows, vocoder_chain)
 
 __all__ = [
     "spectrogram",
@@ -75,6 +78,7 @@ __all__ = [
     "treble_biquad",
     "preemphasis",
     "deemphasis",
+    "fftconvolve",
 ]
 
 
@@ -745,3 +749,102 @@ class _RatioFunction(torch.autograd.Function):
     def backward(ctx, g):
         (pairs,) = ctx.saved_tensors
         return _ops.ratio_backward(g, pairs)
+
+
+# ---- FFT convolution (reference functional.py:2189-2258) -------------------------------------------------------
+def _check_shape_compatible(x: Tensor, y: Tensor) -> None:
+    if x.ndim != y.ndim:
+        raise ValueError(f"The operands must be the same dimension (got {x.ndim} and {y.ndim}).")
+    for i in range(x.ndim - 1):
+        xi, yi = x.size(i), y.size(i)
+        if xi == yi or xi == 1 or yi == 1:
+            continue
+        raise ValueError(f"Leading dimensions of x and y are not broadcastable (got {x.shape} and {y.shape}).")
+
+
+def _check_convolve_mode(mode: str) -> None:
+    valid_convolve_modes = ["full", "valid", "same"]
+    if mode not in valid_convolve_modes:
+        raise ValueError(f"Unrecognized mode value '{mode}'. Please specify one of {valid_convolve_modes}.")
+
+
+def _convolve_slice(n: int, m: int, mode: str):
+    """(start, length) of ``_apply_convolve_mode``'s slice of the full (n + m - 1)-sample result, with Python's slice
+    rules (a negative start counts from the end, as the reference's slicing does for an empty operand)."""
+    full = n + m - 1
+    if mode == "full":
+        return 0, full
+    target = max(n, m) - min(n, m) + 1 if mode == "valid" else n
+    start = (full - target) // 2
+    lo, hi, _ = slice(start, start + target).indices(full)
+    return lo, max(hi - lo, 0)
+
+
+class _FFTConvolveFunction(torch.autograd.Function):
+    """b200audio::fftconvolve on the operand rows with b200audio::fftconvolve_backward as its backward.  Saved
+    (save_for_backward): the two operands' rows only.  The per-output-row gradients are summed onto the operand rows
+    that broadcasting shared (``sum_to_size``: a fixed-order reduction, no atomics)."""
+
+    @staticmethod
+    def forward(ctx, x2, y2, ix, iy, start, out_len, shapes):
+        ctx.save_for_backward(x2, y2)
+        ctx.ix, ctx.iy, ctx.start, ctx.shapes = ix, iy, start, shapes
+        return _ops.fftconvolve(x2, y2, ix, iy, start, out_len)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x2, y2 = ctx.saved_tensors
+        gx, gy = _ops.fftconvolve_backward(g, x2, y2, ctx.ix, ctx.iy, ctx.start)
+        lo, lx, ly = ctx.shapes
+        need = ctx.needs_input_grad
+        gx = gx.reshape(lo + (x2.shape[1],)).sum_to_size(lx + (x2.shape[1],)).reshape(x2.shape) if need[0] else None
+        gy = gy.reshape(lo + (y2.shape[1],)).sum_to_size(ly + (y2.shape[1],)).reshape(y2.shape) if need[1] else None
+        return gx, gy, None, None, None, None, None
+
+
+def fftconvolve(x: Tensor, y: Tensor, mode: str = "full") -> Tensor:
+    """Convolves ``x (..., N)`` and ``y (..., M)`` along their last dimension (reference functional.py:2222-2258): the
+    true convolution, leading dimensions broadcast, output ``(..., L)`` with L = N + M - 1 (``"full"``),
+    max(N, M) - min(N, M) + 1 (``"valid"``) or N (``"same"``).  Runs uniformly partitioned overlap-save
+    (``csrc/convolve.cu``): the shorter operand is cut into blocks of B = 256 .. 2048 samples, and only the output
+    blocks the mode returns are computed.  The shorter operand may have up to 128 * 2048 = 262144 samples."""
+    _check_shape_compatible(x, y)
+    _check_convolve_mode(mode)
+    _require_cuda_f32(x, "x")
+    _require_cuda_f32(y, "y")
+    if y.device != x.device:
+        raise RuntimeError(f"audio_b200: y is on {y.device} but x is on {x.device}")
+    n, m = x.shape[-1], y.shape[-1]
+    lx, ly = tuple(x.shape[:-1]), tuple(y.shape[:-1])
+    lo = tuple(torch.broadcast_shapes(lx, ly))
+    if n + m - 1 <= 0:  # what torch.fft.rfft reports for the reference's n = N + M - 1 points
+        raise RuntimeError(f"Invalid number of data points ({n + m - 1}) specified")
+    start, out_len = _convolve_slice(n, m, mode)
+    if n == 0 or m == 0:
+        return x.new_zeros(lo + (out_len,))  # the transform of an empty operand is zero
+    k = min(n, m)
+    block = min(max(1 << (k - 1).bit_length(), 256), _lib.FFTCONVOLVE_MAX_BLOCK)
+    if -(-k // block) > _lib.FFTCONVOLVE_MAX_PARTITIONS:
+        raise RuntimeError(
+            f"audio_b200: fftconvolve of a {k}-sample shorter operand is not supported: it is capped at "
+            f"{_lib.FFTCONVOLVE_MAX_PARTITIONS} partitions of {block} samples (B200A_FFTCONVOLVE_MAX_PARTITIONS), "
+            f"{_lib.FFTCONVOLVE_MAX_PARTITIONS * block} samples")
+    if math.prod(lo) == 0:
+        return x.new_empty(lo + (out_len,))
+    x2, _ = pack_rows(x)
+    y2, _ = pack_rows(y)
+    dev = x.device
+    # output row -> operand row, by broadcasting the operands' row numbers on the device (no host synchronisation); the
+    # kernels read one int64 per output row, so the vectors are materialised (a broadcast view may have stride 0)
+    ix = torch.arange(x2.shape[0], device=dev).reshape(lx).broadcast_to(lo).contiguous().reshape(-1)
+    iy = torch.arange(y2.shape[0], device=dev).reshape(ly).broadcast_to(lo).contiguous().reshape(-1)
+    grad = torch.is_grad_enabled() and (x.requires_grad or y.requires_grad)
+    if grad and not is_filtering_differentiable():
+        _no_autograd(x)
+        _no_autograd(y)
+    if grad:
+        out = _FFTConvolveFunction.apply(x2, y2, ix, iy, start, out_len, (lo, lx, ly))
+    else:
+        out = _ops.fftconvolve(x2, y2, ix, iy, start, out_len)
+    return out.reshape(lo + (out_len,))

@@ -539,6 +539,53 @@ int b200a_lfilter_backward(const float* a, const float* b, int32_t n_filters, in
                            const float* y_unclamped, const float* grad, int32_t clamp, int32_t reverse, float* grad_x,
                            float* grad_a, float* grad_b, void* workspace, size_t workspace_bytes, b200a_stream stream);
 
+/* ---- FFT convolution: fftconvolve (functional/functional.py:2189-2258) ------------------------------------------ */
+/*
+ * out[r][i] = sum_k x_r[k] y_r[start + i - k],  i < out_len, the slice [start, start + out_len) of the full
+ * (n + m - 1)-sample linear convolution of output row r's operands x_r = x + x_index[r] * x_stride (n samples) and
+ * y_r = y + y_index[r] * y_stride (m samples).  The index vectors express broadcasting: operand rows shared by several
+ * output rows are transformed once.
+ * Uniformly partitioned overlap-save: the shorter operand (the filter, K = min(n, m) taps; y when n == m) is cut into
+ * P = ceil(K / B) partitions of B samples, B = the next power of two of K clamped to [256, 2048], and every FFT is 2B
+ * points.  B depends on K alone and every sum runs in a fixed order without atomics: reruns are bit-identical and a
+ * row's output does not depend on the other rows.
+ */
+#define B200A_FFTCONVOLVE_MAX_PARTITIONS 128 /* P cap: filters up to 128 * 2048 = 262144 taps (B200A_EUNSUPPORTED above) */
+
+typedef struct b200a_fftconvolve_desc {
+  int64_t n, m;            /* operand lengths, >= 1 each; n + m - 1 <= INT32_MAX */
+  int64_t out_len, start;  /* the output slice of the full range: start >= 0, start + out_len <= n + m - 1 */
+  int64_t rows;            /* output rows */
+  int64_t x_rows, y_rows;  /* operand rows (>= 1); x_index[r] < x_rows, y_index[r] < y_rows */
+  const int64_t* x_index;  /* DEVICE [rows] */
+  const int64_t* y_index;  /* DEVICE [rows] */
+  int64_t x_stride, y_stride; /* element stride between operand rows; unit stride in time */
+} b200a_fftconvolve_desc;
+
+/* Workspace bytes of b200a_fftconvolve_run / b200a_fftconvolve_backward for `desc`; 0 for an invalid or unsupported
+ * descriptor. */
+size_t b200a_fftconvolve_workspace_bytes(const b200a_fftconvolve_desc* desc);
+size_t b200a_fftconvolve_backward_workspace_bytes(const b200a_fftconvolve_desc* desc);
+/*
+ *   out : [rows][out_len] contiguous, every element written once
+ * B200A_EINVAL for a null pointer, a length < 1, negative sizes or strides, or a slice outside the full range;
+ * B200A_EUNSUPPORTED above B200A_FFTCONVOLVE_MAX_PARTITIONS or for n + m - 1 > INT32_MAX; B200A_EWORKSPACE when
+ * workspace_bytes is too small.  rows == 0 or out_len == 0 enqueues nothing.
+ */
+int b200a_fftconvolve_run(const b200a_fftconvolve_desc* desc, const float* x, const float* y, float* out,
+                          void* workspace, size_t workspace_bytes, b200a_stream stream);
+/*
+ * Gradients of b200a_fftconvolve_run for the upstream gradient g = grad[r] placed at `start` of the full range (zero
+ * elsewhere), per OUTPUT row:  grad_x[r][k] = sum_j g[k + j] y_r[j],  grad_y[r][j] = sum_k g[k + j] x_r[k].  The
+ * caller sums the rows that share an operand.
+ *   grad   : [rows][out_len] contiguous
+ *   grad_x : [rows][n] contiguous;  grad_y : [rows][m] contiguous
+ * Statuses as b200a_fftconvolve_run; out_len == 0 zero-fills both gradients.
+ */
+int b200a_fftconvolve_backward(const b200a_fftconvolve_desc* desc, const float* x, const float* y, const float* grad,
+                               float* grad_x, float* grad_y, void* workspace, size_t workspace_bytes,
+                               b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);

@@ -88,5 +88,10 @@ a16 = 0.01 * torch.rand(3, 17, device="cuda")
 a16[:, 0] = 1.0
 F.lfilter(x, a16, torch.rand(3, 17, device="cuda"), batching=False)
 F.deemphasis(x)
+# FFT convolution: a broadcast two-partition filter forward + backward (swapped operands), and "same" with P = 1
+with audio_b200.differentiable(filtering=True):
+    xg = x.clone().requires_grad_()
+    F.fftconvolve(torch.randn(1, 1, 2500, device="cuda", requires_grad=True), xg[:, None, :3000]).sum().backward()
+F.fftconvolve(x, torch.randn(3, 255, device="cuda"), "same")
 torch.cuda.synchronize()
 print("done")
