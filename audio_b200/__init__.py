@@ -4,7 +4,7 @@
                                                # GriffinLim, TimeStretch, PitchShift, Speed, ...
     import audio_b200.functional as F          # spectrogram, resample, melscale_fbanks, griffinlim, phase_vocoder,
                                                # lfilter, filtfilt, the *_biquad filters, deemphasis,
-                                               # fftconvolve, ...
+                                               # fftconvolve, convolve, ...
     import audio_b200.compliance.kaldi as K    # spectrogram, fbank, mfcc (Kaldi-compatible)
 
 Everything computes in hand-written CUDA kernels reached through the C ABI of

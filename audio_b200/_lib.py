@@ -22,6 +22,7 @@ LSTSQ_DRIVER = {"gels": 0, "gelsy": 1, "gelsd": 2, "gelss": 3}
 INVERSE_MEL_MAX_BANDWIDTH, INVERSE_MEL_MAX_MELS = 4, 512  # B200A_INVERSE_MEL_MAX_BANDWIDTH / _MAX_MELS
 LFILTER_MAX_ORDER = 16  # B200A_LFILTER_MAX_ORDER
 FFTCONVOLVE_MAX_PARTITIONS, FFTCONVOLVE_MAX_BLOCK = 128, 2048  # B200A_FFTCONVOLVE_MAX_PARTITIONS; the largest block
+CONVOLVE_MAX_TAPS = 4096  # B200A_CONVOLVE_MAX_TAPS
 
 
 class FrontendDesc(ctypes.Structure):
@@ -70,7 +71,7 @@ class KaldiDesc(ctypes.Structure):
 
 
 class FftconvolveDesc(ctypes.Structure):
-    """Mirror of ``b200a_fftconvolve_desc``."""
+    """Mirror of ``b200a_fftconvolve_desc`` (also ``b200a_convolve_desc``)."""
 
     _fields_ = [
         ("n", c_int64),
@@ -231,6 +232,16 @@ _SIGNATURES = {
         [POINTER(FftconvolveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
     ),
     "b200a_fftconvolve_backward": (
+        ctypes.c_int,
+        [POINTER(FftconvolveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_convolve_workspace_bytes": (c_size_t, [POINTER(FftconvolveDesc)]),
+    "b200a_convolve_backward_workspace_bytes": (c_size_t, [POINTER(FftconvolveDesc)]),
+    "b200a_convolve_run": (
+        ctypes.c_int,
+        [POINTER(FftconvolveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_convolve_backward": (
         ctypes.c_int,
         [POINTER(FftconvolveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
     ),

@@ -3,7 +3,7 @@ capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` 
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
 ``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward`` / ``rnnt_features`` /
 ``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward`` / ``lfilter`` / ``lfilter_backward`` /
-``fftconvolve`` / ``fftconvolve_backward``.
+``fftconvolve`` / ``fftconvolve_backward`` / ``convolve`` / ``convolve_backward``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -86,6 +86,10 @@ _LIB.define(
 _LIB.define("fftconvolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor")
 _LIB.define(
     "fftconvolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)"
+)
+_LIB.define("convolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor")
+_LIB.define(
+    "convolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)"
 )
 
 _KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
@@ -571,28 +575,26 @@ def _fftconvolve_desc(x, y, x_index, y_index, start, out_len):
                                 y_index=y_index.data_ptr(), x_stride=x.stride(0), y_stride=y.stride(0))
 
 
-def _fftconvolve_cuda(x, y, x_index, y_index, start, out_len):
+def _conv_run(kind, x, y, x_index, y_index, start, out_len):
     """(x_rows, N) and (y_rows, M) operand rows with a unit time stride, and int64 (rows,) index vectors naming each
-    output row's operand rows -> the (rows, out_len) slice [start, start + out_len) of the full convolution."""
+    output row's operand rows -> the (rows, out_len) slice [start, start + out_len) of the full convolution, by
+    b200a_{kind}_run."""
     dev = x.device
     lib = _lib.lib()
     d = _fftconvolve_desc(x, y, x_index, y_index, start, out_len)
     with torch.cuda.device(dev):
         out = torch.empty((x_index.shape[0], out_len), dtype=torch.float32, device=dev)
-        nbytes = lib.b200a_fftconvolve_workspace_bytes(ctypes.byref(d))
+        nbytes = getattr(lib, f"b200a_{kind}_workspace_bytes")(ctypes.byref(d))
         ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-        rc = lib.b200a_fftconvolve_run(ctypes.byref(d), x.data_ptr(), y.data_ptr(), out.data_ptr(), ws.data_ptr(),
-                                       nbytes, _stream(dev))
-    _lib.check(rc, "fftconvolve")
+        rc = getattr(lib, f"b200a_{kind}_run")(ctypes.byref(d), x.data_ptr(), y.data_ptr(), out.data_ptr(),
+                                               ws.data_ptr(), nbytes, _stream(dev))
+    _lib.check(rc, kind)
     return out
 
 
-def _fftconvolve_meta(x, y, x_index, y_index, start, out_len):
-    return x.new_empty((x_index.shape[0], out_len))
-
-
-def _fftconvolve_backward_cuda(grad, x, y, x_index, y_index, start):
-    """Upstream gradient of the (rows, L) output -> per-output-row (grad_x (rows, N), grad_y (rows, M))."""
+def _conv_backward(kind, grad, x, y, x_index, y_index, start):
+    """Upstream gradient of the (rows, L) output -> per-output-row (grad_x (rows, N), grad_y (rows, M)), by
+    b200a_{kind}_backward."""
     dev = x.device
     lib = _lib.lib()
     grad = grad.contiguous()
@@ -601,17 +603,38 @@ def _fftconvolve_backward_cuda(grad, x, y, x_index, y_index, start):
     with torch.cuda.device(dev):
         gx = torch.empty((rows, x.shape[1]), dtype=torch.float32, device=dev)
         gy = torch.empty((rows, y.shape[1]), dtype=torch.float32, device=dev)
-        nbytes = lib.b200a_fftconvolve_backward_workspace_bytes(ctypes.byref(d))
+        nbytes = getattr(lib, f"b200a_{kind}_backward_workspace_bytes")(ctypes.byref(d))
         ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-        rc = lib.b200a_fftconvolve_backward(ctypes.byref(d), x.data_ptr(), y.data_ptr(), grad.data_ptr(), gx.data_ptr(),
-                                            gy.data_ptr(), ws.data_ptr(), nbytes, _stream(dev))
-    _lib.check(rc, "fftconvolve_backward")
+        rc = getattr(lib, f"b200a_{kind}_backward")(ctypes.byref(d), x.data_ptr(), y.data_ptr(), grad.data_ptr(),
+                                                    gx.data_ptr(), gy.data_ptr(), ws.data_ptr(), nbytes, _stream(dev))
+    _lib.check(rc, f"{kind}_backward")
     return gx, gy
+
+
+def _fftconvolve_cuda(x, y, x_index, y_index, start, out_len):
+    return _conv_run("fftconvolve", x, y, x_index, y_index, start, out_len)
+
+
+def _fftconvolve_meta(x, y, x_index, y_index, start, out_len):
+    return x.new_empty((x_index.shape[0], out_len))
+
+
+def _fftconvolve_backward_cuda(grad, x, y, x_index, y_index, start):
+    return _conv_backward("fftconvolve", grad, x, y, x_index, y_index, start)
 
 
 def _fftconvolve_backward_meta(grad, x, y, x_index, y_index, start):
     rows = x_index.shape[0]
     return x.new_empty((rows, x.shape[1])), y.new_empty((rows, y.shape[1]))
+
+
+# ---- convolve / convolve_backward: the direct method on the same descriptor -----------------------------------------
+def _convolve_cuda(x, y, x_index, y_index, start, out_len):
+    return _conv_run("convolve", x, y, x_index, y_index, start, out_len)
+
+
+def _convolve_backward_cuda(grad, x, y, x_index, y_index, start):
+    return _conv_backward("convolve", grad, x, y, x_index, y_index, start)
 
 
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
@@ -634,7 +657,9 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("lfilter", _lfilter_cuda, _lfilter_meta),
                             ("lfilter_backward", _lfilter_backward_cuda, _lfilter_backward_meta),
                             ("fftconvolve", _fftconvolve_cuda, _fftconvolve_meta),
-                            ("fftconvolve_backward", _fftconvolve_backward_cuda, _fftconvolve_backward_meta)):
+                            ("fftconvolve_backward", _fftconvolve_backward_cuda, _fftconvolve_backward_meta),
+                            ("convolve", _convolve_cuda, _fftconvolve_meta),
+                            ("convolve_backward", _convolve_backward_cuda, _fftconvolve_backward_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -659,3 +684,5 @@ lfilter = torch.ops.b200audio.lfilter
 lfilter_backward = torch.ops.b200audio.lfilter_backward
 fftconvolve = torch.ops.b200audio.fftconvolve
 fftconvolve_backward = torch.ops.b200audio.fftconvolve_backward
+convolve = torch.ops.b200audio.convolve
+convolve_backward = torch.ops.b200audio.convolve_backward

@@ -67,8 +67,8 @@ def is_vocoder_differentiable() -> bool:
 
 def is_filtering_differentiable() -> bool:
     """Whether F.lfilter, F.filtfilt, the ``*_biquad`` filters, F.deemphasis, F.preemphasis, Preemphasis and
-    Deemphasis accept waveforms and coefficients, and F.fftconvolve and FFTConvolve operands, that require grad (in
-    this thread)."""
+    Deemphasis accept waveforms and coefficients, and F.convolve, Convolve, F.fftconvolve and FFTConvolve operands, that
+    require grad (in this thread)."""
     return getattr(_GRAD_STATE, "filtering", False)
 
 
@@ -81,8 +81,8 @@ def set_differentiable(mode: bool, *, inverse: bool = False, resample: bool = Fa
     ``kaldi=True`` (with ``mode``) the waveform gradients of the Kaldi spectrogram, fbank and mfcc, ``vocoder=True`` (with ``mode``) the spectrogram gradients of the phase
     vocoder and TimeStretch and the waveform gradients of PitchShift, ``filtering=True`` (with ``mode``) the waveform
     and coefficient gradients of lfilter, filtfilt, the biquads and pre-/de-emphasis and the input gradients of
-    F.fftconvolve and FFTConvolve (FFT convolution is FIR filtering).  They are separate switches so that vocoder
-    inference, augmentation code (Speed, SpeedPerturbation, TimeStretch, PitchShift) and Kaldi feature preprocessing in
+    F.convolve, Convolve, F.fftconvolve and FFTConvolve (convolution is FIR filtering).  They are separate switches so
+    that vocoder inference, augmentation code (Speed, SpeedPerturbation, TimeStretch, PitchShift) and Kaldi feature preprocessing in
     data pipelines do not build graphs when loss gradients are on, and so that the top_db clamp's gradient -- every
     clamped element's share goes to the group maximum -- is opted into knowingly."""
     _GRAD_STATE.on = bool(mode)
@@ -147,7 +147,8 @@ def _no_autograd(t: torch.Tensor) -> None:
             "gradients inside audio_b200.differentiable(kaldi=True); F.phase_vocoder and TimeStretch compute spectrogram "
             "gradients, F.pitch_shift and PitchShift waveform gradients, inside audio_b200.differentiable(vocoder=True); F.lfilter, "
             "F.filtfilt, the *_biquad filters, F.preemphasis, F.deemphasis, Preemphasis and Deemphasis compute waveform and "
-            "coefficient gradients, and F.fftconvolve and FFTConvolve the gradients of both operands, inside "
+            "coefficient gradients, and F.convolve, Convolve, F.fftconvolve and FFTConvolve the gradients of both operands, "
+            "inside "
             "audio_b200.differentiable(filtering=True).)"
         )
 

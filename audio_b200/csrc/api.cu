@@ -526,5 +526,25 @@ int b200a_fftconvolve_backward(const b200a_fftconvolve_desc* desc, const float* 
                                    static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_convolve_workspace_bytes(const b200a_convolve_desc* desc) {
+  return convolve_workspace_bytes_impl(desc, false);
+}
+
+size_t b200a_convolve_backward_workspace_bytes(const b200a_convolve_desc* desc) {
+  return convolve_workspace_bytes_impl(desc, true);
+}
+
+int b200a_convolve_run(const b200a_convolve_desc* desc, const float* x, const float* y, float* out, void* workspace,
+                       size_t workspace_bytes, b200a_stream stream) {
+  return convolve_run_impl(desc, x, y, out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int b200a_convolve_backward(const b200a_convolve_desc* desc, const float* x, const float* y, const float* grad,
+                            float* grad_x, float* grad_y, void* workspace, size_t workspace_bytes,
+                            b200a_stream stream) {
+  return convolve_backward_impl(desc, x, y, grad, grad_x, grad_y, workspace, workspace_bytes,
+                                static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -178,6 +178,12 @@ int fftconvolve_run_impl(const b200a_fftconvolve_desc* d, const float* x, const 
                          size_t ws_bytes, cudaStream_t stream);
 int fftconvolve_backward_impl(const b200a_fftconvolve_desc* d, const float* x, const float* y, const float* grad,
                               float* grad_x, float* grad_y, void* ws, size_t ws_bytes, cudaStream_t stream);
+// convolve_direct.cu
+size_t convolve_workspace_bytes_impl(const b200a_convolve_desc* d, bool backward);
+int convolve_run_impl(const b200a_convolve_desc* d, const float* x, const float* y, float* out, void* ws,
+                      size_t ws_bytes, cudaStream_t stream);
+int convolve_backward_impl(const b200a_convolve_desc* d, const float* x, const float* y, const float* grad,
+                           float* grad_x, float* grad_y, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

@@ -15,7 +15,8 @@ gradient of ``inverse_spectrogram`` inside ``audio_b200.differentiable(inverse=T
 ``audio_b200.differentiable(features=True)``, and the spectrogram gradient of ``phase_vocoder`` and the waveform
 gradient of ``pitch_shift`` inside ``audio_b200.differentiable(vocoder=True)``, and the waveform and coefficient
 gradients of ``lfilter``, ``filtfilt``, the ``*_biquad`` filters, ``preemphasis`` and ``deemphasis``, and the input
-gradients of ``fftconvolve``, inside ``audio_b200.differentiable(filtering=True)``.  ``griffinlim`` is forward-only.
+gradients of ``fftconvolve`` and ``convolve``, inside ``audio_b200.differentiable(filtering=True)``.  ``griffinlim`` is
+forward-only.
 
 IIR filtering (reference functional/filtering.py): ``lfilter`` (1032-1099), ``filtfilt`` (672-710), ``biquad`` and the
 ``allpass`` / ``band`` / ``bandpass`` / ``bandreject`` / ``bass`` / ``deemph`` / ``equalizer`` / ``highpass`` /
@@ -23,7 +24,8 @@ IIR filtering (reference functional/filtering.py): ``lfilter`` (1032-1099), ``fi
 all on one chunked-scan kernel family; filter orders up to 16.
 
 FFT convolution: ``fftconvolve`` (functional.py:2222-2258), uniformly partitioned overlap-save on the kernels of
-``csrc/convolve.cu``.
+``csrc/convolve.cu``.  Direct convolution: ``convolve`` (functional.py:2261-2314), a banded TF32 x 3 tensor-core
+product on the kernels of ``csrc/convolve_direct.cu``, for filters up to 4096 taps.
 """
 from __future__ import annotations
 
@@ -79,6 +81,7 @@ __all__ = [
     "preemphasis",
     "deemphasis",
     "fftconvolve",
+    "convolve",
 ]
 
 
@@ -780,27 +783,71 @@ def _convolve_slice(n: int, m: int, mode: str):
     return lo, max(hi - lo, 0)
 
 
-class _FFTConvolveFunction(torch.autograd.Function):
-    """b200audio::fftconvolve on the operand rows with b200audio::fftconvolve_backward as its backward.  Saved
-    (save_for_backward): the two operands' rows only.  The per-output-row gradients are summed onto the operand rows
-    that broadcasting shared (``sum_to_size``: a fixed-order reduction, no atomics)."""
+def _conv_function(name: str, run, backward_op):
+    """An autograd Function for an operand-row convolution op (``run``: b200audio::fftconvolve or b200audio::convolve)
+    with ``backward_op`` as its backward.  Saved (save_for_backward): the two operands' rows only.  The per-output-row
+    gradients are summed onto the operand rows that broadcasting shared (``sum_to_size``: a fixed-order reduction, no
+    atomics)."""
 
-    @staticmethod
-    def forward(ctx, x2, y2, ix, iy, start, out_len, shapes):
-        ctx.save_for_backward(x2, y2)
-        ctx.ix, ctx.iy, ctx.start, ctx.shapes = ix, iy, start, shapes
-        return _ops.fftconvolve(x2, y2, ix, iy, start, out_len)
+    class Fn(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, x2, y2, ix, iy, start, out_len, shapes):
+            ctx.save_for_backward(x2, y2)
+            ctx.ix, ctx.iy, ctx.start, ctx.shapes = ix, iy, start, shapes
+            return run(x2, y2, ix, iy, start, out_len)
 
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        x2, y2 = ctx.saved_tensors
-        gx, gy = _ops.fftconvolve_backward(g, x2, y2, ctx.ix, ctx.iy, ctx.start)
-        lo, lx, ly = ctx.shapes
-        need = ctx.needs_input_grad
-        gx = gx.reshape(lo + (x2.shape[1],)).sum_to_size(lx + (x2.shape[1],)).reshape(x2.shape) if need[0] else None
-        gy = gy.reshape(lo + (y2.shape[1],)).sum_to_size(ly + (y2.shape[1],)).reshape(y2.shape) if need[1] else None
-        return gx, gy, None, None, None, None, None
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, g):
+            x2, y2 = ctx.saved_tensors
+            gx, gy = backward_op(g, x2, y2, ctx.ix, ctx.iy, ctx.start)
+            lo, lx, ly = ctx.shapes
+            need = ctx.needs_input_grad
+            gx = gx.reshape(lo + (x2.shape[1],)).sum_to_size(lx + (x2.shape[1],)).reshape(x2.shape) if need[0] else None
+            gy = gy.reshape(lo + (y2.shape[1],)).sum_to_size(ly + (y2.shape[1],)).reshape(y2.shape) if need[1] else None
+            return gx, gy, None, None, None, None, None
+
+    Fn.__name__ = Fn.__qualname__ = name
+    Fn.run = staticmethod(run)
+    return Fn
+
+
+_FFTConvolveFunction = _conv_function("_FFTConvolveFunction", _ops.fftconvolve, _ops.fftconvolve_backward)
+_ConvolveFunction = _conv_function("_ConvolveFunction", _ops.convolve, _ops.convolve_backward)
+
+
+def _convolve_operands(x: Tensor, y: Tensor, mode: str):
+    """The checks fftconvolve and convolve share, in the reference's order, then the package's: shapes, mode, CUDA
+    float32, one device.  Returns (n, m, lx, ly, lo): the lengths, both operands' leading shapes and the output's."""
+    _check_shape_compatible(x, y)
+    _check_convolve_mode(mode)
+    _require_cuda_f32(x, "x")
+    _require_cuda_f32(y, "y")
+    if y.device != x.device:
+        raise RuntimeError(f"audio_b200: y is on {y.device} but x is on {x.device}")
+    lx, ly = tuple(x.shape[:-1]), tuple(y.shape[:-1])
+    return x.shape[-1], y.shape[-1], lx, ly, tuple(torch.broadcast_shapes(lx, ly))
+
+
+def _convolve_rows(fn, x: Tensor, y: Tensor, lx, ly, lo, start: int, out_len: int) -> Tensor:
+    """Runs ``fn`` (a _conv_function) on the operands' rows for the output slice [start, start + out_len) of every
+    output row, under the filtering gradient switch; returns the (lo..., out_len) output."""
+    x2, _ = pack_rows(x)
+    y2, _ = pack_rows(y)
+    dev = x.device
+    # output row -> operand row, by broadcasting the operands' row numbers on the device (no host synchronisation); the
+    # kernels read one int64 per output row, so the vectors are materialised (a broadcast view may have stride 0)
+    ix = torch.arange(x2.shape[0], device=dev).reshape(lx).broadcast_to(lo).contiguous().reshape(-1)
+    iy = torch.arange(y2.shape[0], device=dev).reshape(ly).broadcast_to(lo).contiguous().reshape(-1)
+    grad = torch.is_grad_enabled() and (x.requires_grad or y.requires_grad)
+    if grad and not is_filtering_differentiable():
+        _no_autograd(x)
+        _no_autograd(y)
+    if grad:
+        out = fn.apply(x2, y2, ix, iy, start, out_len, (lo, lx, ly))
+    else:
+        out = fn.run(x2, y2, ix, iy, start, out_len)
+    return out.reshape(lo + (out_len,))
 
 
 def fftconvolve(x: Tensor, y: Tensor, mode: str = "full") -> Tensor:
@@ -809,15 +856,7 @@ def fftconvolve(x: Tensor, y: Tensor, mode: str = "full") -> Tensor:
     max(N, M) - min(N, M) + 1 (``"valid"``) or N (``"same"``).  Runs uniformly partitioned overlap-save
     (``csrc/convolve.cu``): the shorter operand is cut into blocks of B = 256 .. 2048 samples, and only the output
     blocks the mode returns are computed.  The shorter operand may have up to 128 * 2048 = 262144 samples."""
-    _check_shape_compatible(x, y)
-    _check_convolve_mode(mode)
-    _require_cuda_f32(x, "x")
-    _require_cuda_f32(y, "y")
-    if y.device != x.device:
-        raise RuntimeError(f"audio_b200: y is on {y.device} but x is on {x.device}")
-    n, m = x.shape[-1], y.shape[-1]
-    lx, ly = tuple(x.shape[:-1]), tuple(y.shape[:-1])
-    lo = tuple(torch.broadcast_shapes(lx, ly))
+    n, m, lx, ly, lo = _convolve_operands(x, y, mode)
     if n + m - 1 <= 0:  # what torch.fft.rfft reports for the reference's n = N + M - 1 points
         raise RuntimeError(f"Invalid number of data points ({n + m - 1}) specified")
     start, out_len = _convolve_slice(n, m, mode)
@@ -832,19 +871,30 @@ def fftconvolve(x: Tensor, y: Tensor, mode: str = "full") -> Tensor:
             f"{_lib.FFTCONVOLVE_MAX_PARTITIONS * block} samples")
     if math.prod(lo) == 0:
         return x.new_empty(lo + (out_len,))
-    x2, _ = pack_rows(x)
-    y2, _ = pack_rows(y)
-    dev = x.device
-    # output row -> operand row, by broadcasting the operands' row numbers on the device (no host synchronisation); the
-    # kernels read one int64 per output row, so the vectors are materialised (a broadcast view may have stride 0)
-    ix = torch.arange(x2.shape[0], device=dev).reshape(lx).broadcast_to(lo).contiguous().reshape(-1)
-    iy = torch.arange(y2.shape[0], device=dev).reshape(ly).broadcast_to(lo).contiguous().reshape(-1)
-    grad = torch.is_grad_enabled() and (x.requires_grad or y.requires_grad)
-    if grad and not is_filtering_differentiable():
-        _no_autograd(x)
-        _no_autograd(y)
-    if grad:
-        out = _FFTConvolveFunction.apply(x2, y2, ix, iy, start, out_len, (lo, lx, ly))
-    else:
-        out = _ops.fftconvolve(x2, y2, ix, iy, start, out_len)
-    return out.reshape(lo + (out_len,))
+    return _convolve_rows(_FFTConvolveFunction, x, y, lx, ly, lo, start, out_len)
+
+
+def convolve(x: Tensor, y: Tensor, mode: str = "full") -> Tensor:
+    """Convolves ``x (..., N)`` and ``y (..., M)`` along their last dimension using the direct method (reference
+    functional.py:2261-2314): the true convolution, leading dimensions broadcast, output ``(..., L)`` with
+    L = N + M - 1 (``"full"``), max(N, M) - min(N, M) + 1 (``"valid"``) or N (``"same"``).  Runs a banded Toeplitz
+    product on TF32 x 3 tensor-core MMAs at float32 grade (``csrc/convolve_direct.cu``), and only the outputs the mode
+    returns are computed.  The shorter operand (the filter) may have up to 4096 taps; longer filters are the job of
+    ``fftconvolve``."""
+    n, m, lx, ly, lo = _convolve_operands(x, y, mode)
+    if lx != ly:  # the reference broadcasts to the per-dimension maximum, which refuses a 0 against a 1
+        big, small = (y, x) if n < m else (x, y)
+        new = [max(i, j) for i, j in zip(big.shape[:-1], small.shape[:-1])]
+        big.broadcast_to(new + [big.shape[-1]])
+        small.broadcast_to(new + [small.shape[-1]])
+    if math.prod(lo) == 0:  # the reference's grouped conv1d with zero groups
+        raise RuntimeError("non-positive groups is not supported")
+    if n == 0 or m == 0:  # and with padding min(N, M) - 1 < 0
+        raise RuntimeError("negative padding is not supported")
+    k = min(n, m)
+    if k > _lib.CONVOLVE_MAX_TAPS:
+        raise RuntimeError(
+            f"audio_b200: convolve of a {k}-sample shorter operand is not supported: the direct method is capped at "
+            f"{_lib.CONVOLVE_MAX_TAPS} taps (B200A_CONVOLVE_MAX_TAPS); use fftconvolve for longer filters")
+    start, out_len = _convolve_slice(n, m, mode)
+    return _convolve_rows(_ConvolveFunction, x, y, lx, ly, lo, start, out_len)

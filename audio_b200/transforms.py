@@ -14,8 +14,8 @@ Gradients are opt-in, per thread: Spectrogram and MelSpectrogram inside ``audio_
 InverseSpectrogram with ``inverse=True``, Resample / Speed / SpeedPerturbation with ``resample=True``, and MFCC,
 LFCC, AmplitudeToDB, MelScale, InverseMelScale and SpectralCentroid with ``features=True``, the Kaldi features
 (``audio_b200.compliance.kaldi``) with ``kaldi=True``, TimeStretch (spectrogram gradient) and PitchShift
-(waveform gradient) with ``vocoder=True``, and Preemphasis and Deemphasis (waveform gradient) and FFTConvolve (input
-gradients) with ``filtering=True``.
+(waveform gradient) with ``vocoder=True``, and Preemphasis and Deemphasis (waveform gradient) and Convolve and
+FFTConvolve (input gradients) with ``filtering=True``.
 GriffinLim is forward-only.
 """
 from __future__ import annotations
@@ -34,7 +34,7 @@ from ._plans import (FrontendPlan, InverseMelPlan, ResamplePlan, _InverseMelFunc
 
 __all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "InverseMelScale", "MelSpectrogram", "MFCC", "LFCC",
            "SpectralCentroid", "Resample", "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift", "Preemphasis",
-           "Deemphasis", "FFTConvolve"]
+           "Deemphasis", "FFTConvolve", "Convolve"]
 
 
 def _setup_framing(mod, n_fft, win_length, hop_length, window_fn=None, wkwargs=None, hop_div=2):
@@ -738,6 +738,19 @@ class FFTConvolve(torch.nn.Module):
 
     def forward(self, x: Tensor, y: Tensor) -> Tensor:
         return F.fftconvolve(x, y, mode=self.mode)
+
+
+class Convolve(torch.nn.Module):
+    """Convolves inputs along their last dimension using the direct method (reference _transforms.py:1863-1903):
+    ``F.convolve(x, y, mode)``, a banded TF32 x 3 tensor-core product on the GPU, for filters up to 4096 taps."""
+
+    def __init__(self, mode: str = "full") -> None:
+        F._check_convolve_mode(mode)
+        super().__init__()
+        self.mode = mode
+
+    def forward(self, x: Tensor, y: Tensor) -> Tensor:
+        return F.convolve(x, y, mode=self.mode)
 
 
 # ---- B200A_REFERENCE=1: A/B switch to the reference implementation (debugging only, never silent) -----------------

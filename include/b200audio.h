@@ -586,6 +586,43 @@ int b200a_fftconvolve_backward(const b200a_fftconvolve_desc* desc, const float* 
                                float* grad_x, float* grad_y, void* workspace, size_t workspace_bytes,
                                b200a_stream stream);
 
+/* ---- direct convolution: convolve (functional/functional.py:2261-2314) ------------------------------------------ */
+/*
+ * The same result as b200a_fftconvolve_run, by the direct method: the filter (the shorter operand, K = min(n, m) taps;
+ * y when n == m) times the signal as a banded Toeplitz product on TF32 x 3 tensor-core MMAs (round-to-nearest splits
+ * and per-k-step round-to-nearest accumulation: float32 grade), 128 consecutive outputs per m16n8 tile over ceil((K + 7) / 8) k-steps.  Tile sizes depend on K alone and
+ * nothing is atomic: reruns are bit-identical and a row's output does not depend on the other rows.  The descriptor is
+ * b200a_fftconvolve_desc with the same meaning.
+ */
+#define B200A_CONVOLVE_MAX_TAPS 4096 /* K cap (B200A_EUNSUPPORTED above): past it fftconvolve does less work */
+
+typedef b200a_fftconvolve_desc b200a_convolve_desc;
+
+/* Workspace bytes of b200a_convolve_run / b200a_convolve_backward for `desc`; 0 for an invalid or unsupported
+ * descriptor. */
+size_t b200a_convolve_workspace_bytes(const b200a_convolve_desc* desc);
+size_t b200a_convolve_backward_workspace_bytes(const b200a_convolve_desc* desc);
+/*
+ *   out : [rows][out_len] contiguous, every element written once
+ * B200A_EINVAL for a null pointer, a length < 1, negative sizes or strides, or a slice outside the full range;
+ * B200A_EUNSUPPORTED for K > B200A_CONVOLVE_MAX_TAPS or n + m - 1 > INT32_MAX; B200A_EWORKSPACE when workspace_bytes
+ * is too small.  rows == 0 or out_len == 0 enqueues nothing.
+ */
+int b200a_convolve_run(const b200a_convolve_desc* desc, const float* x, const float* y, float* out, void* workspace,
+                       size_t workspace_bytes, b200a_stream stream);
+/*
+ * Gradients of b200a_convolve_run, per OUTPUT row, as b200a_fftconvolve_backward defines them:
+ *   grad_x[r][k] = sum_j g[k + j] y_r[j],  grad_y[r][j] = sum_k g[k + j] x_r[k]
+ * with g = grad[r] placed at `start` of the full range.  The signal gradient is the forward kernel on g with the
+ * reversed filter; the filter gradient is a tensor-core correlation per 2048-sample tile, whose partials are summed in
+ * tile order.  The caller sums the rows that share an operand.
+ *   grad   : [rows][out_len] contiguous
+ *   grad_x : [rows][n] contiguous;  grad_y : [rows][m] contiguous
+ * Statuses as b200a_convolve_run; out_len == 0 zero-fills both gradients.
+ */
+int b200a_convolve_backward(const b200a_convolve_desc* desc, const float* x, const float* y, const float* grad,
+                            float* grad_x, float* grad_y, void* workspace, size_t workspace_bytes, b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);

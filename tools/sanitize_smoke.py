@@ -93,5 +93,10 @@ with audio_b200.differentiable(filtering=True):
     xg = x.clone().requires_grad_()
     F.fftconvolve(torch.randn(1, 1, 2500, device="cuda", requires_grad=True), xg[:, None, :3000]).sum().backward()
 F.fftconvolve(x, torch.randn(3, 255, device="cuda"), "same")
+# direct convolution: a broadcast filter forward + backward (swapped operands), and "same" with fragments streamed
+with audio_b200.differentiable(filtering=True):
+    xg = x.clone().requires_grad_()
+    F.convolve(torch.randn(1, 1, 200, device="cuda", requires_grad=True), xg[:, None, :3000]).sum().backward()
+F.convolve(x, torch.randn(3, 1025, device="cuda"), "same")
 torch.cuda.synchronize()
 print("done")
