@@ -6,18 +6,22 @@ inside ``audio_b200.differentiable(filtering=True)`` the waveform and coefficien
 The biquad designs are the Audio-EQ-Cookbook and SoX formulas, evaluated with torch scalar ops in the waveform's dtype
 and device, so a tensor ``cutoff_freq`` / ``Q`` / ``gain`` that requires grad gets its gradient through the
 coefficient gradient.  The ``_design_*`` helpers return ``(b, a)`` as lists of three coefficients and run on any device.
+
+``vad`` (filtering.py:1414-1702) measures on two front-end passes around the per-bin walk and the trigger kernel of
+``csrc/vad.cu`` (b200audio::vad_walk, b200audio::vad_trigger) and returns a view of its input.
 """
 from __future__ import annotations
 
 import math
-from typing import List, Tuple
+import warnings
+from typing import List, Optional, Tuple
 
 import torch
 from torch import Tensor
 from torch.autograd.function import once_differentiable
 
 from . import _lib, _ops
-from ._plans import _no_autograd, _require_cuda_f32, is_filtering_differentiable, pack_rows
+from ._plans import FrontendPlan, _no_autograd, _require_cuda_f32, is_filtering_differentiable, pack_rows
 
 
 class _LfilterFunction(torch.autograd.Function):
@@ -317,3 +321,200 @@ def deemphasis(waveform: Tensor, coeff: float = 0.97) -> Tensor:
     a = torch.tensor([1.0, -coeff], dtype=waveform.dtype, device=waveform.device)
     b = torch.tensor([1.0, 0.0], dtype=waveform.dtype, device=waveform.device)
     return lfilter(waveform, a, b)
+
+
+# ---- vad (reference filtering.py:1414-1702) -----------------------------------------------------------------------
+VAD_CHUNK = 1024  # measurement frames per chunk: 51 s at the default 20 Hz; the status is read back once per chunk
+
+
+class VadPlan:
+    """The host constants of one vad parameter set, computed with the reference's own Python-float and CPU-tensor
+    arithmetic (filtering.py:1579-1629, so its errors are raised here, in its order), and per device the uploaded
+    windows and the two prepared front-end workspaces: the measurement FFT (|X|, power 1) and the cepstrum FFT (power 2
+    summed over the lifter band by a one-column indicator bank)."""
+
+    def __init__(self, sample_rate, trigger_level=7.0, trigger_time=0.25, search_time=1.0, allowed_gap=0.25,
+                 pre_trigger_time=0.0, boot_time=0.35, noise_up_time=0.1, noise_down_time=0.01,
+                 noise_reduction_amount=1.35, measure_freq=20.0, measure_duration=None, measure_smooth_time=0.4,
+                 hp_filter_freq=50.0, lp_filter_freq=6000.0, hp_lifter_freq=150.0, lp_lifter_freq=2000.0):
+        measure_duration = 2.0 / measure_freq if measure_duration is None else measure_duration
+        self.measure_len_ws = measure_len_ws = int(sample_rate * measure_duration + 0.5)
+        dft_len_ws = 16
+        while dft_len_ws < measure_len_ws:
+            dft_len_ws *= 2
+        self.dft_len_ws = dft_len_ws
+        self.measure_period_ns = int(sample_rate / measure_freq + 0.5)
+        self.measures_len = math.ceil(search_time * measure_freq)
+        self.gap_len = int(allowed_gap * measure_freq + 0.5)
+        self.fixed_pre_trigger_len_ns = int(pre_trigger_time * sample_rate + 0.5)
+        self.samples_len_ns = (self.fixed_pre_trigger_len_ns + self.measures_len * self.measure_period_ns
+                               + measure_len_ws)
+        self.spectrum_window = torch.zeros(measure_len_ws)
+        self.spectrum_window[:] = 2.0 / math.sqrt(float(measure_len_ws))
+        self.spectrum_window *= torch.hann_window(measure_len_ws, dtype=torch.float)
+        s0 = max(int(hp_filter_freq / sample_rate * dft_len_ws + 0.5), 1)
+        s1 = min(int(lp_filter_freq / sample_rate * dft_len_ws + 0.5), dft_len_ws // 2)
+        self.spectrum_start, self.spectrum_end = s0, s1
+        self.cepstrum_window = torch.zeros(s1 - s0)
+        self.cepstrum_window[:] = 2.0 / math.sqrt(float(s1) - s0)
+        self.cepstrum_window *= torch.hann_window(s1 - s0, dtype=torch.float)
+        c0 = math.ceil(sample_rate * 0.5 / lp_lifter_freq)
+        c1 = min(math.floor(sample_rate * 0.5 / hp_lifter_freq), dft_len_ws // 4)
+        if c1 <= c0:
+            raise ValueError(
+                "Expected cepstrum_start to be smaller than cepstrum_end."
+                f"Found: cepstrum_start: {c0}, cepstrum_end: {c1}."
+            )
+        self.cepstrum_start, self.cepstrum_end = c0, c1
+        self.noise_up_time_mult = math.exp(-1.0 / (noise_up_time * measure_freq))
+        self.noise_down_time_mult = math.exp(-1.0 / (noise_down_time * measure_freq))
+        self.measure_smooth_time_mult = math.exp(-1.0 / (measure_smooth_time * measure_freq))
+        self.trigger_meas_time_mult = math.exp(-1.0 / (trigger_time * measure_freq))
+        self.boot_count_max = int(boot_time * measure_freq - 0.5)
+        self.noise_reduction_amount = noise_reduction_amount
+        self.trigger_level = trigger_level
+        self._devices = {}
+
+    def desc(self, channels: int) -> "_lib.VadDesc":
+        return _lib.VadDesc(
+            channels=channels, dft_len=self.dft_len_ws, spectrum_start=self.spectrum_start,
+            spectrum_end=self.spectrum_end, cepstrum_start=self.cepstrum_start, cepstrum_end=self.cepstrum_end,
+            measures_len=self.measures_len, gap_len=self.gap_len, boot_count_max=self.boot_count_max,
+            period=self.measure_period_ns, fixed_pre_trigger=self.fixed_pre_trigger_len_ns,
+            noise_up_mult=self.noise_up_time_mult, noise_down_mult=self.noise_down_time_mult,
+            noise_reduction_amount=self.noise_reduction_amount, measure_smooth_mult=self.measure_smooth_time_mult,
+            trigger_mult=self.trigger_meas_time_mult, trigger_level=self.trigger_level)
+
+    def num_frames(self, length: int) -> int:
+        """Measurement frames the reference runs on `length` samples: len(range(measure_len_ws, length, period))."""
+        return len(range(self.measure_len_ws, length, self.measure_period_ns))
+
+    def device_state(self, device: torch.device):
+        """(measurement plan, its workspace, cepstrum plan, its workspace, cepstrum window) on ``device``."""
+        key = str(device)
+        state = self._devices.get(key)
+        if state is not None:
+            return state
+        if self.dft_len_ws > _lib.VAD_MAX_DFT:
+            raise RuntimeError(
+                f"audio_b200: vad with dft_len_ws = {self.dft_len_ws} (sample_rate * measure_duration = "
+                f"{self.measure_len_ws} samples) is not supported: the measurement FFT is capped at {_lib.VAD_MAX_DFT} "
+                "points (about 82 kHz at the default measure_duration); resample the input first")
+        half = self.dft_len_ws // 2
+        measure = FrontendPlan(FrontendPlan.make_desc(self.dft_len_ws, self.measure_len_ws, self.measure_period_ns, 0,
+                                                      False, "constant", True, False, False, 1.0))
+        cepstrum = FrontendPlan(FrontendPlan.make_desc(half, half, half, 0, False, "constant", True, False, False, 2.0,
+                                                       n_mels=1))
+        lifter = torch.zeros(half // 2 + 1, 1)
+        lifter[self.cepstrum_start:self.cepstrum_end] = 1.0
+        ones = torch.ones(half, device=device)
+        state = (measure, measure.workspace(self.spectrum_window.to(device), None, None), cepstrum,
+                 cepstrum.workspace(ones, lifter.to(device), None), self.cepstrum_window.to(device))
+        self._devices[key] = state
+        return state
+
+    def run(self, x: Tensor, chunk: int = VAD_CHUNK, keep_measures: bool = False):
+        """Measure the (C, L) CUDA float32 rows chunk by chunk until a frame triggers.  Returns (trigger frame or -1,
+        trim start, the float32 measures of the frames run as a (C, frames) tensor or None)."""
+        channels, length = x.shape
+        frames = self.num_frames(length)
+        if channels == 0 or frames == 0:
+            return -1, 0, x.new_zeros(channels, 0) if keep_measures else None
+        if self.measures_len < 1:
+            raise RuntimeError(f"audio_b200: vad with search_time * measure_freq <= 0 (a measure ring of "
+                               f"{self.measures_len} frames) is not supported")
+        measure, ws_measure, cepstrum, ws_cepstrum, cep_window = self.device_state(x.device)
+        m_i, m_f = measure._packed_desc()
+        c_i, c_f = cepstrum._packed_desc()
+        desc_i, desc_f = _ops.pack_vad_desc(self.desc(channels))
+        dft, period, half = self.dft_len_ws, self.measure_period_ns, self.dft_len_ws // 2
+        chunk = min(int(chunk), frames)
+        lib = _lib.lib()
+        nbytes = lib.b200a_vad_workspace_bytes(self.desc(channels), chunk)
+        if nbytes == 0:
+            raise _lib.B200AudioError(_lib.EUNSUPPORTED, "vad_workspace_bytes (descriptor rejected)")
+        # the measured signal: (dft - ws) // 2 leading zeros centre the window in the FFT buffer as the reference's
+        # left-aligned one (|X| is the same under the circular shift), trailing zeros complete the last frame
+        left = (dft - self.measure_len_ws) // 2
+        padded = x.new_zeros(channels, (frames - 1) * period + dft)
+        n_copy = min(length, padded.shape[1] - left)
+        padded[:, left:left + n_copy] = x[:, :n_copy]
+        rows = x.new_zeros(channels, chunk * half)  # cepstrum rows; bins outside [s0, s1) stay zero
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+        kept = []
+        for f0 in range(0, frames, chunk):
+            k = min(chunk, frames - f0)
+            span = padded[:, f0 * period:f0 * period + (k - 1) * period + dft]
+            spec = _ops.frontend_run(span, ws_measure, m_i, m_f, _lib.STAGE_POWER, k, half + 1, padded.stride(0), None, 1)
+            _ops.vad_walk(spec, cep_window, rows, ws, desc_i, desc_f, chunk, f0)
+            power = _ops.frontend_run(rows[:, :k * half], ws_cepstrum, c_i, c_f, _lib.STAGE_MEL, k, 1, chunk * half,
+                                      None, 1)
+            meas = _ops.vad_trigger(power.view(channels, k), ws, desc_i, desc_f, chunk, f0)
+            if keep_measures:
+                kept.append(meas)
+            trigger, start = ws[:16].view(torch.int64).tolist()
+            if trigger >= 0:
+                break
+        return trigger, start, torch.cat(kept, 1) if keep_measures else None
+
+
+_VAD_PLANS: "dict[tuple, VadPlan]" = {}
+
+
+def vad_plan(sample_rate, *args) -> VadPlan:
+    """One VadPlan per parameter tuple (the plan keeps one device state per device)."""
+    key = (sample_rate,) + tuple(args)
+    plan = _VAD_PLANS.get(key)
+    if plan is None:
+        plan = VadPlan(sample_rate, *args)
+        if len(_VAD_PLANS) >= 64:
+            _VAD_PLANS.pop(next(iter(_VAD_PLANS)))
+        _VAD_PLANS[key] = plan
+    return plan
+
+
+def _warn_batch(waveform: Tensor) -> None:
+    if waveform.ndim > 2:
+        warnings.warn(
+            "Expected input tensor dimension of 1 for single channel"
+            f" or 2 for multi-channel. Got {waveform.ndim} instead. "
+            "Batch semantics is not supported. "
+            "Please refer to https://github.com/pytorch/audio/issues/1348"
+            " and https://github.com/pytorch/audio/issues/1468."
+        )
+
+
+def _vad_trim(waveform: Tensor, plan: VadPlan, chunk: int = VAD_CHUNK) -> Tensor:
+    """The reference's batch packing and output slicing (filtering.py:1632-1702) around ``plan.run``: the result is a
+    view of ``waveform``, so autograd through the trim is the reference's."""
+    _require_cuda_f32(waveform, "waveform")
+    shape = waveform.size()
+    waveform = waveform.view(-1, shape[-1])
+    trigger, start, _ = plan.run(waveform.detach(), chunk)
+    fixed_pre = plan.fixed_pre_trigger_len_ns
+    if trigger < 0:
+        if shape[-1] >= fixed_pre:
+            return waveform[..., :fixed_pre].view(shape[:-1] + torch.Size([fixed_pre]))
+        frames = plan.num_frames(shape[-1])
+        pos = plan.measure_len_ws + (frames - 1) * plan.measure_period_ns if frames > 0 else 0
+        start = max(pos - plan.samples_len_ns, 0)
+    res = waveform[:, start:]
+    return res.view(shape[:-1] + res.shape[-1:])
+
+
+def vad(waveform: Tensor, sample_rate: int, trigger_level: float = 7.0, trigger_time: float = 0.25,
+        search_time: float = 1.0, allowed_gap: float = 0.25, pre_trigger_time: float = 0.0, boot_time: float = 0.35,
+        noise_up_time: float = 0.1, noise_down_time: float = 0.01, noise_reduction_amount: float = 1.35,
+        measure_freq: float = 20.0, measure_duration: Optional[float] = None, measure_smooth_time: float = 0.4,
+        hp_filter_freq: float = 50.0, lp_filter_freq: float = 6000.0, hp_lifter_freq: float = 150.0,
+        lp_lifter_freq: float = 2000.0) -> Tensor:
+    """Voice-activity trim from the front of ``(..., time)`` audio, as SoX's vad (reference filtering.py:1485-1702):
+    every leading dimension is one channel of a single recording, trimmed jointly to the earliest activity in any
+    channel.  Returns a view of ``waveform``; a waveform that requires grad gets 1 on the kept samples and 0 on the
+    trimmed ones.  The measurements run on the GPU in chunks of frames and stop at the first triggering chunk;
+    ``sample_rate * measure_duration`` is capped at 8192 samples (the measurement FFT)."""
+    _warn_batch(waveform)
+    plan = vad_plan(sample_rate, trigger_level, trigger_time, search_time, allowed_gap, pre_trigger_time, boot_time,
+                    noise_up_time, noise_down_time, noise_reduction_amount, measure_freq, measure_duration,
+                    measure_smooth_time, hp_filter_freq, lp_filter_freq, hp_lifter_freq, lp_lifter_freq)
+    return _vad_trim(waveform, plan)

@@ -23,6 +23,7 @@ INVERSE_MEL_MAX_BANDWIDTH, INVERSE_MEL_MAX_MELS = 4, 512  # B200A_INVERSE_MEL_MA
 LFILTER_MAX_ORDER = 16  # B200A_LFILTER_MAX_ORDER
 FFTCONVOLVE_MAX_PARTITIONS, FFTCONVOLVE_MAX_BLOCK = 128, 2048  # B200A_FFTCONVOLVE_MAX_PARTITIONS; the largest block
 CONVOLVE_MAX_TAPS = 4096  # B200A_CONVOLVE_MAX_TAPS
+VAD_MAX_DFT = 8192  # the largest dft_len of b200a_vad_desc
 
 
 class FrontendDesc(ctypes.Structure):
@@ -85,6 +86,30 @@ class FftconvolveDesc(ctypes.Structure):
         ("y_index", c_void_p),
         ("x_stride", c_int64),
         ("y_stride", c_int64),
+    ]
+
+
+class VadDesc(ctypes.Structure):
+    """Mirror of ``b200a_vad_desc``."""
+
+    _fields_ = [
+        ("channels", c_int32),
+        ("dft_len", c_int32),
+        ("spectrum_start", c_int32),
+        ("spectrum_end", c_int32),
+        ("cepstrum_start", c_int32),
+        ("cepstrum_end", c_int32),
+        ("measures_len", c_int32),
+        ("gap_len", c_int32),
+        ("boot_count_max", c_int32),
+        ("period", c_int32),
+        ("fixed_pre_trigger", c_int64),
+        ("noise_up_mult", c_double),
+        ("noise_down_mult", c_double),
+        ("noise_reduction_amount", c_double),
+        ("measure_smooth_mult", c_double),
+        ("trigger_mult", c_double),
+        ("trigger_level", c_double),
     ]
 
 
@@ -244,6 +269,15 @@ _SIGNATURES = {
     "b200a_convolve_backward": (
         ctypes.c_int,
         [POINTER(FftconvolveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_vad_workspace_bytes": (c_size_t, [POINTER(VadDesc), c_int64]),
+    "b200a_vad_walk": (
+        ctypes.c_int,
+        [POINTER(VadDesc), c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_vad_trigger": (
+        ctypes.c_int,
+        [POINTER(VadDesc), c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
     ),
 }
 

@@ -3,7 +3,7 @@ capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` 
 ``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
 ``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward`` / ``rnnt_features`` /
 ``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward`` / ``lfilter`` / ``lfilter_backward`` /
-``fftconvolve`` / ``fftconvolve_backward`` / ``convolve`` / ``convolve_backward``.
+``fftconvolve`` / ``fftconvolve_backward`` / ``convolve`` / ``convolve_backward`` / ``vad_walk`` / ``vad_trigger``.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -90,6 +90,13 @@ _LIB.define(
 _LIB.define("convolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor")
 _LIB.define(
     "convolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)"
+)
+_LIB.define(
+    "vad_walk(Tensor spectrum, Tensor cepstrum_window, Tensor(a!) rows, Tensor(b!) workspace, int[] desc_i, "
+    "float[] desc_f, int chunk, int frame0) -> ()"
+)
+_LIB.define(
+    "vad_trigger(Tensor power, Tensor(a!) workspace, int[] desc_i, float[] desc_f, int chunk, int frame0) -> Tensor"
 )
 
 _KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
@@ -637,6 +644,58 @@ def _convolve_backward_cuda(grad, x, y, x_index, y_index, start):
     return _conv_backward("convolve", grad, x, y, x_index, y_index, start)
 
 
+# ---- vad_walk / vad_trigger ----------------------------------------------------------------------------------------
+_VAD_INTS = ("channels", "dft_len", "spectrum_start", "spectrum_end", "cepstrum_start", "cepstrum_end", "measures_len",
+             "gap_len", "boot_count_max", "period", "fixed_pre_trigger")
+_VAD_FLOATS = ("noise_up_mult", "noise_down_mult", "noise_reduction_amount", "measure_smooth_mult", "trigger_mult",
+               "trigger_level")
+
+
+def pack_vad_desc(d: "_lib.VadDesc"):
+    return [int(getattr(d, k)) for k in _VAD_INTS], [float(getattr(d, k)) for k in _VAD_FLOATS]
+
+
+def _unpack_vad_desc(desc_i: List[int], desc_f: List[float]) -> "_lib.VadDesc":
+    d = _lib.VadDesc()
+    for k, v in zip(_VAD_INTS, desc_i):
+        setattr(d, k, int(v))
+    for k, v in zip(_VAD_FLOATS, desc_f):
+        setattr(d, k, float(v))
+    return d
+
+
+def _vad_walk_cuda(spectrum, cepstrum_window, rows, workspace, desc_i, desc_f, chunk, frame0):
+    """(C, frames, dft/2+1) |X| of a chunk -> bins [s0, s1) of the first `frames` rows of the (C, chunk, dft/2) cepstrum
+    rows, carrying the smoothed spectrum and the noise estimate in ``workspace`` (b200a_vad_walk)."""
+    d = _unpack_vad_desc(desc_i, desc_f)
+    dev = spectrum.device
+    with torch.cuda.device(dev):
+        rc = _lib.lib().b200a_vad_walk(d, chunk, frame0, spectrum.shape[1], spectrum.data_ptr(), cepstrum_window.data_ptr(),
+                                       rows.data_ptr(), workspace.data_ptr(), workspace.numel(), _stream(dev))
+    _lib.check(rc, "vad_walk")
+
+
+def _vad_walk_meta(spectrum, cepstrum_window, rows, workspace, desc_i, desc_f, chunk, frame0):
+    return None
+
+
+def _vad_trigger_cuda(power, workspace, desc_i, desc_f, chunk, frame0):
+    """(C, frames) cepstral band powers of a chunk -> (C, frames) float32 measures; the trigger status goes to the first
+    16 bytes of ``workspace`` (b200a_vad_trigger)."""
+    d = _unpack_vad_desc(desc_i, desc_f)
+    dev = power.device
+    with torch.cuda.device(dev):
+        measures = torch.empty(power.shape, dtype=torch.float32, device=dev)
+        rc = _lib.lib().b200a_vad_trigger(d, chunk, frame0, power.shape[1], power.data_ptr(), measures.data_ptr(),
+                                          workspace.data_ptr(), workspace.numel(), _stream(dev))
+    _lib.check(rc, "vad_trigger")
+    return measures
+
+
+def _vad_trigger_meta(power, workspace, desc_i, desc_f, chunk, frame0):
+    return power.new_empty(power.shape)
+
+
 for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
                             ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
                             ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
@@ -659,7 +718,9 @@ for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_m
                             ("fftconvolve", _fftconvolve_cuda, _fftconvolve_meta),
                             ("fftconvolve_backward", _fftconvolve_backward_cuda, _fftconvolve_backward_meta),
                             ("convolve", _convolve_cuda, _fftconvolve_meta),
-                            ("convolve_backward", _convolve_backward_cuda, _fftconvolve_backward_meta)):
+                            ("convolve_backward", _convolve_backward_cuda, _fftconvolve_backward_meta),
+                            ("vad_walk", _vad_walk_cuda, _vad_walk_meta),
+                            ("vad_trigger", _vad_trigger_cuda, _vad_trigger_meta)):
     _LIB.impl(_name, _cuda, "CUDA")
     _LIB.impl(_name, _meta, "Meta")
 
@@ -686,3 +747,5 @@ fftconvolve = torch.ops.b200audio.fftconvolve
 fftconvolve_backward = torch.ops.b200audio.fftconvolve_backward
 convolve = torch.ops.b200audio.convolve
 convolve_backward = torch.ops.b200audio.convolve_backward
+vad_walk = torch.ops.b200audio.vad_walk
+vad_trigger = torch.ops.b200audio.vad_trigger

@@ -546,5 +546,22 @@ int b200a_convolve_backward(const b200a_convolve_desc* desc, const float* x, con
                                 static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_vad_workspace_bytes(const b200a_vad_desc* desc, int64_t chunk) {
+  return vad_workspace_bytes_impl(desc, chunk);
+}
+
+int b200a_vad_walk(const b200a_vad_desc* desc, int64_t chunk, int64_t frame0, int64_t frames, const float* spectrum,
+                   const float* cepstrum_window, float* rows, void* workspace, size_t workspace_bytes,
+                   b200a_stream stream) {
+  return vad_walk_impl(desc, chunk, frame0, frames, spectrum, cepstrum_window, rows, workspace, workspace_bytes,
+                       static_cast<cudaStream_t>(stream));
+}
+
+int b200a_vad_trigger(const b200a_vad_desc* desc, int64_t chunk, int64_t frame0, int64_t frames, const float* power,
+                      float* measures, void* workspace, size_t workspace_bytes, b200a_stream stream) {
+  return vad_trigger_impl(desc, chunk, frame0, frames, power, measures, workspace, workspace_bytes,
+                          static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -184,6 +184,12 @@ int convolve_run_impl(const b200a_convolve_desc* d, const float* x, const float*
                       size_t ws_bytes, cudaStream_t stream);
 int convolve_backward_impl(const b200a_convolve_desc* d, const float* x, const float* y, const float* grad,
                            float* grad_x, float* grad_y, void* ws, size_t ws_bytes, cudaStream_t stream);
+// vad.cu
+size_t vad_workspace_bytes_impl(const b200a_vad_desc* d, int64_t chunk);
+int vad_walk_impl(const b200a_vad_desc* d, int64_t chunk, int64_t frame0, int64_t frames, const float* spectrum,
+                  const float* cepstrum_window, float* rows, void* ws, size_t ws_bytes, cudaStream_t stream);
+int vad_trigger_impl(const b200a_vad_desc* d, int64_t chunk, int64_t frame0, int64_t frames, const float* power,
+                     float* measures, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

@@ -21,7 +21,8 @@ forward-only.
 IIR filtering (reference functional/filtering.py): ``lfilter`` (1032-1099), ``filtfilt`` (672-710), ``biquad`` and the
 ``allpass`` / ``band`` / ``bandpass`` / ``bandreject`` / ``bass`` / ``deemph`` / ``equalizer`` / ``highpass`` /
 ``lowpass`` / ``riaa`` / ``treble`` ``_biquad`` designs, and ``preemphasis`` / ``deemphasis`` (functional.py:2426-2473),
-all on one chunked-scan kernel family; filter orders up to 16.
+all on one chunked-scan kernel family; filter orders up to 16.  ``vad`` (filtering.py:1485-1702): SoX's voice-activity
+trim, measured on the GPU (the front end's FFT passes around a per-bin walk kernel), returning a view of its input.
 
 FFT convolution: ``fftconvolve`` (functional.py:2222-2258), uniformly partitioned overlap-save on the kernels of
 ``csrc/convolve.cu``.  Direct convolution: ``convolve`` (functional.py:2261-2314), a banded TF32 x 3 tensor-core
@@ -44,7 +45,7 @@ from ._bookkeeping import resample_ratio
 from ._constants import create_dct, linear_fbanks, melscale_fbanks, sinc_resample_kernel
 from ._filtering import (allpass_biquad, band_biquad, bandpass_biquad, bandreject_biquad, bass_biquad,  # noqa: F401
                          biquad, deemph_biquad, deemphasis, equalizer_biquad, filtfilt, highpass_biquad, lfilter,
-                         lowpass_biquad, preemphasis, riaa_biquad, treble_biquad)
+                         lowpass_biquad, preemphasis, riaa_biquad, treble_biquad, vad)
 from ._plans import (FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad,
                      is_feature_differentiable, is_filtering_differentiable, is_inverse_differentiable,
                      is_vocoder_differentiable, new_group_max, pack_rows, vocoder_chain)
@@ -82,6 +83,7 @@ __all__ = [
     "deemphasis",
     "fftconvolve",
     "convolve",
+    "vad",
 ]
 
 

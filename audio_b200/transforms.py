@@ -27,14 +27,14 @@ from typing import Callable, Optional, Union
 import torch
 from torch import Tensor
 
-from . import _lib, _ops
+from . import _filtering, _lib, _ops
 from . import functional as F
 from ._plans import (FrontendPlan, InverseMelPlan, ResamplePlan, _InverseMelFunction, _no_autograd, _require_cuda_f32,
                      _wants_grad, is_feature_differentiable, vocoder_chain)
 
 __all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "InverseMelScale", "MelSpectrogram", "MFCC", "LFCC",
            "SpectralCentroid", "Resample", "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift", "Preemphasis",
-           "Deemphasis", "FFTConvolve", "Convolve"]
+           "Deemphasis", "FFTConvolve", "Convolve", "Vad"]
 
 
 def _setup_framing(mod, n_fft, win_length, hop_length, window_fn=None, wkwargs=None, hop_div=2):
@@ -751,6 +751,52 @@ class Convolve(torch.nn.Module):
 
     def forward(self, x: Tensor, y: Tensor) -> Tensor:
         return F.convolve(x, y, mode=self.mode)
+
+
+class Vad(torch.nn.Module):
+    """Voice-activity trim from the front of the audio, as SoX's vad (reference _transforms.py:1478-1612):
+    ``F.vad(waveform, sample_rate, ...)`` with the module's parameters.  The host constants, windows and front-end
+    workspaces are built at the first ``forward`` and kept."""
+
+    def __init__(self, sample_rate: int, trigger_level: float = 7.0, trigger_time: float = 0.25,
+                 search_time: float = 1.0, allowed_gap: float = 0.25, pre_trigger_time: float = 0.0,
+                 boot_time: float = 0.35, noise_up_time: float = 0.1, noise_down_time: float = 0.01,
+                 noise_reduction_amount: float = 1.35, measure_freq: float = 20.0,
+                 measure_duration: Optional[float] = None, measure_smooth_time: float = 0.4,
+                 hp_filter_freq: float = 50.0, lp_filter_freq: float = 6000.0, hp_lifter_freq: float = 150.0,
+                 lp_lifter_freq: float = 2000.0) -> None:
+        super().__init__()
+        self.sample_rate = sample_rate
+        self.trigger_level = trigger_level
+        self.trigger_time = trigger_time
+        self.search_time = search_time
+        self.allowed_gap = allowed_gap
+        self.pre_trigger_time = pre_trigger_time
+        self.boot_time = boot_time
+        self.noise_up_time = noise_up_time
+        self.noise_down_time = noise_down_time
+        self.noise_reduction_amount = noise_reduction_amount
+        self.measure_freq = measure_freq
+        self.measure_duration = measure_duration
+        self.measure_smooth_time = measure_smooth_time
+        self.hp_filter_freq = hp_filter_freq
+        self.lp_filter_freq = lp_filter_freq
+        self.hp_lifter_freq = hp_lifter_freq
+        self.lp_lifter_freq = lp_lifter_freq
+        self._plan = None
+
+    def _params(self):
+        return (self.sample_rate, self.trigger_level, self.trigger_time, self.search_time, self.allowed_gap,
+                self.pre_trigger_time, self.boot_time, self.noise_up_time, self.noise_down_time,
+                self.noise_reduction_amount, self.measure_freq, self.measure_duration, self.measure_smooth_time,
+                self.hp_filter_freq, self.lp_filter_freq, self.hp_lifter_freq, self.lp_lifter_freq)
+
+    def forward(self, waveform: Tensor) -> Tensor:
+        _filtering._warn_batch(waveform)
+        params = self._params()
+        if self._plan is None or self._plan[0] != params:  # rebuilt only when an attribute was changed
+            self._plan = (params, _filtering.VadPlan(*params))
+        return _filtering._vad_trim(waveform, self._plan[1])
 
 
 # ---- B200A_REFERENCE=1: A/B switch to the reference implementation (debugging only, never silent) -----------------

@@ -623,6 +623,66 @@ int b200a_convolve_run(const b200a_convolve_desc* desc, const float* x, const fl
 int b200a_convolve_backward(const b200a_convolve_desc* desc, const float* x, const float* y, const float* grad,
                             float* grad_x, float* grad_y, void* workspace, size_t workspace_bytes, b200a_stream stream);
 
+/* ---- voice-activity trim: vad (functional/filtering.py:1414-1702) ---------------------------------------------- */
+/*
+ * The measurement loop of SoX's vad, run over `frames` consecutive measurement frames (a chunk) of `channels` channels
+ * at a time.  Per frame f (global index g = frame0 + f) and channel c:
+ *   1. |X| = b200a_frontend_run(B200A_STAGE_POWER, power 1) of the frame (the caller's pass: n_fft = dft_len,
+ *      win_length = measure_len_ws, hop = period, center 0)
+ *   2. b200a_vad_walk, per bin k of [spectrum_start, spectrum_end), in float32 with one rounding per operation:
+ *        mult = b / (1 + b) while booting (b = g while g <= boot_count_max, or always when that is negative), else
+ *        measure_smooth_mult;  S = S mult + |X| (1 - mult);  d = S^2;  nm = 0 while booting, else (d > N ? up : down);
+ *        N = N nm + d (1 - nm);  r = sqrt(max(0, d - noise_reduction_amount N));  row[k] = r * cepstrum_window[k - s0]
+ *   3. P = b200a_frontend_run(B200A_STAGE_MEL) of the rows (the caller's pass: n_fft = win_length = hop = dft_len / 2,
+ *      window of ones, power 2, one filter of ones on [cepstrum_start, cepstrum_end))
+ *   4. b200a_vad_trigger: meas = max(0, 21 + log(P / (cepstrum_end - cepstrum_start))) in double (0 for P <= 0), stored
+ *      as float32;  mean = mean * trigger_mult + meas * (1 - trigger_mult) in float32;  the first (frame, channel) in
+ *      frame-major order with mean >= trigger_level triggers, and the reference's flush scan over the last
+ *      measures_len measures runs for that channel and every later one at that frame.
+ * Chunks must be run in order on one workspace: frame0 == 0 starts from zero state, a later chunk continues the state
+ * the previous one left exactly.  (The front end packs two frames into one complex FFT within a launch, so |X| and P
+ * next to a chunk edge can differ in the last bits from a run with other chunk boundaries.)
+ */
+typedef struct b200a_vad_desc {
+  int32_t channels;                      /* >= 1 */
+  int32_t dft_len;                       /* power of two, 16..8192 (B200A_EUNSUPPORTED above) */
+  int32_t spectrum_start, spectrum_end;  /* 1 <= start <= end <= dft_len / 2 */
+  int32_t cepstrum_start, cepstrum_end;  /* 0 <= start < end <= dft_len / 4 */
+  int32_t measures_len;                  /* ring length ceil(search_time * measure_freq) >= 1 */
+  int32_t gap_len;                       /* int(allowed_gap * measure_freq + 0.5) */
+  int32_t boot_count_max;                /* int(boot_time * measure_freq - 0.5) */
+  int32_t period;                        /* measure_period_ns >= 1 */
+  int64_t fixed_pre_trigger;             /* fixed_pre_trigger_len_ns */
+  double noise_up_mult, noise_down_mult; /* rounded to float32 where used, as the reference's float32 tensors */
+  double noise_reduction_amount;
+  double measure_smooth_mult, trigger_mult;
+  double trigger_level;                  /* compared in float32 */
+} b200a_vad_desc;
+
+/* Workspace bytes for `chunk` frames per call: the 16-byte status, the carried spectra, means and measure ring, and
+ * per-chunk scratch; 0 for an invalid or unsupported descriptor. */
+size_t b200a_vad_workspace_bytes(const b200a_vad_desc* desc, int64_t chunk);
+/*
+ *   spectrum        : [channels][frames][dft_len / 2 + 1] |X| of the chunk's frames
+ *   cepstrum_window : [spectrum_end - spectrum_start]
+ *   rows            : [channels][chunk][dft_len / 2]; bins [spectrum_start, spectrum_end) of the first `frames` rows
+ *                     of each channel are written, the rest is left as it is (the caller zeroes it once)
+ */
+int b200a_vad_walk(const b200a_vad_desc* desc, int64_t chunk, int64_t frame0, int64_t frames, const float* spectrum,
+                   const float* cepstrum_window, float* rows, void* workspace, size_t workspace_bytes,
+                   b200a_stream stream);
+/*
+ *   power    : [channels][frames] cepstral band powers P
+ *   measures : [channels][frames] the measures, float32
+ * Writes the workspace's first 16 bytes: int64 {g, start} with g the triggering frame and start the first sample the
+ * trim keeps, or {-1, 0} when no frame of the chunk triggered.  One CTA; no atomics.
+ * Both calls: B200A_EINVAL for a null pointer or descriptor, a field outside its range, frame0 < 0 or frames outside
+ * [0, chunk]; B200A_EUNSUPPORTED for dft_len > 8192, more than 65535 channels or chunk > 2^20; B200A_EWORKSPACE when
+ * workspace_bytes is too small.  frames == 0 enqueues nothing.
+ */
+int b200a_vad_trigger(const b200a_vad_desc* desc, int64_t chunk, int64_t frame0, int64_t frames, const float* power,
+                      float* measures, void* workspace, size_t workspace_bytes, b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);

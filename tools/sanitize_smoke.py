@@ -98,5 +98,9 @@ with audio_b200.differentiable(filtering=True):
     xg = x.clone().requires_grad_()
     F.convolve(torch.randn(1, 1, 200, device="cuda", requires_grad=True), xg[:, None, :3000]).sum().backward()
 F.convolve(x, torch.randn(3, 1025, device="cuda"), "same")
+# vad: a trim over several chunks with carried state, and an input shorter than one measurement frame
+from audio_b200 import _filtering  # noqa: E402
+_filtering.VadPlan(16000, trigger_level=1e9).run(x, chunk=7)
+F.vad(x[:1, :1000], 16000)
 torch.cuda.synchronize()
 print("done")
