@@ -426,7 +426,7 @@ class VadPlan:
         measure, ws_measure, cepstrum, ws_cepstrum, cep_window = self.device_state(x.device)
         m_i, m_f = measure._packed_desc()
         c_i, c_f = cepstrum._packed_desc()
-        desc_i, desc_f = _ops.pack_vad_desc(self.desc(channels))
+        desc_i, desc_f = _ops.pack(self.desc(channels))
         dft, period, half = self.dft_len_ws, self.measure_period_ns, self.dft_len_ws // 2
         chunk = min(int(chunk), frames)
         lib = _lib.lib()

@@ -1,9 +1,6 @@
 """``torch.library`` registration of the hot-path ops, so the dispatcher, ``torch.profiler`` and CUDA-graph
-capture tooling see them as ``b200audio::frontend_run`` / ``frontend_backward`` / ``istft_backward`` / ``mfcc_finish`` /
-``mfcc_backward`` / ``amplitude_to_db_backward`` / ``apply_fbank_backward`` / ``ratio_backward`` / ``resample_run`` /
-``resample_backward`` / ``kaldi_run`` / ``kaldi_backward`` / ``phase_vocoder_backward`` / ``rnnt_features`` /
-``rnnt_features_backward`` / ``inverse_mel`` / ``inverse_mel_backward`` / ``lfilter`` / ``lfilter_backward`` /
-``fftconvolve`` / ``fftconvolve_backward`` / ``convolve`` / ``convolve_backward`` / ``vad_walk`` / ``vad_trigger``.
+capture tooling see them as ``b200audio::<name>``.  Each op is defined by one ``_op`` call next to its two
+implementations.
 
 Same shape as the reference's native ops -- ``STABLE_TORCH_LIBRARY_FRAGMENT(torchaudio, m){ m.def(...) }`` with a
 per-backend ``..._IMPL(torchaudio, CUDA, m)`` (pytorch/audio/src/libtorchaudio/lfilter.cpp:118-138) bound on the
@@ -12,122 +9,62 @@ schema is defined from Python (the library itself has no torch headers), the CUD
 C ABI of libb200audio.so on the current stream, and a Meta implementation gives shapes for fake tensors.  There is
 deliberately NO CPU implementation: a CPU tensor fails in the dispatcher ("no kernel for CPU"), never falls back.
 
-The descriptor travels as a list of ints + a list of floats (``b200a_frontend_desc`` is plain old data).
+A descriptor structure (``b200a_frontend_desc``, ``b200a_kaldi_desc``, ``b200a_vad_desc``: plain old data) travels as
+an ``int[]`` and a ``float[]`` list: ``pack`` and ``unpack`` derive both from the structure's ``_fields_``.
 """
 from __future__ import annotations
 
 import ctypes
-
-from typing import List, Optional
+import functools
 
 import torch
 
 from . import _lib
 
-_DESC_INTS = ("n_fft", "win_length", "hop", "pad", "center", "pad_mode", "onesided", "frame_length_norm", "window_norm",
-              "n_mels", "n_mfcc", "log_mels")
-_DESC_FLOATS = ("power", "db_multiplier", "db_amin", "db_offset")
-DESC_N_MELS = _DESC_INTS.index("n_mels")
+
+@functools.cache
+def _layout(cls):
+    """(int field names, float field names, position in ints + floats of each field in struct order) of a descriptor
+    structure.  Integer fields go to the int[] list and floating-point fields to the float[] list, in struct order."""
+    ints = tuple(name for name, ctype in cls._fields_ if ctype in (ctypes.c_int32, ctypes.c_int64))
+    floats = tuple(name for name, ctype in cls._fields_ if ctype in (ctypes.c_float, ctypes.c_double))
+    names = ints + floats
+    if len(names) != len(cls._fields_):
+        raise TypeError(f"{cls.__name__} has fields that are neither integers nor floats; it cannot be packed")
+    return ints, floats, tuple(names.index(name) for name, _ in cls._fields_)
+
+
+def pack(d: ctypes.Structure):
+    """The (ints, floats) lists of a descriptor structure, as the ops' ``int[]`` / ``float[]`` arguments take it."""
+    ints, floats, _ = _layout(type(d))
+    return [getattr(d, name) for name in ints], [getattr(d, name) for name in floats]
+
+
+def unpack(cls, ints, floats):
+    """The ``cls`` descriptor that ``pack`` turned into ``ints`` and ``floats``."""
+    int_names, float_names, order = _layout(cls)
+    if len(ints) != len(int_names) or len(floats) != len(float_names):
+        raise ValueError(f"audio_b200: a packed {cls.__name__} has {len(int_names)} ints and {len(float_names)} floats, "
+                         f"got {len(ints)} and {len(floats)}")
+    values = [*ints, *floats]
+    return cls(*[values[i] for i in order])  # positional construction: the fastest way to fill every field
+
+
+def field_index(cls, name: str) -> int:
+    """Where field ``name`` of ``cls`` sits in the list ``pack`` puts it in."""
+    ints, floats, _ = _layout(cls)
+    return ints.index(name) if name in ints else floats.index(name)
+
 
 _LIB = torch.library.Library("b200audio", "DEF")
-_LIB.define(
-    "frontend_run(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int stage, int frames, int width, "
-    "int row_stride, Tensor(a!)? group_max, int rows_per_group) -> Tensor"
-)
-_LIB.define(
-    "frontend_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int stage, int row_stride, "
-    "Tensor grad_out) -> Tensor"
-)
-_LIB.define(
-    "istft_backward(Tensor grad, Tensor workspace, int[] desc_i, float[] desc_f, int start, int frames) -> Tensor"
-)
-_LIB.define(
-    "mfcc_finish(Tensor feat, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? group_max, int rows_per_group, "
-    "float top_db) -> Tensor"
-)
-_LIB.define(
-    "mfcc_backward(Tensor grad, Tensor feat, Tensor mel, Tensor? group_max, Tensor workspace, int[] desc_i, "
-    "float[] desc_f, int rows_per_group, float top_db) -> Tensor"
-)
-_LIB.define(
-    "amplitude_to_db_backward(Tensor grad, Tensor x, Tensor? group_max, int groups, float multiplier, float amin, "
-    "float offset, float top_db) -> Tensor"
-)
-_LIB.define("apply_fbank_backward(Tensor grad, Tensor fb) -> Tensor")
-_LIB.define("ratio_backward(Tensor grad, Tensor pairs) -> Tensor")
-_LIB.define(
-    "resample_run(Tensor wave, Tensor workspace, Tensor kernel, int orig_r, int new_r, int width, int row_stride, "
-    "int out_len, int pitch) -> Tensor"
-)
-_LIB.define("resample_backward(Tensor grad, Tensor workspace, int orig_r, int new_r, int width, int length) -> Tensor")
-_LIB.define(
-    "kaldi_run(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int[] kaldi_i, float[] kaldi_f, int stage, "
-    "int frames, int width, int row_stride) -> Tensor"
-)
-_LIB.define(
-    "kaldi_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int[] kaldi_i, float[] kaldi_f, "
-    "int stage, int row_stride, Tensor grad_out) -> Tensor"
-)
-_LIB.define(
-    "phase_vocoder_backward(Tensor spec, Tensor out, Tensor grad, float rate) -> Tensor"
-)
-_LIB.define(
-    "rnnt_features(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? lengths, Tensor stats, float gain, "
-    "int out_frames, int pad_frames, int row_stride, bool with_mel) -> (Tensor, Tensor)"
-)
-_LIB.define("rnnt_features_backward(Tensor stats, float gain, Tensor mel, Tensor grad) -> Tensor")
-_LIB.define("inverse_mel(Tensor mel, Tensor plan, int n_stft) -> Tensor")
-_LIB.define("inverse_mel_backward(Tensor grad, Tensor mel, Tensor plan, int n_stft) -> Tensor")
-_LIB.define("lfilter(Tensor x, Tensor a, Tensor b, bool clamp, bool reverse, bool with_raw) -> (Tensor, Tensor)")
-_LIB.define(
-    "lfilter_backward(Tensor grad, Tensor x, Tensor y_raw, Tensor a, Tensor b, bool clamp, bool reverse) "
-    "-> (Tensor, Tensor, Tensor)"
-)
-_LIB.define("fftconvolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor")
-_LIB.define(
-    "fftconvolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)"
-)
-_LIB.define("convolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor")
-_LIB.define(
-    "convolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)"
-)
-_LIB.define(
-    "vad_walk(Tensor spectrum, Tensor cepstrum_window, Tensor(a!) rows, Tensor(b!) workspace, int[] desc_i, "
-    "float[] desc_f, int chunk, int frame0) -> ()"
-)
-_LIB.define(
-    "vad_trigger(Tensor power, Tensor(a!) workspace, int[] desc_i, float[] desc_f, int chunk, int frame0) -> Tensor"
-)
-
-_KALDI_INTS = ("window_size", "window_shift", "padded_size", "snip_edges", "remove_dc_offset", "energy_mode", "energy_col",
-               "out_width", "out_col0", "use_log")
-_KALDI_FLOATS = ("preemphasis", "energy_floor")
 
 
-def pack_desc(d: "_lib.FrontendDesc"):
-    return [int(getattr(d, k)) for k in _DESC_INTS], [float(getattr(d, k)) for k in _DESC_FLOATS]
-
-
-def _unpack_desc(desc_i: List[int], desc_f: List[float]) -> "_lib.FrontendDesc":
-    d = _lib.FrontendDesc()
-    for k, v in zip(_DESC_INTS, desc_i):
-        setattr(d, k, int(v))
-    for k, v in zip(_DESC_FLOATS, desc_f):
-        setattr(d, k, float(v))
-    return d
-
-
-def pack_kaldi_desc(k: "_lib.KaldiDesc"):
-    return [int(getattr(k, f)) for f in _KALDI_INTS], [float(getattr(k, f)) for f in _KALDI_FLOATS]
-
-
-def _unpack_kaldi_desc(kaldi_i: List[int], kaldi_f: List[float]) -> "_lib.KaldiDesc":
-    k = _lib.KaldiDesc()
-    for f, v in zip(_KALDI_INTS, kaldi_i):
-        setattr(k, f, int(v))
-    for f, v in zip(_KALDI_FLOATS, kaldi_f):
-        setattr(k, f, float(v))
-    return k
+def _op(schema: str, cuda, meta):
+    """Define ``b200audio::<name>`` from ``schema`` with its CUDA and Meta implementations; returns the op."""
+    name = _LIB.define(schema)
+    _LIB.impl(name, cuda, "CUDA")
+    _LIB.impl(name, meta, "Meta")
+    return getattr(torch.ops.b200audio, name)
 
 
 def _stream(dev: torch.device) -> int:
@@ -141,7 +78,7 @@ def _out_shape(wave, stage, frames, width):
 
 # ---- frontend_run ------------------------------------------------------------------------------------------------
 def _frontend_run_cuda(wave, workspace, desc_i, desc_f, stage, frames, width, row_stride, group_max, rows_per_group):
-    d = _unpack_desc(desc_i, desc_f)
+    d = unpack(_lib.FrontendDesc, desc_i, desc_f)
     dev = wave.device
     with torch.cuda.device(dev):
         out = torch.empty(_out_shape(wave, stage, frames, width), dtype=torch.float32, device=dev)
@@ -160,6 +97,11 @@ def _frontend_run_meta(wave, workspace, desc_i, desc_f, stage, frames, width, ro
     return wave.new_empty(_out_shape(wave, stage, frames, width), dtype=torch.float32)
 
 
+frontend_run = _op(
+    "frontend_run(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int stage, int frames, int width, "
+    "int row_stride, Tensor(a!)? group_max, int rows_per_group) -> Tensor", _frontend_run_cuda, _frontend_run_meta)
+
+
 # ---- frontend_backward -------------------------------------------------------------------------------------------
 def _complex_strides(grad_out):
     """Element strides of a (rows, T, bins, 2) float gradient in complex elements, copying it when the pairs are not
@@ -172,7 +114,7 @@ def _complex_strides(grad_out):
 
 
 def _frontend_backward_cuda(wave, workspace, desc_i, desc_f, stage, row_stride, grad_out):
-    d = _unpack_desc(desc_i, desc_f)
+    d = unpack(_lib.FrontendDesc, desc_i, desc_f)
     rows, length = wave.shape
     dev = wave.device
     if stage == _lib.STAGE_COMPLEX:
@@ -195,10 +137,15 @@ def _frontend_backward_meta(wave, workspace, desc_i, desc_f, stage, row_stride, 
     return wave.new_empty(wave.shape, dtype=torch.float32)
 
 
+frontend_backward = _op(
+    "frontend_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int stage, int row_stride, "
+    "Tensor grad_out) -> Tensor", _frontend_backward_cuda, _frontend_backward_meta)
+
+
 # ---- istft_backward ----------------------------------------------------------------------------------------------
 def _istft_backward_cuda(grad, workspace, desc_i, desc_f, start, frames):
     """(rows, L) upstream gradient -> (rows, frames, n_fft//2+1, 2) frame-major spectrogram gradient."""
-    d = _unpack_desc(desc_i, desc_f)
+    d = unpack(_lib.FrontendDesc, desc_i, desc_f)
     if grad.shape[0] > 0 and grad.shape[1] > 0 and grad.stride(1) != 1:
         grad = grad.contiguous()
     rows, g_len = grad.shape
@@ -216,12 +163,18 @@ def _istft_backward_cuda(grad, workspace, desc_i, desc_f, start, frames):
 
 
 def _istft_backward_meta(grad, workspace, desc_i, desc_f, start, frames):
-    return grad.new_empty((grad.shape[0], frames, int(desc_i[_DESC_INTS.index("n_fft")]) // 2 + 1, 2))
+    n_fft = int(desc_i[field_index(_lib.FrontendDesc, "n_fft")])
+    return grad.new_empty((grad.shape[0], frames, n_fft // 2 + 1, 2))
+
+
+istft_backward = _op(
+    "istft_backward(Tensor grad, Tensor workspace, int[] desc_i, float[] desc_f, int start, int frames) -> Tensor",
+    _istft_backward_cuda, _istft_backward_meta)
 
 
 # ---- mfcc_finish -------------------------------------------------------------------------------------------------
 def _mfcc_finish_cuda(feat, workspace, desc_i, desc_f, group_max, rows_per_group, top_db):
-    d = _unpack_desc(desc_i, desc_f)
+    d = unpack(_lib.FrontendDesc, desc_i, desc_f)
     rows, frames, _ = feat.shape
     dev = feat.device
     with torch.cuda.device(dev):
@@ -234,13 +187,18 @@ def _mfcc_finish_cuda(feat, workspace, desc_i, desc_f, group_max, rows_per_group
 
 
 def _mfcc_finish_meta(feat, workspace, desc_i, desc_f, group_max, rows_per_group, top_db):
-    return feat.new_empty((feat.shape[0], feat.shape[1], int(desc_i[_DESC_INTS.index("n_mfcc")])))
+    return feat.new_empty((feat.shape[0], feat.shape[1], int(desc_i[field_index(_lib.FrontendDesc, "n_mfcc")])))
+
+
+mfcc_finish = _op(
+    "mfcc_finish(Tensor feat, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? group_max, int rows_per_group, "
+    "float top_db) -> Tensor", _mfcc_finish_cuda, _mfcc_finish_meta)
 
 
 # ---- mfcc_backward -----------------------------------------------------------------------------------------------
 def _mfcc_backward_cuda(grad, feat, mel, group_max, workspace, desc_i, desc_f, rows_per_group, top_db):
     """(rows, T, n_mfcc) cepstral gradient at any element strides -> (rows, T, n_mels) mel-stage gradient."""
-    d = _unpack_desc(desc_i, desc_f)
+    d = unpack(_lib.FrontendDesc, desc_i, desc_f)
     rows, frames, n_mels = mel.shape
     dev = mel.device
     gs = grad.stride()
@@ -260,6 +218,11 @@ def _mfcc_backward_cuda(grad, feat, mel, group_max, workspace, desc_i, desc_f, r
 
 def _mfcc_backward_meta(grad, feat, mel, group_max, workspace, desc_i, desc_f, rows_per_group, top_db):
     return mel.new_empty(mel.shape)
+
+
+mfcc_backward = _op(
+    "mfcc_backward(Tensor grad, Tensor feat, Tensor mel, Tensor? group_max, Tensor workspace, int[] desc_i, "
+    "float[] desc_f, int rows_per_group, float top_db) -> Tensor", _mfcc_backward_cuda, _mfcc_backward_meta)
 
 
 # ---- amplitude_to_db_backward ------------------------------------------------------------------------------------
@@ -289,6 +252,11 @@ def _amplitude_to_db_backward_meta(grad, x, group_max, groups, multiplier, amin,
     return x.new_empty(x.shape)
 
 
+amplitude_to_db_backward = _op(
+    "amplitude_to_db_backward(Tensor grad, Tensor x, Tensor? group_max, int groups, float multiplier, float amin, "
+    "float offset, float top_db) -> Tensor", _amplitude_to_db_backward_cuda, _amplitude_to_db_backward_meta)
+
+
 # ---- apply_fbank_backward ----------------------------------------------------------------------------------------
 def _apply_fbank_backward_cuda(grad, fb):
     """(rows, T, n_filters) MelScale output gradient at any element strides -> (rows, T, n_bins) frame-major."""
@@ -308,6 +276,10 @@ def _apply_fbank_backward_meta(grad, fb):
     return grad.new_empty((grad.shape[0], grad.shape[1], fb.shape[0]))
 
 
+apply_fbank_backward = _op("apply_fbank_backward(Tensor grad, Tensor fb) -> Tensor", _apply_fbank_backward_cuda,
+                           _apply_fbank_backward_meta)
+
+
 # ---- ratio_backward ----------------------------------------------------------------------------------------------
 def _ratio_backward_cuda(grad, pairs):
     """(rows, T) SpectralCentroid gradient at any element strides -> (rows, T, 2) gradient of the (N, D) pairs."""
@@ -325,6 +297,9 @@ def _ratio_backward_meta(grad, pairs):
     return pairs.new_empty(pairs.shape)
 
 
+ratio_backward = _op("ratio_backward(Tensor grad, Tensor pairs) -> Tensor", _ratio_backward_cuda, _ratio_backward_meta)
+
+
 # ---- resample_run ------------------------------------------------------------------------------------------------
 def _resample_run_cuda(wave, workspace, kernel, orig_r, new_r, width, row_stride, out_len, pitch):
     rows, length = wave.shape
@@ -340,6 +315,11 @@ def _resample_run_cuda(wave, workspace, kernel, orig_r, new_r, width, row_stride
 
 def _resample_run_meta(wave, workspace, kernel, orig_r, new_r, width, row_stride, out_len, pitch):
     return wave.new_empty((wave.shape[0], pitch))
+
+
+resample_run = _op(
+    "resample_run(Tensor wave, Tensor workspace, Tensor kernel, int orig_r, int new_r, int width, int row_stride, "
+    "int out_len, int pitch) -> Tensor", _resample_run_cuda, _resample_run_meta)
 
 
 # ---- resample_backward -------------------------------------------------------------------------------------------
@@ -362,10 +342,15 @@ def _resample_backward_meta(grad, workspace, orig_r, new_r, width, length):
     return grad.new_empty((grad.shape[0], length))
 
 
+resample_backward = _op(
+    "resample_backward(Tensor grad, Tensor workspace, int orig_r, int new_r, int width, int length) -> Tensor",
+    _resample_backward_cuda, _resample_backward_meta)
+
+
 # ---- kaldi_run / kaldi_backward ---------------------------------------------------------------------------------
 def _kaldi_run_cuda(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, frames, width, row_stride):
     """(rows, L) waveform -> (rows, frames, width) Kaldi feature rows (b200a_kaldi_run)."""
-    d, k = _unpack_desc(desc_i, desc_f), _unpack_kaldi_desc(kaldi_i, kaldi_f)
+    d, k = unpack(_lib.FrontendDesc, desc_i, desc_f), unpack(_lib.KaldiDesc, kaldi_i, kaldi_f)
     rows, length = wave.shape
     dev = wave.device
     with torch.cuda.device(dev):
@@ -380,9 +365,14 @@ def _kaldi_run_meta(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, fr
     return wave.new_empty((wave.shape[0], frames, width), dtype=torch.float32)
 
 
+kaldi_run = _op(
+    "kaldi_run(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int[] kaldi_i, float[] kaldi_f, int stage, "
+    "int frames, int width, int row_stride) -> Tensor", _kaldi_run_cuda, _kaldi_run_meta)
+
+
 def _kaldi_backward_cuda(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, row_stride, grad_out):
     """(rows, frames, width) feature-row gradient at any element strides -> (rows, L) waveform gradient."""
-    d, k = _unpack_desc(desc_i, desc_f), _unpack_kaldi_desc(kaldi_i, kaldi_f)
+    d, k = unpack(_lib.FrontendDesc, desc_i, desc_f), unpack(_lib.KaldiDesc, kaldi_i, kaldi_f)
     rows, length = wave.shape
     dev = wave.device
     gs = grad_out.stride()
@@ -400,6 +390,11 @@ def _kaldi_backward_cuda(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stag
 
 def _kaldi_backward_meta(wave, workspace, desc_i, desc_f, kaldi_i, kaldi_f, stage, row_stride, grad_out):
     return wave.new_empty(wave.shape, dtype=torch.float32)
+
+
+kaldi_backward = _op(
+    "kaldi_backward(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, int[] kaldi_i, float[] kaldi_f, "
+    "int stage, int row_stride, Tensor grad_out) -> Tensor", _kaldi_backward_cuda, _kaldi_backward_meta)
 
 
 # ---- phase_vocoder_backward --------------------------------------------------------------------------------------
@@ -425,16 +420,20 @@ def _phase_vocoder_backward_meta(spec, out, grad, rate):
     return spec.new_empty((spec.shape[0], spec.shape[2], spec.shape[1], 2), dtype=torch.float32)
 
 
+phase_vocoder_backward = _op("phase_vocoder_backward(Tensor spec, Tensor out, Tensor grad, float rate) -> Tensor",
+                             _phase_vocoder_backward_cuda, _phase_vocoder_backward_meta)
+
+
 # ---- rnnt_features / rnnt_features_backward ----------------------------------------------------------------------
 def _rnnt_shapes(wave, desc_i, out_frames, pad_frames):
-    n_mels = int(desc_i[DESC_N_MELS])
+    n_mels = int(desc_i[field_index(_lib.FrontendDesc, "n_mels")])
     return (wave.shape[0], out_frames + pad_frames, n_mels), (wave.shape[0], out_frames, n_mels)
 
 
 def _rnnt_features_cuda(wave, workspace, desc_i, desc_f, lengths, stats, gain, out_frames, pad_frames, row_stride, with_mel):
     """(rows, L) waveform -> ((rows, out_frames + pad_frames, n_mels) features, (rows, out_frames, n_mels) mel values
     or an empty tensor).  ``pad_frames`` zero rows after the features (one row only) are written by b200a_fill_f32."""
-    d = _unpack_desc(desc_i, desc_f)
+    d = unpack(_lib.FrontendDesc, desc_i, desc_f)
     rows, length = wave.shape
     if pad_frames > 0 and rows != 1:
         raise RuntimeError("audio_b200: rnnt_features pads a single row only")
@@ -465,6 +464,12 @@ def _rnnt_features_meta(wave, workspace, desc_i, desc_f, lengths, stats, gain, o
                                                                            dtype=torch.float32)
 
 
+rnnt_features = _op(
+    "rnnt_features(Tensor wave, Tensor workspace, int[] desc_i, float[] desc_f, Tensor? lengths, Tensor stats, float gain, "
+    "int out_frames, int pad_frames, int row_stride, bool with_mel) -> (Tensor, Tensor)",
+    _rnnt_features_cuda, _rnnt_features_meta)
+
+
 def _rnnt_features_backward_cuda(stats, gain, mel, grad):
     """(rows, T, n_mels) feature gradient at any element strides (0 included) -> (rows, T, n_mels) mel gradient."""
     rows, frames, n_mels = mel.shape
@@ -480,6 +485,10 @@ def _rnnt_features_backward_cuda(stats, gain, mel, grad):
 
 def _rnnt_features_backward_meta(stats, gain, mel, grad):
     return mel.new_empty(mel.shape)
+
+
+rnnt_features_backward = _op("rnnt_features_backward(Tensor stats, float gain, Tensor mel, Tensor grad) -> Tensor",
+                             _rnnt_features_backward_cuda, _rnnt_features_backward_meta)
 
 
 # ---- inverse_mel / inverse_mel_backward ----------------------------------------------------------------------------
@@ -500,6 +509,9 @@ def _inverse_mel_meta(mel, plan, n_stft):
     return mel.new_empty((mel.shape[0], mel.shape[2], n_stft))
 
 
+inverse_mel = _op("inverse_mel(Tensor mel, Tensor plan, int n_stft) -> Tensor", _inverse_mel_cuda, _inverse_mel_meta)
+
+
 def _inverse_mel_backward_cuda(grad, mel, plan, n_stft):
     """(rows, T, n_stft) output gradient at any element strides (0 included) -> (rows, T, n_mels) frame-major."""
     rows, n_mels, frames = mel.shape
@@ -516,6 +528,10 @@ def _inverse_mel_backward_cuda(grad, mel, plan, n_stft):
 
 def _inverse_mel_backward_meta(grad, mel, plan, n_stft):
     return mel.new_empty((mel.shape[0], mel.shape[2], mel.shape[1]))
+
+
+inverse_mel_backward = _op("inverse_mel_backward(Tensor grad, Tensor mel, Tensor plan, int n_stft) -> Tensor",
+                           _inverse_mel_backward_cuda, _inverse_mel_backward_meta)
 
 
 # ---- lfilter / lfilter_backward ---------------------------------------------------------------------------------
@@ -548,6 +564,10 @@ def _lfilter_meta(x, a, b, clamp, reverse, with_raw):
     return x.new_empty(x.shape), x.new_empty(x.shape if with_raw else (0,))
 
 
+lfilter = _op("lfilter(Tensor x, Tensor a, Tensor b, bool clamp, bool reverse, bool with_raw) -> (Tensor, Tensor)",
+              _lfilter_cuda, _lfilter_meta)
+
+
 def _lfilter_backward_cuda(grad, x, y_raw, a, b, clamp, reverse):
     """Upstream gradient of the (batch, n_filters, T) output -> (grad_x (batch, n_filters, T), grad_a, grad_b)."""
     batch, n_filters, length = x.shape
@@ -571,6 +591,11 @@ def _lfilter_backward_cuda(grad, x, y_raw, a, b, clamp, reverse):
 
 def _lfilter_backward_meta(grad, x, y_raw, a, b, clamp, reverse):
     return x.new_empty(x.shape), a.new_empty(a.shape), b.new_empty(b.shape)
+
+
+lfilter_backward = _op(
+    "lfilter_backward(Tensor grad, Tensor x, Tensor y_raw, Tensor a, Tensor b, bool clamp, bool reverse) "
+    "-> (Tensor, Tensor, Tensor)", _lfilter_backward_cuda, _lfilter_backward_meta)
 
 
 # ---- fftconvolve / fftconvolve_backward -------------------------------------------------------------------------
@@ -626,6 +651,10 @@ def _fftconvolve_meta(x, y, x_index, y_index, start, out_len):
     return x.new_empty((x_index.shape[0], out_len))
 
 
+fftconvolve = _op("fftconvolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor",
+                  _fftconvolve_cuda, _fftconvolve_meta)
+
+
 def _fftconvolve_backward_cuda(grad, x, y, x_index, y_index, start):
     return _conv_backward("fftconvolve", grad, x, y, x_index, y_index, start)
 
@@ -633,6 +662,11 @@ def _fftconvolve_backward_cuda(grad, x, y, x_index, y_index, start):
 def _fftconvolve_backward_meta(grad, x, y, x_index, y_index, start):
     rows = x_index.shape[0]
     return x.new_empty((rows, x.shape[1])), y.new_empty((rows, y.shape[1]))
+
+
+fftconvolve_backward = _op(
+    "fftconvolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)",
+    _fftconvolve_backward_cuda, _fftconvolve_backward_meta)
 
 
 # ---- convolve / convolve_backward: the direct method on the same descriptor -----------------------------------------
@@ -644,30 +678,18 @@ def _convolve_backward_cuda(grad, x, y, x_index, y_index, start):
     return _conv_backward("convolve", grad, x, y, x_index, y_index, start)
 
 
+convolve = _op("convolve(Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start, int out_len) -> Tensor",
+               _convolve_cuda, _fftconvolve_meta)
+convolve_backward = _op(
+    "convolve_backward(Tensor grad, Tensor x, Tensor y, Tensor x_index, Tensor y_index, int start) -> (Tensor, Tensor)",
+    _convolve_backward_cuda, _fftconvolve_backward_meta)
+
+
 # ---- vad_walk / vad_trigger ----------------------------------------------------------------------------------------
-_VAD_INTS = ("channels", "dft_len", "spectrum_start", "spectrum_end", "cepstrum_start", "cepstrum_end", "measures_len",
-             "gap_len", "boot_count_max", "period", "fixed_pre_trigger")
-_VAD_FLOATS = ("noise_up_mult", "noise_down_mult", "noise_reduction_amount", "measure_smooth_mult", "trigger_mult",
-               "trigger_level")
-
-
-def pack_vad_desc(d: "_lib.VadDesc"):
-    return [int(getattr(d, k)) for k in _VAD_INTS], [float(getattr(d, k)) for k in _VAD_FLOATS]
-
-
-def _unpack_vad_desc(desc_i: List[int], desc_f: List[float]) -> "_lib.VadDesc":
-    d = _lib.VadDesc()
-    for k, v in zip(_VAD_INTS, desc_i):
-        setattr(d, k, int(v))
-    for k, v in zip(_VAD_FLOATS, desc_f):
-        setattr(d, k, float(v))
-    return d
-
-
 def _vad_walk_cuda(spectrum, cepstrum_window, rows, workspace, desc_i, desc_f, chunk, frame0):
     """(C, frames, dft/2+1) |X| of a chunk -> bins [s0, s1) of the first `frames` rows of the (C, chunk, dft/2) cepstrum
     rows, carrying the smoothed spectrum and the noise estimate in ``workspace`` (b200a_vad_walk)."""
-    d = _unpack_vad_desc(desc_i, desc_f)
+    d = unpack(_lib.VadDesc, desc_i, desc_f)
     dev = spectrum.device
     with torch.cuda.device(dev):
         rc = _lib.lib().b200a_vad_walk(d, chunk, frame0, spectrum.shape[1], spectrum.data_ptr(), cepstrum_window.data_ptr(),
@@ -679,10 +701,15 @@ def _vad_walk_meta(spectrum, cepstrum_window, rows, workspace, desc_i, desc_f, c
     return None
 
 
+vad_walk = _op(
+    "vad_walk(Tensor spectrum, Tensor cepstrum_window, Tensor(a!) rows, Tensor(b!) workspace, int[] desc_i, "
+    "float[] desc_f, int chunk, int frame0) -> ()", _vad_walk_cuda, _vad_walk_meta)
+
+
 def _vad_trigger_cuda(power, workspace, desc_i, desc_f, chunk, frame0):
     """(C, frames) cepstral band powers of a chunk -> (C, frames) float32 measures; the trigger status goes to the first
     16 bytes of ``workspace`` (b200a_vad_trigger)."""
-    d = _unpack_vad_desc(desc_i, desc_f)
+    d = unpack(_lib.VadDesc, desc_i, desc_f)
     dev = power.device
     with torch.cuda.device(dev):
         measures = torch.empty(power.shape, dtype=torch.float32, device=dev)
@@ -696,56 +723,6 @@ def _vad_trigger_meta(power, workspace, desc_i, desc_f, chunk, frame0):
     return power.new_empty(power.shape)
 
 
-for _name, _cuda, _meta in (("frontend_run", _frontend_run_cuda, _frontend_run_meta),
-                            ("frontend_backward", _frontend_backward_cuda, _frontend_backward_meta),
-                            ("istft_backward", _istft_backward_cuda, _istft_backward_meta),
-                            ("mfcc_finish", _mfcc_finish_cuda, _mfcc_finish_meta),
-                            ("mfcc_backward", _mfcc_backward_cuda, _mfcc_backward_meta),
-                            ("amplitude_to_db_backward", _amplitude_to_db_backward_cuda, _amplitude_to_db_backward_meta),
-                            ("apply_fbank_backward", _apply_fbank_backward_cuda, _apply_fbank_backward_meta),
-                            ("ratio_backward", _ratio_backward_cuda, _ratio_backward_meta),
-                            ("resample_run", _resample_run_cuda, _resample_run_meta),
-                            ("resample_backward", _resample_backward_cuda, _resample_backward_meta),
-                            ("kaldi_run", _kaldi_run_cuda, _kaldi_run_meta),
-                            ("kaldi_backward", _kaldi_backward_cuda, _kaldi_backward_meta),
-                            ("phase_vocoder_backward", _phase_vocoder_backward_cuda, _phase_vocoder_backward_meta),
-                            ("rnnt_features", _rnnt_features_cuda, _rnnt_features_meta),
-                            ("rnnt_features_backward", _rnnt_features_backward_cuda, _rnnt_features_backward_meta),
-                            ("inverse_mel", _inverse_mel_cuda, _inverse_mel_meta),
-                            ("inverse_mel_backward", _inverse_mel_backward_cuda, _inverse_mel_backward_meta),
-                            ("lfilter", _lfilter_cuda, _lfilter_meta),
-                            ("lfilter_backward", _lfilter_backward_cuda, _lfilter_backward_meta),
-                            ("fftconvolve", _fftconvolve_cuda, _fftconvolve_meta),
-                            ("fftconvolve_backward", _fftconvolve_backward_cuda, _fftconvolve_backward_meta),
-                            ("convolve", _convolve_cuda, _fftconvolve_meta),
-                            ("convolve_backward", _convolve_backward_cuda, _fftconvolve_backward_meta),
-                            ("vad_walk", _vad_walk_cuda, _vad_walk_meta),
-                            ("vad_trigger", _vad_trigger_cuda, _vad_trigger_meta)):
-    _LIB.impl(_name, _cuda, "CUDA")
-    _LIB.impl(_name, _meta, "Meta")
-
-frontend_run = torch.ops.b200audio.frontend_run
-frontend_backward = torch.ops.b200audio.frontend_backward
-istft_backward = torch.ops.b200audio.istft_backward
-mfcc_finish = torch.ops.b200audio.mfcc_finish
-mfcc_backward = torch.ops.b200audio.mfcc_backward
-amplitude_to_db_backward = torch.ops.b200audio.amplitude_to_db_backward
-apply_fbank_backward = torch.ops.b200audio.apply_fbank_backward
-ratio_backward = torch.ops.b200audio.ratio_backward
-resample_run = torch.ops.b200audio.resample_run
-resample_backward = torch.ops.b200audio.resample_backward
-kaldi_run = torch.ops.b200audio.kaldi_run
-kaldi_backward = torch.ops.b200audio.kaldi_backward
-phase_vocoder_backward = torch.ops.b200audio.phase_vocoder_backward
-rnnt_features = torch.ops.b200audio.rnnt_features
-rnnt_features_backward = torch.ops.b200audio.rnnt_features_backward
-inverse_mel = torch.ops.b200audio.inverse_mel
-inverse_mel_backward = torch.ops.b200audio.inverse_mel_backward
-lfilter = torch.ops.b200audio.lfilter
-lfilter_backward = torch.ops.b200audio.lfilter_backward
-fftconvolve = torch.ops.b200audio.fftconvolve
-fftconvolve_backward = torch.ops.b200audio.fftconvolve_backward
-convolve = torch.ops.b200audio.convolve
-convolve_backward = torch.ops.b200audio.convolve_backward
-vad_walk = torch.ops.b200audio.vad_walk
-vad_trigger = torch.ops.b200audio.vad_trigger
+vad_trigger = _op(
+    "vad_trigger(Tensor power, Tensor(a!) workspace, int[] desc_i, float[] desc_f, int chunk, int frame0) -> Tensor",
+    _vad_trigger_cuda, _vad_trigger_meta)

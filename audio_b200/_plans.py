@@ -196,7 +196,7 @@ class _MfccFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, flat, ws, desc_i, desc_f, frames, stride, groups, rows_per_group, top_db):
-        n_mels = desc_i[_ops.DESC_N_MELS]
+        n_mels = desc_i[_ops.field_index(_lib.FrontendDesc, "n_mels")]
         gmax = new_group_max(groups, flat.device) if groups > 0 else None
         feat = _ops.frontend_run(flat, ws, desc_i, desc_f, _lib.STAGE_FEAT, frames, n_mels, stride, gmax, rows_per_group)
         out = _ops.mfcc_finish(feat, ws, desc_i, desc_f, gmax, rows_per_group, top_db)
@@ -210,8 +210,8 @@ class _MfccFunction(torch.autograd.Function):
     def backward(ctx, grad_out):
         (flat,) = ctx.saved_tensors
         desc_i, desc_f, frames, stride, rows_per_group, top_db = ctx.args
-        mel = _ops.frontend_run(flat, ctx.ws, desc_i, desc_f, _lib.STAGE_MEL, frames, desc_i[_ops.DESC_N_MELS], stride,
-                                None, 1)
+        n_mels = desc_i[_ops.field_index(_lib.FrontendDesc, "n_mels")]
+        mel = _ops.frontend_run(flat, ctx.ws, desc_i, desc_f, _lib.STAGE_MEL, frames, n_mels, stride, None, 1)
         g_mel = _ops.mfcc_backward(grad_out, ctx.feat, mel, ctx.gmax, ctx.ws, desc_i, desc_f, rows_per_group, top_db)
         grad = _ops.frontend_backward(flat, ctx.ws, desc_i, desc_f, _lib.STAGE_MEL, stride, g_mel)
         return grad, None, None, None, None, None, None, None, None
@@ -243,9 +243,26 @@ class _RNNTFunction(torch.autograd.Function):
         return grad, None, None, None, None, None, None, None, None, None, None
 
 
-def _version_of(t: torch.Tensor) -> int:
-    """In-place edit counter of a tensor; inference tensors (created under torch.inference_mode) keep none."""
-    return -1 if t.is_inference() else t._version
+class StampCache:
+    """A value built from constant tensors, rebuilt when any of them changes.  A tensor's stamp is its (data_ptr,
+    in-place edit counter, device); inference tensors (created under torch.inference_mode) keep no edit counter.  The
+    tensors behind the stamp are held, so their storage cannot be recycled and an equal stamp can only mean the same,
+    unmodified tensors."""
+
+    def __init__(self):
+        self.value = None
+        self._stamp = None
+        self._held = None
+
+    def get(self, tensors: tuple, build):
+        """The cached value while the stamp of ``tensors`` (``None`` entries allowed) is unchanged, else
+        ``build(*tensors)``."""
+        stamp = tuple(None if t is None else (t.data_ptr(), -1 if t.is_inference() else t._version, str(t.device))
+                      for t in tensors)
+        if stamp != self._stamp:
+            self.value = build(*tensors)
+            self._stamp, self._held = stamp, tensors
+        return self.value
 
 
 def _stream_ptr(device: torch.device) -> int:
@@ -267,11 +284,7 @@ class FrontendPlan:
 
     def __init__(self, desc: "_lib.FrontendDesc"):
         self.desc = desc
-        self._ws: Optional[torch.Tensor] = None
-        self._stamp = None
-        # the constant tensors the workspace was built from: holding them keeps their storage from being
-        # recycled, so an equal (data_ptr, _version) stamp can only mean "the same, unmodified tensor"
-        self._held = None
+        self._ws = StampCache()  # keyed on the (window, fb, dct) the workspace is built from
         self._desc_lists = None  # the descriptor as (ints, floats) for the torch.library ops
 
     @staticmethod
@@ -302,14 +315,11 @@ class FrontendPlan:
         d.db_offset = 10.0 * math.log10(max(1e-10, 1.0))
         return d
 
-    def _stamp_of(self, *tensors):
-        return tuple(None if t is None else (t.data_ptr(), _version_of(t), str(t.device)) for t in tensors)
-
     def workspace(self, window: torch.Tensor, fb: Optional[torch.Tensor], dct: Optional[torch.Tensor]) -> torch.Tensor:
         """Return a prepared workspace, rebuilding it if any constant buffer changed."""
-        stamp = self._stamp_of(window, fb, dct)
-        if self._ws is not None and stamp == self._stamp:
-            return self._ws
+        return self._ws.get((window, fb, dct), self._prepare)
+
+    def _prepare(self, window: torch.Tensor, fb: Optional[torch.Tensor], dct: Optional[torch.Tensor]) -> torch.Tensor:
         lib = _lib.lib()
         _require_cuda_f32(window, "window")
         dev = window.device
@@ -341,7 +351,6 @@ class FrontendPlan:
                 _stream_ptr(dev),
             )
         _lib.check(rc, "frontend_prepare")
-        self._ws, self._stamp, self._held = ws, stamp, (window, fb, dct)
         return ws
 
     def frames(self, length: int) -> int:
@@ -407,7 +416,7 @@ class FrontendPlan:
 
     def _packed_desc(self):
         if self._desc_lists is None:
-            self._desc_lists = _ops.pack_desc(self.desc)
+            self._desc_lists = _ops.pack(self.desc)
         return self._desc_lists
 
 
@@ -417,19 +426,22 @@ _RANK_MESSAGE = ("torch.linalg.lstsq: The least squares solution could not be co
 
 class InverseMelPlan:
     """InverseMelScale's banded L D L^T factorisation of G = fb^T fb (b200a_inverse_mel_plan) on fb's device.  Built on
-    the host from one device-to-host copy of ``fb`` and uploaded once; rebuilt only when ``fb`` changes, by the stamp
-    rule of :meth:`FrontendPlan.workspace`.  The errors of the reference's ``lstsq`` are raised here, at ``forward``."""
+    the host from one device-to-host copy of ``fb`` and uploaded once; rebuilt only when ``fb`` changes (a
+    :class:`StampCache`).  The errors of the reference's ``lstsq`` are raised here, at ``forward``."""
 
     def __init__(self, driver: str):
         self.driver = driver
-        self._plan: Optional[torch.Tensor] = None
-        self._stamp = None
-        self._held = None  # the fb behind the stamp (see FrontendPlan._held)
+        self._cache = StampCache()
+
+    @property
+    def _plan(self) -> Optional[torch.Tensor]:
+        """The uploaded blob of the last build (None before the first)."""
+        return self._cache.value
 
     def plan(self, fb: torch.Tensor) -> torch.Tensor:
-        stamp = (fb.data_ptr(), _version_of(fb), str(fb.device))
-        if self._plan is not None and stamp == self._stamp:
-            return self._plan
+        return self._cache.get((fb,), self._build)
+
+    def _build(self, fb: torch.Tensor) -> torch.Tensor:
         import ctypes
 
         lib = _lib.lib()
@@ -453,8 +465,7 @@ class InverseMelPlan:
                 f"(an underdetermined system), n_mels <= {_lib.INVERSE_MEL_MAX_MELS} and a Gram bandwidth <= "
                 f"{_lib.INVERSE_MEL_MAX_BANDWIDTH} (this bank: {bw.value})")
         _lib.check(rc, "inverse_mel_plan")
-        self._plan, self._stamp, self._held = blob.to(fb.device), stamp, fb
-        return self._plan
+        return blob.to(fb.device)
 
 
 class _InverseMelFunction(torch.autograd.Function):
@@ -509,17 +520,14 @@ class ResamplePlan:
     def __init__(self, orig_r: int, new_r: int, width: int):
         self.orig_r, self.new_r, self.width = int(orig_r), int(new_r), int(width)
         self.taps = 2 * self.width + self.orig_r
-        self._ws: Optional[torch.Tensor] = None
-        self._stamp = None
-        self._kernel: Optional[torch.Tensor] = None
-        self._held = None  # the kernel tensor behind the stamp (see FrontendPlan._held)
-        self._bws: Optional[torch.Tensor] = None
-        self._bws_stamp = None
+        self._forward = StampCache()  # (workspace, contiguous kernel) keyed on the kernel buffer
+        self._backward = StampCache()  # adjoint tables keyed on the contiguous kernel the forward was built from
 
     def workspace(self, kernel: torch.Tensor):
-        stamp = (kernel.data_ptr(), _version_of(kernel), str(kernel.device))
-        if self._ws is not None and stamp == self._stamp:
-            return self._ws, self._kernel
+        """The prepared workspace and the contiguous (new_r, taps) kernel it was built from."""
+        return self._forward.get((kernel,), self._prepare)
+
+    def _prepare(self, kernel: torch.Tensor):
         _require_cuda_f32(kernel, "kernel")
         if kernel.numel() != self.new_r * self.taps:
             raise RuntimeError(
@@ -533,15 +541,14 @@ class ResamplePlan:
             ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             rc = lib.b200a_resample_prepare(k.data_ptr(), self.orig_r, self.new_r, self.width, ws.data_ptr(), nbytes, _stream_ptr(dev))
         _lib.check(rc, "resample_prepare")
-        self._ws, self._stamp, self._kernel, self._held = ws, stamp, k, kernel
         return ws, k
 
     def backward_workspace(self) -> torch.Tensor:
         """The adjoint tables of the kernel the forward workspace was last built from (call after ``workspace``)."""
-        if self._bws is not None and self._bws_stamp == self._stamp:
-            return self._bws
+        return self._backward.get((self._forward.value[1],), self._prepare_backward)
+
+    def _prepare_backward(self, k: torch.Tensor) -> torch.Tensor:
         lib = _lib.lib()
-        k = self._kernel
         dev = k.device
         nbytes = lib.b200a_resample_backward_workspace_bytes(self.orig_r, self.new_r, self.width)
         with torch.cuda.device(dev):
@@ -549,7 +556,6 @@ class ResamplePlan:
             rc = lib.b200a_resample_backward_prepare(k.data_ptr(), self.orig_r, self.new_r, self.width, bws.data_ptr(),
                                                      nbytes, _stream_ptr(dev))
         _lib.check(rc, "resample_backward_prepare")
-        self._bws, self._bws_stamp = bws, self._stamp
         return bws
 
     def run(self, kernel: torch.Tensor, waveform: torch.Tensor) -> torch.Tensor:

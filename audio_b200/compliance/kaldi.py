@@ -398,7 +398,7 @@ def _features(kind: str, rows: Tensor, o: dict) -> Tensor:
     batch = flat.shape[0]
     stage = _lib.STAGE_MEL if mel else _lib.STAGE_POWER
     if frames > 0 and batch > 0:
-        args = (flat, plan, _ops.pack_kaldi_desc(kd), stage, frames, width, stride, bool(o["subtract_mean"]))
+        args = (flat, plan, _ops.pack(kd), stage, frames, width, stride, bool(o["subtract_mean"]))
         return _KaldiFunction.apply(*args) if grad else _launch(*args)
     with torch.cuda.device(dev):
         out = torch.empty((batch, frames, width), dtype=torch.float32, device=dev)

@@ -266,7 +266,7 @@ class _IstftFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, spec3, ws, desc, start, out_len, cut):
-        ctx.ws, ctx.desc_lists, ctx.start, ctx.frames = ws, _ops.pack_desc(desc), start + cut, spec3.shape[2]
+        ctx.ws, ctx.desc_lists, ctx.start, ctx.frames = ws, _ops.pack(desc), start + cut, spec3.shape[2]
         return _istft_run(spec3, ws, desc, start, out_len, cut)
 
     @staticmethod

@@ -19,8 +19,8 @@ import torch
 from torch import Tensor
 
 from . import _lib, _ops
-from ._plans import (_no_autograd, _require_cuda_f32, _RNNTFunction, _version_of, _wants_grad,
-                     is_feature_differentiable, pack_rows)
+from ._plans import (_no_autograd, _require_cuda_f32, _RNNTFunction, _wants_grad, StampCache, is_feature_differentiable,
+                     pack_rows)
 from .transforms import MelSpectrogram
 
 __all__ = ["RNNTFeatureExtractor"]
@@ -65,9 +65,7 @@ class RNNTFeatureExtractor(torch.nn.Module):
         # indices 1, 2 (and 4) of the reference's Sequential are the parameterless transpose, log and pad steps
         self.pipeline = torch.nn.ModuleDict({"0": mel, "3": _GlobalStatsNormalization(global_stats_path)})
         self.right_padding = int(right_padding)
-        self._stats: Optional[Tensor] = None
-        self._stats_stamp = None
-        self._stats_held = None
+        self._stats = StampCache()
 
     @classmethod
     def from_bundle(cls, bundle, global_stats_path: str, streaming: bool = False) -> "RNNTFeatureExtractor":
@@ -85,10 +83,9 @@ class RNNTFeatureExtractor(torch.nn.Module):
     def _packed_stats(self, device: torch.device) -> Tensor:
         """[2][n_mels] (mean, invstddev) on the workspace's device, rebuilt only when either buffer changes."""
         norm = self.pipeline["3"]
-        mean, invstd = norm.mean, norm.invstddev
-        stamp = tuple((t.data_ptr(), _version_of(t), str(t.device)) for t in (mean, invstd))
-        if self._stats is not None and stamp == self._stats_stamp:
-            return self._stats
+        return self._stats.get((norm.mean, norm.invstddev), lambda mean, invstd: self._pack_stats(mean, invstd, device))
+
+    def _pack_stats(self, mean: Tensor, invstd: Tensor, device: torch.device) -> Tensor:
         n_mels = self.pipeline["0"].mel_scale.fb.shape[1]
         for name, t in (("mean", mean), ("invstddev", invstd)):
             _require_cuda_f32(t, name)
@@ -97,9 +94,7 @@ class RNNTFeatureExtractor(torch.nn.Module):
             if t.numel() != n_mels:
                 raise RuntimeError(f"audio_b200: {name} has {t.numel()} elements, expected n_mels={n_mels}")
         with torch.no_grad():
-            stats = torch.stack([mean.reshape(-1), invstd.reshape(-1)]).contiguous()
-        self._stats, self._stats_stamp, self._stats_held = stats, stamp, (mean, invstd)
-        return stats
+            return torch.stack([mean.reshape(-1), invstd.reshape(-1)]).contiguous()
 
     def _prepare(self, waveform: Tensor, lengths_given: bool = False):
         """The plan, workspace, packed statistics and whether the call carries a gradient."""
