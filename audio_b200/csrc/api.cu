@@ -270,7 +270,7 @@ int b200a_istft_run(const b200a_frontend_desc* desc, const void* workspace, cons
                     float* out, int64_t out_row_stride, int64_t start, int64_t out_len, b200a_stream stream) {
   int rc = validate_desc(desc);
   if (rc != B200A_OK) return rc;
-  if (!desc->onesided || desc->n_fft % 2 != 0) return B200A_EUNSUPPORTED;
+  if (!desc->onesided) return B200A_EUNSUPPORTED;
   if (rows < 0 || frames < 1 || out_len < 0 || start < 0 || out_row_stride < out_len) return B200A_EINVAL;
   if (rows == 0 || out_len == 0) return B200A_OK;
   if (workspace == nullptr || spec == nullptr || frame_buf == nullptr || out == nullptr) return B200A_EINVAL;

@@ -925,8 +925,8 @@ __global__ void __launch_bounds__(256) istft_ola_kernel(const float* __restrict_
 
 // First half of b200a_istft_run: the windowed time frames w * irfft(spec) / scale of every frame into frame_buf, on the
 // register FFT for n_fft = 256 / 512 / 1024 (onesided descriptors) and the shared-memory Stockham FFT otherwise.  Any
-// n_fft works, odd ones included (bins (N+1)/2 .. N-1 are the Hermitian mirror of 1 .. (N-1)/2): torch.istft's
-// even-size rule is checked by b200a_istft_run, not needed here.
+// n_fft works, odd ones included (bins (N+1)/2 .. N-1 are the Hermitian mirror of 1 .. (N-1)/2), as torch.istft
+// inverts odd sizes too.
 static int istft_frames_impl(const b200a_frontend_desc* d, const void* ws, const float* spec, int64_t rows, int64_t frames,
                              int64_t stride_row, int64_t stride_bin, int64_t stride_frame, float* frame_buf,
                              cudaStream_t stream) {

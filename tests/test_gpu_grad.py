@@ -61,6 +61,10 @@ SPEC_CASES = [
     (77, 20, None, 0, None, False, True, "reflect", False),
     (512, 128, None, 0, 2.0, False, True, "reflect", False),
     (1024, 256, None, 0, None, "frame_length", True, "replicate", False),
+    (97, 31, None, 0, 2.0, False, True, "reflect", True),
+    (4096, 1024, None, 0, None, False, True, "reflect", True),
+    (2187, 500, None, 0, None, False, True, "reflect", False),
+    (600, 150, 401, 0, 2.0, "window", True, "constant", True),
 ]
 
 

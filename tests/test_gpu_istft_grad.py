@@ -113,17 +113,23 @@ def test_frame_major_input_and_expanded_or_strided_grads(n_fft):
 
 
 def test_odd_n_fft_through_the_op():
-    """Odd n_fft: b200a_istft_run refuses it (torch.istft's even-size rule), the adjoint takes the composition path."""
+    """Odd n_fft, as torch.istft takes it: the forward inverts through the Stockham frame stage, the adjoint takes the
+    composition path."""
     n_fft, hop, frames, rows, start = 77, 20, 40, 2, 38
     window = _window(n_fft, 3)
+    window_t = torch.tensor(window, dtype=torch.float32, device=DEV)
     plan = FrontendPlan(FrontendPlan.make_desc(n_fft, n_fft, hop, 0, True, "reflect", True, False, False, 2.0))
-    ws = plan.workspace(torch.tensor(window, dtype=torch.float32, device=DEV), None, None)
+    ws = plan.workspace(window_t, None, None)
     gen = torch.Generator().manual_seed(n_fft)
+    w32 = np.asarray(torch.tensor(window, dtype=torch.float32), dtype=np.float64)
+    spec = _rand_complex((rows, n_fft // 2 + 1, frames), gen)
+    y = F.inverse_spectrogram(spec.to(DEV), None, 0, window_t, n_fft, hop, n_fft, False)
+    close(y, O.inverse_spectrogram(spec.numpy(), None, 0, w32, n_fft, hop, n_fft))
     g_len = n_fft + hop * (frames - 1) - 2 * start
+    assert tuple(y.shape) == (rows, g_len)
     g = torch.randn(rows, g_len, generator=gen)
     got = _ops.istft_backward(g.to(DEV), ws, *plan._packed_desc(), start, frames)
     got = torch.view_as_complex(got).transpose(1, 2)
-    w32 = np.asarray(torch.tensor(window, dtype=torch.float32), dtype=np.float64)
     close(got, V.inverse_spectrogram_vjp(g.double().numpy(), frames, None, 0, w32, n_fft, hop, n_fft))
 
 

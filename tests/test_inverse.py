@@ -100,7 +100,8 @@ class _nullcontext:
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("n_fft,hop,win", [(400, 100, 400), (512, 128, 512), (1024, 256, 1024), (600, 150, 400)])
+@pytest.mark.parametrize("n_fft,hop,win", [(400, 100, 400), (512, 128, 512), (1024, 256, 1024), (600, 150, 400),
+                                           (2048, 512, 2048), (401, 100, 401)])
 def test_gpu_round_trip(n_fft, hop, win):
     """Spectrogram(power=None) -> InverseSpectrogram returns the waveform (reference transforms_test_impl.py:84-110)."""
     import audio_b200.transforms as T

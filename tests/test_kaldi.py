@@ -178,20 +178,26 @@ def test_gpu_batch_extension_and_edges(kaldi_ref):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("sr", [22050.0, 44100.0, 11025.0])
+@pytest.mark.parametrize("sr,pow2", [pytest.param(22050.0, True, id="22050.0"), pytest.param(44100.0, True, id="44100.0"),
+                                     pytest.param(11025.0, True, id="11025.0"),
+                                     pytest.param(44100.0, False, id="44100.0-unrounded"),
+                                     pytest.param(16000.0, False, id="16000.0-unrounded")])
 @pytest.mark.parametrize("snip", [True, False])
-def test_gpu_other_sample_rates_against_oracle(kaldi_ref, sr, snip):
+def test_gpu_other_sample_rates_against_oracle(kaldi_ref, sr, pow2, snip):
     """Frame sizes that are not multiples of 4 samples (551 / 1102 / 275 at 25 ms) and shifts such as 220: the
     register path stages every unit through the gather (no 16-byte aligned bulk copy), 2048-point frames take the
-    generic kernel."""
+    generic kernel.  round_to_power_of_two=False: the frame length itself is the FFT size (1102 = 2 * 19 * 29, 400),
+    on the generic kernel."""
     import audio_b200.compliance.kaldi as K
 
     x = kaldi_ref["wave"][:1, :15000]
-    kw = dict(sample_frequency=sr, num_mel_bins=40, snip_edges=snip, use_energy=True, low_freq=40.0)
+    kw = dict(sample_frequency=sr, num_mel_bins=40, snip_edges=snip, use_energy=True, low_freq=40.0,
+              round_to_power_of_two=pow2)
     got = K.fbank(torch.from_numpy(x).cuda(), **kw).cpu().numpy()
     exp = KO.fbank(x, **kw)
     assert got.shape == exp.shape
     assert np.abs(got - exp).max() <= 2e-5 * np.abs(exp).max() + 1e-4
-    got = K.mfcc(torch.from_numpy(x).cuda(), sample_frequency=sr, snip_edges=snip, num_mel_bins=30, num_ceps=12).cpu().numpy()
-    exp = KO.mfcc(x, sample_frequency=sr, snip_edges=snip, num_mel_bins=30, num_ceps=12)
+    kw = dict(sample_frequency=sr, snip_edges=snip, num_mel_bins=30, num_ceps=12, round_to_power_of_two=pow2)
+    got = K.mfcc(torch.from_numpy(x).cuda(), **kw).cpu().numpy()
+    exp = KO.mfcc(x, **kw)
     assert got.shape == exp.shape and np.abs(got - exp).max() <= 2e-5 * np.abs(exp).max() + 2e-4
