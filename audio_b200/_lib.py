@@ -24,6 +24,8 @@ LFILTER_MAX_ORDER = 16  # B200A_LFILTER_MAX_ORDER
 FFTCONVOLVE_MAX_PARTITIONS, FFTCONVOLVE_MAX_BLOCK = 128, 2048  # B200A_FFTCONVOLVE_MAX_PARTITIONS; the largest block
 CONVOLVE_MAX_TAPS = 4096  # B200A_CONVOLVE_MAX_TAPS
 VAD_MAX_DFT = 8192  # the largest dft_len of b200a_vad_desc
+DTYPE_F32, DTYPE_F16 = 0, 1  # B200A_DTYPE_*
+RNNT_MAX_U = 8192  # B200A_RNNT_MAX_U
 
 
 class FrontendDesc(ctypes.Structure):
@@ -110,6 +112,21 @@ class VadDesc(ctypes.Structure):
         ("measure_smooth_mult", c_double),
         ("trigger_mult", c_double),
         ("trigger_level", c_double),
+    ]
+
+
+class RnntLossDesc(ctypes.Structure):
+    """Mirror of ``b200a_rnnt_loss_desc``."""
+
+    _fields_ = [
+        ("batch", c_int32),
+        ("max_t", c_int32),
+        ("max_u", c_int32),
+        ("classes", c_int32),
+        ("blank", c_int32),
+        ("dtype", c_int32),
+        ("fused", c_int32),
+        ("clamp", c_float),
     ]
 
 
@@ -278,6 +295,19 @@ _SIGNATURES = {
     "b200a_vad_trigger": (
         ctypes.c_int,
         [POINTER(VadDesc), c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    ),
+    "b200a_rnnt_loss_check": (
+        ctypes.c_int, [c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200a_rnnt_loss_workspace_bytes": (c_size_t, [POINTER(RnntLossDesc)]),
+    "b200a_rnnt_loss_forward": (
+        ctypes.c_int,
+        [POINTER(RnntLossDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+         c_size_t, c_void_p],
+    ),
+    "b200a_rnnt_loss_backward": (
+        ctypes.c_int,
+        [POINTER(RnntLossDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+         c_void_p, c_void_p],
     ),
 }
 

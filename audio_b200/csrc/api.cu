@@ -563,5 +563,29 @@ int b200a_vad_trigger(const b200a_vad_desc* desc, int64_t chunk, int64_t frame0,
                           static_cast<cudaStream_t>(stream));
 }
 
+int b200a_rnnt_loss_check(int32_t batch, int32_t classes, const int32_t* targets, int64_t target_cols,
+                          const int32_t* logit_lengths, const int32_t* target_lengths, int32_t* out,
+                          b200a_stream stream) {
+  return rnnt_loss_check_impl(batch, classes, targets, target_cols, logit_lengths, target_lengths, out,
+                              static_cast<cudaStream_t>(stream));
+}
+
+size_t b200a_rnnt_loss_workspace_bytes(const b200a_rnnt_loss_desc* desc) { return rnnt_loss_workspace_bytes_impl(desc); }
+
+int b200a_rnnt_loss_forward(const b200a_rnnt_loss_desc* desc, const void* logits, const int32_t* targets,
+                            const int32_t* logit_lengths, const int32_t* target_lengths, void* costs, float* denom,
+                            float* alpha, float* beta, void* workspace, size_t workspace_bytes, b200a_stream stream) {
+  return rnnt_loss_forward_impl(desc, logits, targets, logit_lengths, target_lengths, costs, denom, alpha, beta,
+                                workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int b200a_rnnt_loss_backward(const b200a_rnnt_loss_desc* desc, const void* logits, const int32_t* targets,
+                             const int32_t* logit_lengths, const int32_t* target_lengths, const float* denom,
+                             const float* alpha, const float* beta, const void* grad_costs, int64_t grad_costs_stride,
+                             void* grad_logits, b200a_stream stream) {
+  return rnnt_loss_backward_impl(desc, logits, targets, logit_lengths, target_lengths, denom, alpha, beta, grad_costs,
+                                 grad_costs_stride, grad_logits, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -190,6 +190,18 @@ int vad_walk_impl(const b200a_vad_desc* d, int64_t chunk, int64_t frame0, int64_
                   const float* cepstrum_window, float* rows, void* ws, size_t ws_bytes, cudaStream_t stream);
 int vad_trigger_impl(const b200a_vad_desc* d, int64_t chunk, int64_t frame0, int64_t frames, const float* power,
                      float* measures, void* ws, size_t ws_bytes, cudaStream_t stream);
+// rnnt_loss.cu
+size_t rnnt_loss_workspace_bytes_impl(const b200a_rnnt_loss_desc* d);
+int rnnt_loss_check_impl(int32_t batch, int32_t classes, const int32_t* targets, int64_t target_cols,
+                         const int32_t* logit_lengths, const int32_t* target_lengths, int32_t* out,
+                         cudaStream_t stream);
+int rnnt_loss_forward_impl(const b200a_rnnt_loss_desc* d, const void* logits, const int32_t* targets,
+                           const int32_t* logit_lengths, const int32_t* target_lengths, void* costs, float* denom,
+                           float* alpha, float* beta, void* ws, size_t ws_bytes, cudaStream_t stream);
+int rnnt_loss_backward_impl(const b200a_rnnt_loss_desc* d, const void* logits, const int32_t* targets,
+                            const int32_t* logit_lengths, const int32_t* target_lengths, const float* denom,
+                            const float* alpha, const float* beta, const void* grad_costs, int64_t grad_costs_stride,
+                            void* grad_logits, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

@@ -27,6 +27,9 @@ trim, measured on the GPU (the front end's FFT passes around a per-bin walk kern
 FFT convolution: ``fftconvolve`` (functional.py:2222-2258), uniformly partitioned overlap-save on the kernels of
 ``csrc/convolve.cu``.  Direct convolution: ``convolve`` (functional.py:2261-2314), a banded TF32 x 3 tensor-core
 product on the kernels of ``csrc/convolve_direct.cu``, for filters up to 4096 taps.
+
+RNN-T loss: ``rnnt_loss`` (functional.py:1747-1796) on the kernels of ``csrc/rnnt_loss.cu``, float32 or float16 logits,
+differentiable with respect to the logits without a switch.
 """
 from __future__ import annotations
 
@@ -84,6 +87,7 @@ __all__ = [
     "fftconvolve",
     "convolve",
     "vad",
+    "rnnt_loss",
 ]
 
 
@@ -900,3 +904,172 @@ def convolve(x: Tensor, y: Tensor, mode: str = "full") -> Tensor:
             f"{_lib.CONVOLVE_MAX_TAPS} taps (B200A_CONVOLVE_MAX_TAPS); use fftconvolve for longer filters")
     start, out_len = _convolve_slice(n, m, mode)
     return _convolve_rows(_ConvolveFunction, x, y, lx, ly, lo, start, out_len)
+
+
+def _rnnt_check_device(t: Tensor, name: str, logits: Tensor) -> None:
+    if not isinstance(t, Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor")
+    if not t.is_cuda or t.device != logits.device:
+        raise RuntimeError(f"logits and {name} must be on the same device")
+
+
+def _rnnt_inputs(logits: Tensor, targets: Tensor, logit_lengths: Tensor, target_lengths: Tensor, blank: int):
+    """The reference's checks (rnnt/gpu/compute.cu:25-85) in its order and with its messages, then the ones where the
+    reference reads out of bounds.  The lengths are checked on the device by one launch and read back once."""
+    if not isinstance(logits, Tensor):
+        raise TypeError("logits must be a torch.Tensor")
+    if not logits.is_cuda:
+        raise RuntimeError(
+            f"audio_b200: logits is on '{logits.device}'. This package runs only hand-written sm_90a CUDA "
+            "kernels; there is no CPU or ATen fallback -- move the tensor (and the module) to a CUDA device."
+        )
+    _rnnt_check_device(targets, "targets", logits)
+    _rnnt_check_device(logit_lengths, "logit_lengths", logits)
+    _rnnt_check_device(target_lengths, "target_lengths", logits)
+    if logits.dtype not in (torch.float32, torch.float16):
+        raise RuntimeError("logits must be float32 or float16 (half) type")
+    if targets.dtype != torch.int32:
+        raise RuntimeError("targets must be int32 type")
+    if logit_lengths.dtype != torch.int32:
+        raise RuntimeError("logit_lengths must be int32 type")
+    if target_lengths.dtype != torch.int32:
+        raise RuntimeError("target_lengths must be int32 type")
+    for t, name in ((logits, "logits"), (targets, "targets"), (logit_lengths, "logit_lengths"),
+                    (target_lengths, "target_lengths")):
+        if not t.is_contiguous():
+            raise RuntimeError(f"{name} must be contiguous")
+    if logits.dim() != 4:
+        raise RuntimeError("logits must be 4-D (batch, time, target, class)")
+    if targets.dim() != 2:
+        raise RuntimeError("targets must be 2-D (batch, max target length)")
+    if logit_lengths.dim() != 1:
+        raise RuntimeError("logit_lengths must be 1-D")
+    if target_lengths.dim() != 1:
+        raise RuntimeError("target_lengths must be 1-D")
+    batch, max_t, max_u, classes = logits.shape
+    if logit_lengths.size(0) != batch:
+        raise RuntimeError("batch dimension mismatch between logits and logit_lengths")
+    if target_lengths.size(0) != batch:
+        raise RuntimeError("batch dimension mismatch between logits and target_lengths")
+    if targets.size(0) != batch:
+        raise RuntimeError("batch dimension mismatch between logits and targets")
+    if not 0 <= blank < classes:
+        raise RuntimeError("blank must be within [0, logits.shape[-1])")
+    dev = logits.device
+    with torch.cuda.device(dev):
+        stats = torch.empty(5, dtype=torch.int32, device=dev)
+        rc = _lib.lib().b200a_rnnt_loss_check(batch, classes, targets.data_ptr(), targets.size(1),
+                                              logit_lengths.data_ptr(), target_lengths.data_ptr(), stats.data_ptr(),
+                                              _stream_ptr(dev))
+    _lib.check(rc, "rnnt_loss check")
+    t_max, t_min, u_max, u_min, bad_target = stats.tolist()
+    if max_t != t_max:
+        raise RuntimeError("input length mismatch")
+    if max_u != u_max + 1:
+        raise RuntimeError("output length mismatch")
+    if targets.size(1) + 1 != max_u:
+        raise RuntimeError("target length mismatch")
+    if t_min < 1:
+        raise ValueError(f"rnnt_loss: every logit_lengths entry must be at least 1 (got {t_min})")
+    if u_min < 0:
+        raise ValueError(f"rnnt_loss: target_lengths entries must be non-negative (got {u_min})")
+    if bad_target:
+        raise ValueError(f"rnnt_loss: a target within its sequence's target_length lies outside [0, {classes})")
+    if max_u > _lib.RNNT_MAX_U:
+        raise ValueError(f"rnnt_loss: logits.shape[2] = {max_u} is above the supported {_lib.RNNT_MAX_U}")
+
+
+def _rnnt_desc(logits: Tensor, blank: int, clamp: float, fused: bool):
+    batch, max_t, max_u, classes = logits.shape
+    return _lib.RnntLossDesc(batch, max_t, max_u, classes, blank,
+                             _lib.DTYPE_F16 if logits.dtype == torch.float16 else _lib.DTYPE_F32, int(bool(fused)),
+                             float(clamp))
+
+
+def _rnnt_forward(logits, targets, logit_lengths, target_lengths, desc, save: bool):
+    """b200a_rnnt_loss_forward: the costs, and the float32 (denom, alpha, beta) of the gradient when ``save``."""
+    dev = logits.device
+    batch, max_t, max_u, _ = logits.shape
+    with torch.cuda.device(dev):
+        costs = torch.empty(batch, dtype=logits.dtype, device=dev)
+        ws = torch.empty(_lib.lib().b200a_rnnt_loss_workspace_bytes(desc), dtype=torch.uint8, device=dev)
+        saved = [torch.empty((batch, max_t, max_u), dtype=torch.float32, device=dev) if save and (k or desc.fused)
+                 else None for k in range(3)]
+        denom, alpha, beta = saved
+        rc = _lib.lib().b200a_rnnt_loss_forward(
+            desc, logits.data_ptr(), targets.data_ptr(), logit_lengths.data_ptr(), target_lengths.data_ptr(),
+            costs.data_ptr(), 0 if denom is None else denom.data_ptr(), 0 if alpha is None else alpha.data_ptr(),
+            0 if beta is None else beta.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(dev))
+    _lib.check(rc, "rnnt_loss")
+    return costs, denom, alpha, beta
+
+
+class _RnntLossFunction(torch.autograd.Function):
+    """_rnnt_forward with the logit gradient.  Saved: the inputs through save_for_backward (so an in-place edit of the
+    logits before backward is an error) and per-(b, t, u) float32 denom / alpha / beta; nothing joint-sized."""
+
+    @staticmethod
+    def forward(ctx, logits, targets, logit_lengths, target_lengths, desc):
+        costs, denom, alpha, beta = _rnnt_forward(logits, targets, logit_lengths, target_lengths, desc, True)
+        ctx.desc = desc
+        ctx.fused = denom is not None
+        ctx.save_for_backward(logits, targets, logit_lengths, target_lengths, alpha, beta,
+                              *((denom,) if denom is not None else ()))
+        return costs
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        logits, targets, logit_lengths, target_lengths, alpha, beta, *rest = ctx.saved_tensors
+        denom = rest[0] if ctx.fused else None
+        dev = logits.device
+        if dy.dim() != 1 or dy.dtype != logits.dtype:
+            dy = dy.reshape(-1).to(logits.dtype)
+        with torch.cuda.device(dev):
+            grad = torch.empty_like(logits)
+            rc = _lib.lib().b200a_rnnt_loss_backward(
+                ctx.desc, logits.data_ptr(), targets.data_ptr(), logit_lengths.data_ptr(), target_lengths.data_ptr(),
+                0 if denom is None else denom.data_ptr(), alpha.data_ptr(), beta.data_ptr(), dy.data_ptr(),
+                dy.stride(0), grad.data_ptr(), _stream_ptr(dev))
+        _lib.check(rc, "rnnt_loss backward")
+        return grad, None, None, None, None
+
+
+def rnnt_loss(
+    logits: Tensor,
+    targets: Tensor,
+    logit_lengths: Tensor,
+    target_lengths: Tensor,
+    blank: int = -1,
+    clamp: float = -1,
+    reduction: str = "mean",
+    fused_log_softmax: bool = True,
+):
+    """The RNN Transducer loss of Graves (2012) (reference functional.py:1747-1796): logits ``(batch, max seq length,
+    max target length + 1, class)`` in float32 or float16, int32 targets ``(batch, max target length)`` and lengths
+    ``(batch,)``, all contiguous on one CUDA device.  Returns the costs (``reduction="none"``, shape ``(batch,)``) or
+    their mean or sum, in the logits' dtype; the arithmetic is float32.
+
+    Differentiable with respect to ``logits`` whenever grad mode is on and ``logits.requires_grad``, with no
+    ``audio_b200.differentiable`` switch: a loss exists to be differentiated.  Otherwise nothing is saved and no gradient
+    kernel runs.  ``clamp > 0`` clamps each unscaled gradient element to ``[-clamp, clamp]`` (as the reference's CPU
+    path) before the upstream gradient scales it.  A sequence whose paths all have probability 0 costs NaN (or inf when
+    T or U + 1 is 1) and gets a zero gradient.  Beyond the reference's checks, raises ``ValueError`` for a
+    ``logit_lengths`` entry below 1, a negative ``target_lengths`` entry and a target outside ``[0, class)`` within its
+    sequence's length, where the reference reads out of bounds.
+    """
+    if reduction not in ["none", "mean", "sum"]:
+        raise ValueError('reduction should be one of "none", "mean", or "sum"')
+    if blank < 0:  # reinterpret blank index if blank < 0.
+        blank = logits.shape[-1] + blank
+    _rnnt_inputs(logits, targets, logit_lengths, target_lengths, blank)
+    desc = _rnnt_desc(logits, blank, clamp, fused_log_softmax)
+    if torch.is_grad_enabled() and logits.requires_grad:
+        costs = _RnntLossFunction.apply(logits, targets, logit_lengths, target_lengths, desc)
+    else:
+        costs = _rnnt_forward(logits, targets, logit_lengths, target_lengths, desc, False)[0]
+    if reduction == "mean":
+        return costs.mean()
+    elif reduction == "sum":
+        return costs.sum()
+    return costs

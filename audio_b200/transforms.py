@@ -16,7 +16,7 @@ LFCC, AmplitudeToDB, MelScale, InverseMelScale and SpectralCentroid with ``featu
 (``audio_b200.compliance.kaldi``) with ``kaldi=True``, TimeStretch (spectrogram gradient) and PitchShift
 (waveform gradient) with ``vocoder=True``, and Preemphasis and Deemphasis (waveform gradient) and Convolve and
 FFTConvolve (input gradients) with ``filtering=True``.
-GriffinLim is forward-only.
+GriffinLim is forward-only.  RNNTLoss is differentiable with respect to the logits without a switch.
 """
 from __future__ import annotations
 
@@ -34,7 +34,7 @@ from ._plans import (FrontendPlan, InverseMelPlan, ResamplePlan, _InverseMelFunc
 
 __all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "InverseMelScale", "MelSpectrogram", "MFCC", "LFCC",
            "SpectralCentroid", "Resample", "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift", "Preemphasis",
-           "Deemphasis", "FFTConvolve", "Convolve", "Vad"]
+           "Deemphasis", "FFTConvolve", "Convolve", "Vad", "RNNTLoss"]
 
 
 def _setup_framing(mod, n_fft, win_length, hop_length, window_fn=None, wkwargs=None, hop_div=2):
@@ -797,6 +797,23 @@ class Vad(torch.nn.Module):
         if self._plan is None or self._plan[0] != params:  # rebuilt only when an attribute was changed
             self._plan = (params, _filtering.VadPlan(*params))
         return _filtering._vad_trim(waveform, self._plan[1])
+
+
+class RNNTLoss(torch.nn.Module):
+    """The RNN Transducer loss (reference _transforms.py:1783-1850): ``forward(logits, targets, logit_lengths,
+    target_lengths)`` is :func:`audio_b200.functional.rnnt_loss` with this module's ``blank``, ``clamp``, ``reduction``
+    and ``fused_log_softmax``."""
+
+    def __init__(self, blank: int = -1, clamp: float = -1.0, reduction: str = "mean", fused_log_softmax: bool = True):
+        super().__init__()
+        self.blank = blank
+        self.clamp = clamp
+        self.reduction = reduction
+        self.fused_log_softmax = fused_log_softmax
+
+    def forward(self, logits: Tensor, targets: Tensor, logit_lengths: Tensor, target_lengths: Tensor):
+        return F.rnnt_loss(logits, targets, logit_lengths, target_lengths, self.blank, self.clamp, self.reduction,
+                           self.fused_log_softmax)
 
 
 # ---- B200A_REFERENCE=1: A/B switch to the reference implementation (debugging only, never silent) -----------------

@@ -683,6 +683,64 @@ int b200a_vad_walk(const b200a_vad_desc* desc, int64_t chunk, int64_t frame0, in
 int b200a_vad_trigger(const b200a_vad_desc* desc, int64_t chunk, int64_t frame0, int64_t frames, const float* power,
                       float* measures, void* workspace, size_t workspace_bytes, b200a_stream stream);
 
+/* ---- RNN-T loss: rnnt_loss (functional.py:1747-1796, rnnt/cpu/cpu_kernels.h) -------------------------------- */
+/*
+ * The transducer loss of a joiner output logits[batch][max_t][max_u][classes] (max_u = max target length + 1) in
+ * float32 or float16; every step is float32.  Per sequence b with T = logit_lengths[b] >= 1 and U =
+ * target_lengths[b] + 1, on the valid rows t < T, u < U:
+ *   denom(t, u) = log sum_k exp(logits[b][t][u][k])                         (fused only)
+ *   skip(t, u) = logits[..][blank] - denom,  emit(t, u) = logits[..][targets[b][u]] - denom  (u < U - 1; raw logits
+ *   when fused == 0);  alpha / beta by the reference's recursions and lse (max + log1p(exp(min - max)), so the lse of
+ *   two -inf is NaN);  cost[b] = -beta(0, 0).
+ * The logit gradient (b200a_rnnt_loss_backward) is the reference CPU's formula per element, clamped to [-clamp, clamp]
+ * when clamp > 0, times grad_costs[b]; rows outside (T, U) and every row of a sequence whose cost is not finite are 0.
+ * No atomics in the loss kernels: reruns are bit-identical.
+ */
+#define B200A_DTYPE_F32 0
+#define B200A_DTYPE_F16 1
+#define B200A_RNNT_MAX_U 8192 /* max_u cap (B200A_EUNSUPPORTED above): the alpha / beta CTA stages 24 bytes per column */
+
+typedef struct b200a_rnnt_loss_desc {
+  int32_t batch;   /* >= 1 */
+  int32_t max_t;   /* logits.shape[1] = max(logit_lengths) >= 1 */
+  int32_t max_u;   /* logits.shape[2] = max(target_lengths) + 1; targets is [batch][max_u - 1] */
+  int32_t classes; /* >= 1 */
+  int32_t blank;   /* in [0, classes) */
+  int32_t dtype;   /* B200A_DTYPE_F32 or B200A_DTYPE_F16: logits, costs, grad_costs and grad_logits */
+  int32_t fused;   /* 1: log-softmax inside the loss; 0: the logits are log-probabilities already */
+  float clamp;     /* gradient clamp when > 0 */
+} b200a_rnnt_loss_desc;
+
+/*
+ * Input check, one CTA: out[0..4] = {max, min of logit_lengths; max, min of target_lengths; 1 if a target
+ * targets[b][j] with j < target_lengths[b] (and j < target_cols) lies outside [0, classes), else 0}.  batch == 0 gives
+ * {INT32_MIN, INT32_MAX, INT32_MIN, INT32_MAX, 0}.  targets is [batch][target_cols] contiguous.
+ */
+int b200a_rnnt_loss_check(int32_t batch, int32_t classes, const int32_t* targets, int64_t target_cols,
+                          const int32_t* logit_lengths, const int32_t* target_lengths, int32_t* out,
+                          b200a_stream stream);
+/* Workspace bytes of b200a_rnnt_loss_forward: the (skip, emit) pair of every row; 0 for an invalid descriptor. */
+size_t b200a_rnnt_loss_workspace_bytes(const b200a_rnnt_loss_desc* desc);
+/*
+ *   costs              : [batch] in the logits' dtype
+ *   denom, alpha, beta : [batch][max_t][max_u] float32, the valid rows written; all null for a forward without a
+ *                        gradient (only beta is walked), else alpha and beta, and denom when fused
+ * The lengths and targets must have passed b200a_rnnt_loss_check's conditions (lengths within the shape, T >= 1,
+ * U >= 1, targets in range); nothing here reads them back.  B200A_EINVAL for null pointers or fields out of range,
+ * B200A_EUNSUPPORTED for max_u > B200A_RNNT_MAX_U, B200A_EWORKSPACE for a short workspace.
+ */
+int b200a_rnnt_loss_forward(const b200a_rnnt_loss_desc* desc, const void* logits, const int32_t* targets,
+                            const int32_t* logit_lengths, const int32_t* target_lengths, void* costs, float* denom,
+                            float* alpha, float* beta, void* workspace, size_t workspace_bytes, b200a_stream stream);
+/*
+ * grad_logits[b][t][u][k] for every element, written once; grad_costs[b * grad_costs_stride] (0: an expanded scalar).
+ * denom may be null when fused == 0.  Statuses as b200a_rnnt_loss_forward.
+ */
+int b200a_rnnt_loss_backward(const b200a_rnnt_loss_desc* desc, const void* logits, const int32_t* targets,
+                             const int32_t* logit_lengths, const int32_t* target_lengths, const float* denom,
+                             const float* alpha, const float* beta, const void* grad_costs, int64_t grad_costs_stride,
+                             void* grad_logits, b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);

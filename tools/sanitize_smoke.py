@@ -102,5 +102,17 @@ F.convolve(x, torch.randn(3, 1025, device="cuda"), "same")
 from audio_b200 import _filtering  # noqa: E402
 _filtering.VadPlan(16000, trigger_level=1e9).run(x, chunk=7)
 F.vad(x[:1, :1000], 16000)
+# rnnt_loss: forward + backward in float32 and float16 with ragged lengths and a V with a vector tail, U + 1 > 1024
+# (more cells per diagonal than threads), the non-fused path, and a forward without a gradient
+for dt, (B_, T_, U_, V_) in ((torch.float32, (3, 9, 6, 29)), (torch.float16, (2, 5, 4, 4097)),
+                             (torch.float16, (2, 3, 1030, 3))):
+    lg = torch.randn(B_, T_, U_, V_, device="cuda", dtype=dt, requires_grad=True)
+    tl = torch.tensor([T_] + [max(1, T_ - 2)] * (B_ - 1), dtype=torch.int32, device="cuda")
+    ul = torch.tensor([max(0, U_ - 3)] * (B_ - 1) + [U_ - 1], dtype=torch.int32, device="cuda")
+    tg = torch.randint(0, V_ - 1, (B_, U_ - 1), dtype=torch.int32, device="cuda")
+    F.rnnt_loss(lg, tg, tl, ul).backward()
+    F.rnnt_loss(lg, tg, tl, ul, clamp=0.1, fused_log_softmax=False, reduction="none").sum().backward()
+    with torch.no_grad():
+        F.rnnt_loss(lg, tg, tl, ul, blank=0)
 torch.cuda.synchronize()
 print("done")
