@@ -24,8 +24,10 @@ LFILTER_MAX_ORDER = 16  # B200A_LFILTER_MAX_ORDER
 FFTCONVOLVE_MAX_PARTITIONS, FFTCONVOLVE_MAX_BLOCK = 128, 2048  # B200A_FFTCONVOLVE_MAX_PARTITIONS; the largest block
 CONVOLVE_MAX_TAPS = 4096  # B200A_CONVOLVE_MAX_TAPS
 VAD_MAX_DFT = 8192  # the largest dft_len of b200a_vad_desc
-DTYPE_F32, DTYPE_F16 = 0, 1  # B200A_DTYPE_*
+DTYPE_F32, DTYPE_F16, DTYPE_F64 = 0, 1, 2  # B200A_DTYPE_*
 RNNT_MAX_U = 8192  # B200A_RNNT_MAX_U
+INDEX_I32, INDEX_I64 = 0, 1  # B200A_INDEX_*
+FORCED_ALIGN_MAX_L = 8191  # B200A_FORCED_ALIGN_MAX_L
 
 
 class FrontendDesc(ctypes.Structure):
@@ -127,6 +129,21 @@ class RnntLossDesc(ctypes.Structure):
         ("dtype", c_int32),
         ("fused", c_int32),
         ("clamp", c_float),
+    ]
+
+
+class ForcedAlignDesc(ctypes.Structure):
+    """Mirror of ``b200a_forced_align_desc``."""
+
+    _fields_ = [
+        ("batch", c_int32),
+        ("max_t", c_int32),
+        ("max_l", c_int32),
+        ("classes", c_int32),
+        ("blank", c_int32),
+        ("dtype", c_int32),
+        ("target_dtype", c_int32),
+        ("length_dtype", c_int32),
     ]
 
 
@@ -309,6 +326,14 @@ _SIGNATURES = {
         [POINTER(RnntLossDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
          c_void_p, c_void_p],
     ),
+    "b200a_forced_align_check": (
+        ctypes.c_int,
+        [POINTER(ForcedAlignDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b200a_forced_align_workspace_bytes": (c_size_t, [POINTER(ForcedAlignDesc)]),
+    "b200a_forced_align_run": (
+        ctypes.c_int,
+        [POINTER(ForcedAlignDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+         c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -587,5 +587,23 @@ int b200a_rnnt_loss_backward(const b200a_rnnt_loss_desc* desc, const void* logit
                                  grad_costs_stride, grad_logits, static_cast<cudaStream_t>(stream));
 }
 
+int b200a_forced_align_check(const b200a_forced_align_desc* desc, const void* targets, const void* input_lengths,
+                             const void* target_lengths, int64_t* out, void* workspace, size_t workspace_bytes,
+                             b200a_stream stream) {
+  return forced_align_check_impl(desc, targets, input_lengths, target_lengths, out, workspace, workspace_bytes,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+size_t b200a_forced_align_workspace_bytes(const b200a_forced_align_desc* desc) {
+  return forced_align_workspace_bytes_impl(desc);
+}
+
+int b200a_forced_align_run(const b200a_forced_align_desc* desc, const void* log_probs, const void* targets,
+                           const void* input_lengths, const void* target_lengths, void* paths, void* scores,
+                           void* workspace, size_t workspace_bytes, b200a_stream stream) {
+  return forced_align_run_impl(desc, log_probs, targets, input_lengths, target_lengths, paths, scores, workspace,
+                               workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -202,6 +202,13 @@ int rnnt_loss_backward_impl(const b200a_rnnt_loss_desc* d, const void* logits, c
                             const int32_t* logit_lengths, const int32_t* target_lengths, const float* denom,
                             const float* alpha, const float* beta, const void* grad_costs, int64_t grad_costs_stride,
                             void* grad_logits, cudaStream_t stream);
+// forced_align.cu
+size_t forced_align_workspace_bytes_impl(const b200a_forced_align_desc* d);
+int forced_align_check_impl(const b200a_forced_align_desc* d, const void* targets, const void* input_lengths,
+                            const void* target_lengths, int64_t* out, void* ws, size_t ws_bytes, cudaStream_t stream);
+int forced_align_run_impl(const b200a_forced_align_desc* d, const void* log_probs, const void* targets,
+                          const void* input_lengths, const void* target_lengths, void* paths, void* scores, void* ws,
+                          size_t ws_bytes, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

@@ -30,13 +30,17 @@ product on the kernels of ``csrc/convolve_direct.cu``, for filters up to 4096 ta
 
 RNN-T loss: ``rnnt_loss`` (functional.py:1747-1796) on the kernels of ``csrc/rnnt_loss.cu``, float32 or float16 logits,
 differentiable with respect to the logits without a switch.
+
+CTC forced alignment: ``forced_align`` (functional/_alignment.py) on the kernels of ``csrc/forced_align.cu``, batched
+with ragged lengths, bit-identical to the reference CPU per sequence; ``merge_tokens`` and ``TokenSpan`` on the host.
 """
 from __future__ import annotations
 
 import collections
 import math
 import warnings
-from typing import Optional, Union
+from dataclasses import dataclass
+from typing import List, Optional, Tuple, Union
 
 import torch
 from torch import Tensor
@@ -88,6 +92,9 @@ __all__ = [
     "convolve",
     "vad",
     "rnnt_loss",
+    "forced_align",
+    "merge_tokens",
+    "TokenSpan",
 ]
 
 
@@ -1073,3 +1080,170 @@ def rnnt_loss(
     elif reduction == "sum":
         return costs.sum()
     return costs
+
+
+_FA_DTYPES = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.float64: _lib.DTYPE_F64}
+_INDEX_DTYPES = {torch.int32: _lib.INDEX_I32, torch.int64: _lib.INDEX_I64}
+
+
+def _fa_tensor(t, name: str, log_probs: Tensor) -> None:
+    if not isinstance(t, Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor")
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor")
+    if t.device != log_probs.device:
+        raise RuntimeError(f"log_probs and {name} need to be on the same device")
+
+
+def forced_align(
+    log_probs: Tensor,
+    targets: Tensor,
+    input_lengths: Optional[Tensor] = None,
+    target_lengths: Optional[Tensor] = None,
+    blank: int = 0,
+) -> Tuple[Tensor, Tensor]:
+    """Align CTC label sequences to emissions (reference functional/_alignment.py): the Viterbi path of
+    ``targets`` ``(B, L)`` (int32 or int64) through ``log_probs`` ``(B, T, C)`` (float32, float16 or float64), both
+    contiguous on one CUDA device, with optional ``(B,)`` int32 / int64 lengths of any strides (the full sizes when
+    ``None``).
+
+    Returns ``(paths, scores)``, both ``(B, T)``: the label of every frame in the targets' dtype and its log-probability
+    in the log-probs' dtype.  Row ``b`` is exactly the reference CPU's alignment of ``log_probs[b:b+1, :T_b]`` and
+    ``targets[b:b+1, :L_b]`` (same path, same scores, same tie-breaking); frames ``t >= T_b`` hold ``blank`` and 0, and a
+    row with ``L_b = 0`` is all blank.  The reference takes ``B == 1`` only.  The outputs do not require grad.
+
+    Raises as the reference does, with its messages; the blank and range checks cover each sequence's first ``L_b``
+    targets.  Beyond them, raises ``ValueError`` for a negative target, an ``input_lengths`` entry below 1, a negative
+    ``target_lengths`` entry, and ``L`` above ``B200A_FORCED_ALIGN_MAX_L`` (8191).  One launch checks the inputs and
+    its result is read back once; the alignment itself is one more launch.
+    """
+    if not isinstance(log_probs, Tensor):
+        raise TypeError("log_probs must be a torch.Tensor")
+    if not log_probs.is_cuda:
+        raise RuntimeError(
+            f"audio_b200: log_probs is on '{log_probs.device}'. This package runs only hand-written sm_90a CUDA "
+            "kernels; there is no CPU or ATen fallback -- move the tensor (and the module) to a CUDA device."
+        )
+    _fa_tensor(targets, "targets", log_probs)
+    dev = log_probs.device
+    for t, name in ((input_lengths, "input_lengths"), (target_lengths, "target_lengths")):
+        if t is not None:
+            _fa_tensor(t, name, log_probs)
+    if log_probs.dtype not in _FA_DTYPES:
+        raise RuntimeError("log_probs must be float64, float32 or float16 (half) type")
+    if targets.dtype not in _INDEX_DTYPES:
+        raise RuntimeError("targets must be int32 or int64 type")
+    for t, name in ((input_lengths, "input_lengths"), (target_lengths, "target_lengths")):
+        if t is not None and t.dtype not in _INDEX_DTYPES:
+            raise RuntimeError(f"{name} must be int32 or int64 type")
+    if not log_probs.is_contiguous():
+        raise RuntimeError("log_probs must be contiguous")
+    if not targets.is_contiguous():
+        raise RuntimeError("targets must be contiguous")
+    if log_probs.dim() != 3:
+        raise RuntimeError("log_probs must be 3-D (batch_size, input length, num classes)")
+    if targets.dim() != 2:
+        raise RuntimeError("targets must be 2-D (batch_size, target length,)")
+    if input_lengths is None:
+        input_lengths = torch.full((log_probs.size(0),), log_probs.size(1), dtype=torch.int64, device=dev)
+    if target_lengths is None:
+        target_lengths = torch.full((targets.size(0),), targets.size(1), dtype=torch.int64, device=dev)
+    if input_lengths.dim() != 1:
+        raise RuntimeError("input_lengths must be 1-D (batch_size,)")
+    if target_lengths.dim() != 1:
+        raise RuntimeError("target_lengths must be 1-D (batch_size,)")
+    batch, max_t, classes = log_probs.shape
+    if targets.size(0) != batch or input_lengths.size(0) != batch or target_lengths.size(0) != batch:
+        raise RuntimeError("log_probs, targets, input_lengths and target_lengths must have the same batch size")
+    if targets.numel() == 0:  # the reference's torch.max(targets)
+        raise RuntimeError("max(): Expected reduction dim to be specified for input.numel() == 0. "
+                           "Specify the reduction dim with the 'dim' argument.")
+    if batch == 0 or max_t == 0:
+        raise ValueError("forced_align: log_probs must have at least one sequence and one frame")
+    # The kernels read both lengths as dense (B,) vectors of one dtype.  Like the reference (which takes their max()),
+    # any 1-D strides are accepted: a strided or expanded vector is copied, B elements.
+    len_dtype = input_lengths.dtype if input_lengths.dtype == target_lengths.dtype else torch.int64
+    input_lengths = input_lengths.to(len_dtype).contiguous()
+    target_lengths = target_lengths.to(len_dtype).contiguous()
+    max_l = targets.size(1)
+    # a blank outside int32 reaches the check as -1, whose blank flag then means nothing and is ignored below
+    blank_fits = -(2**31) <= blank < 2**31
+    blank32 = blank if blank_fits else -1
+    desc = _lib.ForcedAlignDesc(batch, max_t, min(max_l, 2**31 - 1), classes, blank32, _FA_DTYPES[log_probs.dtype],
+                                _INDEX_DTYPES[targets.dtype], _INDEX_DTYPES[input_lengths.dtype])
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        ws = torch.empty(max(lib.b200a_forced_align_workspace_bytes(desc), 4 * batch), dtype=torch.uint8, device=dev)
+        stats = torch.empty(11, dtype=torch.int64, device=dev)
+        rc = lib.b200a_forced_align_check(desc, targets.data_ptr(), input_lengths.data_ptr(),
+                                          target_lengths.data_ptr(), stats.data_ptr(), ws.data_ptr(), ws.numel(),
+                                          _stream_ptr(dev))
+        _lib.check(rc, "forced_align check")
+        t_max, t_min, l_max, l_min, out_of_range, negative, has_blank, bad, bad_t, bad_l, bad_r = stats.tolist()
+    if has_blank and blank_fits:
+        raise ValueError(f"targets Tensor shouldn't contain blank index. Found {targets}.")
+    if out_of_range:
+        raise ValueError("targets values must be less than the CTC dimension")
+    if not 0 <= blank < classes:
+        raise RuntimeError("blank must be within [0, num classes)")
+    if negative:
+        raise ValueError("forced_align: a target within its sequence's target_length is negative")
+    if max_t != t_max:
+        raise RuntimeError("input length mismatch")
+    if max_l != l_max:
+        raise RuntimeError("target length mismatch")
+    if t_min < 1:
+        raise ValueError(f"forced_align: every input_lengths entry must be at least 1 (got {t_min})")
+    if l_min < 0:
+        raise ValueError(f"forced_align: target_lengths entries must be non-negative (got {l_min})")
+    if bad >= 0:
+        raise RuntimeError(f"targets length is too long for CTC. Found log_probs length: {bad_t}, targets length: "
+                           f"{bad_l}, and number of repeats: {bad_r}")
+    if max_l > _lib.FORCED_ALIGN_MAX_L:
+        raise ValueError(f"forced_align: targets.shape[1] = {max_l} is above the supported {_lib.FORCED_ALIGN_MAX_L}")
+    with torch.cuda.device(dev):
+        paths = torch.empty((batch, max_t), dtype=targets.dtype, device=dev)
+        scores = torch.empty((batch, max_t), dtype=log_probs.dtype, device=dev)
+        rc = lib.b200a_forced_align_run(desc, log_probs.data_ptr(), targets.data_ptr(), input_lengths.data_ptr(),
+                                        target_lengths.data_ptr(), paths.data_ptr(), scores.data_ptr(), ws.data_ptr(),
+                                        ws.numel(), _stream_ptr(dev))
+    _lib.check(rc, "forced_align")
+    return paths, scores
+
+
+@dataclass
+class TokenSpan:
+    """One token of an alignment with its frame span and score, as :func:`merge_tokens` returns it."""
+
+    token: int
+    """The token."""
+    start: int
+    """The first frame of the span (inclusive)."""
+    end: int
+    """The frame after the span (exclusive)."""
+    score: float
+    """The mean of the frame scores over the span."""
+
+    def __len__(self) -> int:
+        """The span's length in frames."""
+        return self.end - self.start
+
+
+def merge_tokens(tokens: Tensor, scores: Tensor, blank: int = 0) -> List[TokenSpan]:
+    """Collapse an unbatched alignment (a row of :func:`forced_align`'s ``paths`` and ``scores``, shape ``(T,)``) into
+    spans of repeated non-blank tokens, each scored by the mean of its frames' scores (reference
+    functional/_alignment.py).  Both tensors are copied to the host once; every span is built there."""
+    if tokens.ndim != 1 or scores.ndim != 1:
+        raise ValueError("`tokens` and `scores` must be 1D Tensor.")
+    if len(tokens) != len(scores):
+        raise ValueError("`tokens` and `scores` must be the same length.")
+    scores = scores.detach().cpu()
+    ids = tokens.tolist()
+    spans = []
+    start = 0
+    for t in range(1, len(ids) + 1):
+        if t == len(ids) or ids[t] != ids[start]:
+            if ids[start] != blank:
+                spans.append(TokenSpan(token=ids[start], start=start, end=t, score=scores[start:t].mean().item()))
+            start = t
+    return spans

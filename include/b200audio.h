@@ -741,6 +741,55 @@ int b200a_rnnt_loss_backward(const b200a_rnnt_loss_desc* desc, const void* logit
                              const float* alpha, const float* beta, const void* grad_costs, int64_t grad_costs_stride,
                              void* grad_logits, b200a_stream stream);
 
+/* ---- CTC forced alignment: forced_align (functional/_alignment.py, forced_align/cpu/compute.cpp) --------------- */
+/*
+ * The Viterbi alignment of targets[batch][max_l] to log_probs[batch][max_t][classes] (float32, float16 or float64),
+ * per sequence b with T_b = input_lengths[b] >= 1 and L_b = target_lengths[b]: the reference CPU's band, its tie rules
+ * and its arithmetic in the input dtype, so every row equals the reference's alignment of that row alone, bit for bit.
+ *   paths  : [batch][max_t] in the targets' dtype; frames t >= T_b hold blank, a row with L_b = 0 is all blank
+ *   scores : [batch][max_t] in the log-probs' dtype, log_probs[b][t][paths[b][t]]; 0 for t >= T_b
+ * One CTA per sequence in one launch, no atomics: reruns are bit-identical.
+ */
+#define B200A_DTYPE_F64 2
+#define B200A_INDEX_I32 0
+#define B200A_INDEX_I64 1
+/* max_l cap (B200A_EUNSUPPORTED above): 2 max_l + 1 states in the registers of 512 threads */
+#define B200A_FORCED_ALIGN_MAX_L 8191
+
+typedef struct b200a_forced_align_desc {
+  int32_t batch;        /* >= 1 */
+  int32_t max_t;        /* log_probs.shape[1] >= 1 */
+  int32_t max_l;        /* targets.shape[1] >= 0 */
+  int32_t classes;      /* >= 1 */
+  int32_t blank;        /* in [0, classes) (any value for b200a_forced_align_check) */
+  int32_t dtype;        /* B200A_DTYPE_F32, B200A_DTYPE_F16 or B200A_DTYPE_F64: log_probs and scores */
+  int32_t target_dtype; /* B200A_INDEX_I32 or B200A_INDEX_I64: targets and paths */
+  int32_t length_dtype; /* B200A_INDEX_I32 or B200A_INDEX_I64: input_lengths and target_lengths */
+} b200a_forced_align_desc;
+
+/*
+ * Input check, one CTA: out[0..10] = {max, min of input_lengths; max, min of target_lengths; 1 if a target
+ * targets[b][j] with j < min(target_lengths[b], max_l) is >= classes, else 0; the same for < 0; the same for == blank;
+ * the first b with input_lengths[b] < target_lengths[b] + R_b (R_b: the repeats targets[b][j] == targets[b][j - 1]
+ * among those targets) or -1, and that sequence's (T_b, L_b, R_b)}.  Writes R_b as int32 to workspace[0 .. batch), the
+ * walk's input: the workspace of b200a_forced_align_run, or at least 4 * batch bytes.  Accepts max_l above the cap.
+ */
+int b200a_forced_align_check(const b200a_forced_align_desc* desc, const void* targets, const void* input_lengths,
+                             const void* target_lengths, int64_t* out, void* workspace, size_t workspace_bytes,
+                             b200a_stream stream);
+/* Workspace bytes of b200a_forced_align_run (R_b and 2-bit backpointers per frame and state); 0 for an invalid
+ * descriptor or max_l above B200A_FORCED_ALIGN_MAX_L. */
+size_t b200a_forced_align_workspace_bytes(const b200a_forced_align_desc* desc);
+/*
+ * The workspace must hold b200a_forced_align_check's R_b for these targets and lengths, and the lengths must have
+ * passed its conditions (1 <= T_b <= max_t, 0 <= L_b <= max_l, T_b >= L_b + R_b, targets in [0, classes)); nothing here
+ * reads them back.  B200A_EINVAL for null pointers or fields out of range, B200A_EUNSUPPORTED for max_l above
+ * B200A_FORCED_ALIGN_MAX_L, B200A_EWORKSPACE for a short workspace.
+ */
+int b200a_forced_align_run(const b200a_forced_align_desc* desc, const void* log_probs, const void* targets,
+                           const void* input_lengths, const void* target_lengths, void* paths, void* scores,
+                           void* workspace, size_t workspace_bytes, b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);

@@ -114,5 +114,9 @@ for dt, (B_, T_, U_, V_) in ((torch.float32, (3, 9, 6, 29)), (torch.float16, (2,
     F.rnnt_loss(lg, tg, tl, ul, clamp=0.1, fused_log_softmax=False, reduction="none").sum().backward()
     with torch.no_grad():
         F.rnnt_loss(lg, tg, tl, ul, blank=0)
+# forced_align: a ragged float16 batch with int64 targets, a row without targets and padding frames
+lp_ = torch.log_softmax(torch.randn(3, 40, 7, device="cuda"), -1).half()
+tg_ = torch.randint(1, 7, (3, 12), device="cuda")
+F.forced_align(lp_, tg_, torch.tensor([40, 31, 9], device="cuda"), torch.tensor([12, 0, 4], device="cuda"))
 torch.cuda.synchronize()
 print("done")
