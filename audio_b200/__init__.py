@@ -12,7 +12,7 @@ Everything computes in hand-written CUDA kernels reached through the C ABI of
 dispatch to ``aten::stft`` / cuFFT / cuBLAS / cuDNN.
 """
 from . import _lib  # noqa: F401  (does not load the .so until first use)
-from . import compliance, functional, transforms  # noqa: F401
+from . import compliance, functional, models, transforms  # noqa: F401
 from ._plans import (differentiable, is_differentiable, is_feature_differentiable,  # noqa: F401
                      is_filtering_differentiable, is_inverse_differentiable, is_kaldi_differentiable,
                      is_resample_differentiable, is_vocoder_differentiable, set_differentiable)

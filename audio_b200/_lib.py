@@ -28,6 +28,7 @@ DTYPE_F32, DTYPE_F16, DTYPE_F64 = 0, 1, 2  # B200A_DTYPE_*
 RNNT_MAX_U = 8192  # B200A_RNNT_MAX_U
 INDEX_I32, INDEX_I64 = 0, 1  # B200A_INDEX_*
 FORCED_ALIGN_MAX_L = 8191  # B200A_FORCED_ALIGN_MAX_L
+CTC_DECODER_MAX_BEAM, CTC_DECODER_MAX_VOCAB = 128, 1 << 24  # B200A_CTC_DECODER_MAX_BEAM / _MAX_VOCAB
 
 
 class FrontendDesc(ctypes.Structure):
@@ -144,6 +145,18 @@ class ForcedAlignDesc(ctypes.Structure):
         ("dtype", c_int32),
         ("target_dtype", c_int32),
         ("length_dtype", c_int32),
+    ]
+
+
+class CtcDecoderDesc(ctypes.Structure):
+    """Mirror of ``b200a_ctc_decoder_desc``."""
+
+    _fields_ = [
+        ("batch", c_int32),
+        ("max_t", c_int32),
+        ("vocab", c_int32),
+        ("beam", c_int32),
+        ("threshold", c_float),
     ]
 
 
@@ -333,6 +346,11 @@ _SIGNATURES = {
     "b200a_forced_align_run": (
         ctypes.c_int,
         [POINTER(ForcedAlignDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+         c_void_p]),
+    "b200a_ctc_decoder_workspace_bytes": (c_size_t, [POINTER(CtcDecoderDesc)]),
+    "b200a_ctc_decoder_run": (
+        ctypes.c_int,
+        [POINTER(CtcDecoderDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
          c_void_p]),
 }
 

@@ -605,5 +605,16 @@ int b200a_forced_align_run(const b200a_forced_align_desc* desc, const void* log_
                                workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_ctc_decoder_workspace_bytes(const b200a_ctc_decoder_desc* desc) {
+  return ctc_decoder_workspace_bytes_impl(desc);
+}
+
+int b200a_ctc_decoder_run(const b200a_ctc_decoder_desc* desc, const float* log_prob, const int32_t* lengths,
+                          int32_t* tokens, int32_t* token_lengths, float* scores, int32_t* status, void* workspace,
+                          size_t workspace_bytes, b200a_stream stream) {
+  return ctc_decoder_run_impl(desc, log_prob, lengths, tokens, token_lengths, scores, status, workspace,
+                              workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -209,6 +209,11 @@ int forced_align_check_impl(const b200a_forced_align_desc* d, const void* target
 int forced_align_run_impl(const b200a_forced_align_desc* d, const void* log_probs, const void* targets,
                           const void* input_lengths, const void* target_lengths, void* paths, void* scores, void* ws,
                           size_t ws_bytes, cudaStream_t stream);
+// ctc_decoder.cu
+size_t ctc_decoder_workspace_bytes_impl(const b200a_ctc_decoder_desc* d);
+int ctc_decoder_run_impl(const b200a_ctc_decoder_desc* d, const float* log_prob, const int32_t* lengths,
+                         int32_t* tokens, int32_t* token_lengths, float* scores, int32_t* status, void* ws,
+                         size_t ws_bytes, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

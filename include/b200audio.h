@@ -790,6 +790,39 @@ int b200a_forced_align_run(const b200a_forced_align_desc* desc, const void* log_
                            const void* input_lengths, const void* target_lengths, void* paths, void* scores,
                            void* workspace, size_t workspace_bytes, b200a_stream stream);
 
+/* ---- CUDA CTC prefix beam search: cuda_ctc_decoder (models/decoder/_cuda_ctc_decoder.py, cuctc/) ------------- */
+/*
+ * The reference's CTC prefix beam search over log_prob[batch][max_t][vocab] (float32, contiguous), blank 0.  Per
+ * sequence b with T_b = lengths[b], the steps are the frames t < T_b with log_prob[b][t][0] < threshold (the log of
+ * the blank-skip threshold); candidates, merges and lse follow the reference's operation order, and among
+ * bit-equal keys the lower beam * vocab + token wins (the stay entry counts as token 0).  Outputs, best first:
+ *   tokens        : [batch][beam][max_t] int32; the first token_lengths[b][r] of each row are the hypothesis
+ *   token_lengths : [batch][beam] int32
+ *   scores        : [batch][beam] float32; a row without a selected frame has every hypothesis empty with score 0
+ *   status        : [batch] int32; 1 where lengths[b] is outside [0, max_t] (that row is not read), else 0
+ * One CTA per sequence in one launch, no atomics across CTAs: a row's result does not depend on the batch.
+ */
+/* beam cap (B200A_EINVAL above): one CTA's candidate list */
+#define B200A_CTC_DECODER_MAX_BEAM 128
+/* vocab cap (B200A_EINVAL above): beam * vocab + token in 31 bits */
+#define B200A_CTC_DECODER_MAX_VOCAB (1 << 24)
+
+typedef struct b200a_ctc_decoder_desc {
+  int32_t batch;   /* >= 1 */
+  int32_t max_t;   /* log_prob.shape[1] >= 0 */
+  int32_t vocab;   /* log_prob.shape[2], in [1, B200A_CTC_DECODER_MAX_VOCAB] */
+  int32_t beam;    /* in [1, min(vocab, B200A_CTC_DECODER_MAX_BEAM)] */
+  float threshold; /* a frame is a step when log_prob[b][t][0] < threshold; not NaN */
+} b200a_ctc_decoder_desc;
+
+/* Workspace bytes of b200a_ctc_decoder_run (selected frames and the token trie); 0 for an invalid descriptor. */
+size_t b200a_ctc_decoder_workspace_bytes(const b200a_ctc_decoder_desc* desc);
+/* B200A_EINVAL for an invalid descriptor or null pointers (log_prob and tokens may be null when max_t is 0),
+ * B200A_EWORKSPACE for a short workspace.  Nothing is read back: check status after the stream's work. */
+int b200a_ctc_decoder_run(const b200a_ctc_decoder_desc* desc, const float* log_prob, const int32_t* lengths,
+                          int32_t* tokens, int32_t* token_lengths, float* scores, int32_t* status, void* workspace,
+                          size_t workspace_bytes, b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);

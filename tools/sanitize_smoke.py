@@ -118,5 +118,10 @@ for dt, (B_, T_, U_, V_) in ((torch.float32, (3, 9, 6, 29)), (torch.float16, (2,
 lp_ = torch.log_softmax(torch.randn(3, 40, 7, device="cuda"), -1).half()
 tg_ = torch.randint(1, 7, (3, 12), device="cuda")
 F.forced_align(lp_, tg_, torch.tensor([40, 31, 9], device="cuda"), torch.tensor([12, 0, 4], device="cuda"))
+# cuda_ctc_decoder: a ragged batch with an empty row, a row that stops early and merges from a small vocabulary
+from audio_b200.models.decoder import cuda_ctc_decoder  # noqa: E402
+lp_ = torch.log_softmax(torch.randn(4, 50, 6, device="cuda") * 3, -1)
+cuda_ctc_decoder(list("abcdef"), nbest=5, beam_size=5)(lp_, torch.tensor([50, 0, 17, 1], dtype=torch.int32,
+                                                                          device="cuda"))
 torch.cuda.synchronize()
 print("done")
