@@ -29,6 +29,7 @@ RNNT_MAX_U = 8192  # B200A_RNNT_MAX_U
 INDEX_I32, INDEX_I64 = 0, 1  # B200A_INDEX_*
 FORCED_ALIGN_MAX_L = 8191  # B200A_FORCED_ALIGN_MAX_L
 CTC_DECODER_MAX_BEAM, CTC_DECODER_MAX_VOCAB = 128, 1 << 24  # B200A_CTC_DECODER_MAX_BEAM / _MAX_VOCAB
+MASK_AXIS_FREQ, MASK_AXIS_TIME = 0, 1  # B200A_MASK_AXIS_*
 
 
 class FrontendDesc(ctypes.Structure):
@@ -157,6 +158,34 @@ class CtcDecoderDesc(ctypes.Structure):
         ("vocab", c_int32),
         ("beam", c_int32),
         ("threshold", c_float),
+    ]
+
+
+class MaskSpec(ctypes.Structure):
+    """Mirror of ``b200a_mask_spec``."""
+
+    _fields_ = [
+        ("axis", c_int32),
+        ("mask_param", c_int32),
+        ("start", c_int64),
+        ("end", c_int64),
+        ("value_draws", c_void_p),
+        ("start_draws", c_void_p),
+    ]
+
+
+class MaskDesc(ctypes.Structure):
+    """Mirror of ``b200a_mask_desc``."""
+
+    _fields_ = [
+        ("rows0", c_int64),
+        ("rows1", c_int64),
+        ("freq", c_int64),
+        ("time", c_int64),
+        ("in_stride", c_int64 * 4),
+        ("out_stride", c_int64 * 4),
+        ("n_masks", c_int32),
+        ("fill", c_float),
     ]
 
 
@@ -352,6 +381,11 @@ _SIGNATURES = {
         ctypes.c_int,
         [POINTER(CtcDecoderDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
          c_void_p]),
+    "b200a_mask_workspace_bytes": (c_size_t, [POINTER(MaskDesc)]),
+    "b200a_mask_run": (
+        ctypes.c_int, [POINTER(MaskDesc), POINTER(MaskSpec), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b200a_mask_backward": (
+        ctypes.c_int, [POINTER(MaskDesc), POINTER(MaskSpec), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -616,5 +616,19 @@ int b200a_ctc_decoder_run(const b200a_ctc_decoder_desc* desc, const float* log_p
                               workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
+size_t b200a_mask_workspace_bytes(const b200a_mask_desc* desc) { return mask_workspace_bytes_impl(desc); }
+
+int b200a_mask_run(const b200a_mask_desc* desc, const b200a_mask_spec* masks, const float* in, float* out,
+                   const float* fill_ptr, void* workspace, size_t workspace_bytes, b200a_stream stream) {
+  return mask_run_impl(desc, masks, in, out, fill_ptr, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int b200a_mask_backward(const b200a_mask_desc* desc, const b200a_mask_spec* masks, const float* grad_out,
+                        float* grad_in, float* grad_fill, void* workspace, size_t workspace_bytes,
+                        b200a_stream stream) {
+  return mask_backward_impl(desc, masks, grad_out, grad_in, grad_fill, workspace, workspace_bytes,
+                            static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

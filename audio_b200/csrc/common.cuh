@@ -214,6 +214,12 @@ size_t ctc_decoder_workspace_bytes_impl(const b200a_ctc_decoder_desc* d);
 int ctc_decoder_run_impl(const b200a_ctc_decoder_desc* d, const float* log_prob, const int32_t* lengths,
                          int32_t* tokens, int32_t* token_lengths, float* scores, int32_t* status, void* ws,
                          size_t ws_bytes, cudaStream_t stream);
+// masking.cu
+size_t mask_workspace_bytes_impl(const b200a_mask_desc* d);
+int mask_run_impl(const b200a_mask_desc* d, const b200a_mask_spec* masks, const float* in, float* out,
+                  const float* fill_ptr, void* ws, size_t ws_bytes, cudaStream_t stream);
+int mask_backward_impl(const b200a_mask_desc* d, const b200a_mask_spec* masks, const float* grad_out, float* grad_in,
+                       float* grad_fill, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t istft_backward_scratch(const b200a_frontend_desc* d, int64_t rows, int64_t frames);
 int istft_backward_impl(const b200a_frontend_desc* d, const void* ws, const float* grad, int64_t rows, int64_t g_row_stride,
                         int64_t start, int64_t g_len, int64_t frames, void* scratch, float* grad_spec, cudaStream_t stream);

@@ -33,6 +33,10 @@ differentiable with respect to the logits without a switch.
 
 CTC forced alignment: ``forced_align`` (functional/_alignment.py) on the kernels of ``csrc/forced_align.cu``, batched
 with ragged lengths, bit-identical to the reference CPU per sequence; ``merge_tokens`` and ``TokenSpan`` on the host.
+
+SpecAugment masking: ``mask_along_axis_iid`` (functional.py:813-882) and ``mask_along_axis`` (885-957) on the kernel of
+``csrc/masking.cu``, with the reference's random draws, values bit for bit and output strides; differentiable with
+respect to the input and a tensor ``mask_value`` without a switch.
 """
 from __future__ import annotations
 
@@ -53,6 +57,7 @@ from ._constants import create_dct, linear_fbanks, melscale_fbanks, sinc_resampl
 from ._filtering import (allpass_biquad, band_biquad, bandpass_biquad, bandreject_biquad, bass_biquad,  # noqa: F401
                          biquad, deemph_biquad, deemphasis, equalizer_biquad, filtfilt, highpass_biquad, lfilter,
                          lowpass_biquad, preemphasis, riaa_biquad, treble_biquad, vad)
+from ._masking import mask_along_axis, mask_along_axis_iid  # noqa: F401
 from ._plans import (FrontendPlan, ResamplePlan, _no_autograd, _require_cuda_f32, _stream_ptr, _wants_grad,
                      is_feature_differentiable, is_filtering_differentiable, is_inverse_differentiable,
                      is_vocoder_differentiable, new_group_max, pack_rows, vocoder_chain)
@@ -95,6 +100,8 @@ __all__ = [
     "forced_align",
     "merge_tokens",
     "TokenSpan",
+    "mask_along_axis",
+    "mask_along_axis_iid",
 ]
 
 

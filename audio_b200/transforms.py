@@ -16,7 +16,8 @@ LFCC, AmplitudeToDB, MelScale, InverseMelScale and SpectralCentroid with ``featu
 (``audio_b200.compliance.kaldi``) with ``kaldi=True``, TimeStretch (spectrogram gradient) and PitchShift
 (waveform gradient) with ``vocoder=True``, and Preemphasis and Deemphasis (waveform gradient) and Convolve and
 FFTConvolve (input gradients) with ``filtering=True``.
-GriffinLim is forward-only.  RNNTLoss is differentiable with respect to the logits without a switch.
+GriffinLim is forward-only.  RNNTLoss is differentiable with respect to the logits without a switch, and FrequencyMasking,
+TimeMasking and SpecAugment with respect to the input and a tensor mask value.
 """
 from __future__ import annotations
 
@@ -27,14 +28,15 @@ from typing import Callable, Optional, Union
 import torch
 from torch import Tensor
 
-from . import _filtering, _lib, _ops
+from . import _filtering, _lib, _masking, _ops
 from . import functional as F
 from ._plans import (FrontendPlan, InverseMelPlan, ResamplePlan, _InverseMelFunction, _no_autograd, _require_cuda_f32,
                      _wants_grad, is_feature_differentiable, vocoder_chain)
 
 __all__ = ["Spectrogram", "InverseSpectrogram", "GriffinLim", "AmplitudeToDB", "MelScale", "InverseMelScale", "MelSpectrogram", "MFCC", "LFCC",
            "SpectralCentroid", "Resample", "Speed", "SpeedPerturbation", "TimeStretch", "PitchShift", "Preemphasis",
-           "Deemphasis", "FFTConvolve", "Convolve", "Vad", "RNNTLoss"]
+           "Deemphasis", "FFTConvolve", "Convolve", "Vad", "RNNTLoss", "FrequencyMasking", "TimeMasking",
+           "SpecAugment"]
 
 
 def _setup_framing(mod, n_fft, win_length, hop_length, window_fn=None, wkwargs=None, hop_div=2):
@@ -814,6 +816,70 @@ class RNNTLoss(torch.nn.Module):
     def forward(self, logits: Tensor, targets: Tensor, logit_lengths: Tensor, target_lengths: Tensor):
         return F.rnnt_loss(logits, targets, logit_lengths, target_lengths, self.blank, self.clamp, self.reduction,
                            self.fused_log_softmax)
+
+
+class _AxisMasking(torch.nn.Module):
+    """Masking along one axis (reference _transforms.py:1167-1206); ``axis`` counts as if the input were 3-D (1: freq,
+    2: time).  With ``iid_masks`` each example gets its own mask (:func:`audio_b200.functional.mask_along_axis_iid`),
+    otherwise one mask for all (:func:`audio_b200.functional.mask_along_axis`, a tensor ``mask_value`` read as a
+    float)."""
+
+    __constants__ = ["mask_param", "axis", "iid_masks", "p"]
+
+    def __init__(self, mask_param: int, axis: int, iid_masks: bool, p: float = 1.0) -> None:
+        super().__init__()
+        self.mask_param = mask_param
+        self.axis = axis
+        self.iid_masks = iid_masks
+        self.p = p
+
+    def forward(self, specgram: Tensor, mask_value: Union[float, torch.Tensor] = 0.0) -> Tensor:
+        axis = self.axis + specgram.dim() - 3
+        if self.iid_masks:
+            return F.mask_along_axis_iid(specgram, self.mask_param, mask_value, axis, p=self.p)
+        mask_value_ = float(mask_value) if isinstance(mask_value, Tensor) else mask_value
+        return F.mask_along_axis(specgram, self.mask_param, mask_value_, axis, p=self.p)
+
+
+class FrequencyMasking(_AxisMasking):
+    """SpecAugment frequency masking (reference _transforms.py:1209-1240)."""
+
+    def __init__(self, freq_mask_param: int, iid_masks: bool = False) -> None:
+        super().__init__(freq_mask_param, 1, iid_masks)
+
+
+class TimeMasking(_AxisMasking):
+    """SpecAugment time masking (reference _transforms.py:1243-1278)."""
+
+    def __init__(self, time_mask_param: int, iid_masks: bool = False, p: float = 1.0) -> None:
+        if not 0.0 <= p <= 1.0:
+            raise ValueError(f"The value of p must be between 0.0 and 1.0 ({p} given).")
+        super().__init__(time_mask_param, 2, iid_masks, p=p)
+
+
+class SpecAugment(torch.nn.Module):
+    """Time and frequency masking (reference _transforms.py:1281-1349): the reference's ``mean()`` fill (or 0 with
+    ``zero_masking``) and its draws in its order -- every time mask, then every frequency mask, per example when the
+    input has more than 2 dimensions and ``iid_masks`` -- then one launch for all of them.  Exact: every mask shares
+    the fill fixed before the first, so their union is the reference's sequential result."""
+
+    __constants__ = ["n_time_masks", "time_mask_param", "n_freq_masks", "freq_mask_param", "iid_masks", "p",
+                     "zero_masking"]
+
+    def __init__(self, n_time_masks: int, time_mask_param: int, n_freq_masks: int, freq_mask_param: int,
+                 iid_masks: bool = True, p: float = 1.0, zero_masking: bool = False) -> None:
+        super().__init__()
+        self.n_time_masks = n_time_masks
+        self.time_mask_param = time_mask_param
+        self.n_freq_masks = n_freq_masks
+        self.freq_mask_param = freq_mask_param
+        self.iid_masks = iid_masks
+        self.p = p
+        self.zero_masking = zero_masking
+
+    def forward(self, specgram: Tensor) -> Tensor:
+        return _masking.spec_augment(specgram, self.n_time_masks, self.time_mask_param, self.n_freq_masks,
+                                     self.freq_mask_param, self.iid_masks, self.p, self.zero_masking)
 
 
 # ---- B200A_REFERENCE=1: A/B switch to the reference implementation (debugging only, never silent) -----------------

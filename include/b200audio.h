@@ -823,6 +823,59 @@ int b200a_ctc_decoder_run(const b200a_ctc_decoder_desc* desc, const float* log_p
                           int32_t* tokens, int32_t* token_lengths, float* scores, int32_t* status, void* workspace,
                           size_t workspace_bytes, b200a_stream stream);
 
+/* ---- SpecAugment masking: mask_along_axis(_iid), FrequencyMasking, TimeMasking, SpecAugment -------------------- */
+/*
+ * out[r][f][t] = fill where (f, t) lies in any mask of row r, else in[r][f][t] bit for bit (NaNs included), over
+ * rows x freq x time float32 with 64-bit element strides; row r = r0 * rows1 + r1.  A mask covers the indices i of its
+ * axis with (float)start <= (float)i < (float)end.  Its [start, end) is either shared by every row, or per row from two
+ * uniform draws u, w (the reference's mask_along_axis_iid, in float32 without contraction):
+ *   value = u[r] * (float)mask_param,  lo = w[r] * ((float)size - value),
+ *   start = trunc(lo),  end = trunc(lo) + trunc(value)      (size: freq or time; start may be negative)
+ * All masks of one call share the fill, so their union is what sequential application of each would give.
+ * Tiles go through shared memory when the input's and the output's unit-stride axes differ, so both sides are
+ * coalesced.  No atomics: reruns are bit-identical.
+ */
+#define B200A_MASK_AXIS_FREQ 0
+#define B200A_MASK_AXIS_TIME 1
+
+typedef struct b200a_mask_spec {
+  int32_t axis;              /* B200A_MASK_AXIS_FREQ or B200A_MASK_AXIS_TIME */
+  int32_t mask_param;        /* per-row masks: the limited mask_param, >= 1; unused for a shared interval */
+  int64_t start, end;        /* the shared interval when value_draws is null */
+  const float* value_draws;  /* per-row masks: [rows] device draws u, or null for the shared interval */
+  const float* start_draws;  /* per-row masks: [rows] device draws w */
+} b200a_mask_spec;
+
+typedef struct b200a_mask_desc {
+  int64_t rows0, rows1;      /* >= 0; rows = rows0 * rows1 */
+  int64_t freq, time;        /* >= 0 */
+  int64_t in_stride[4];      /* elements, for (r0, r1, f, t) */
+  int64_t out_stride[4];
+  int32_t n_masks;           /* >= 0 */
+  float fill;                /* the fill when fill_ptr is null (b200a_mask_run) */
+} b200a_mask_desc;
+
+/* Workspace bytes of b200a_mask_run and b200a_mask_backward (the mask table and the backward's per-CTA partial
+ * sums); 0 for an invalid descriptor. */
+size_t b200a_mask_workspace_bytes(const b200a_mask_desc* desc);
+/*
+ * masks: n_masks host records, copied into the workspace on the stream (the caller may free them on return).
+ * fill_ptr: a device float32 read on the stream in place of desc->fill, or null.  B200A_EINVAL for null pointers
+ * (in and out may be null when the tensor is empty), negative sizes, a bad axis or a per-row mask with mask_param
+ * below 1 or a null start_draws; B200A_EWORKSPACE for a short workspace.
+ */
+int b200a_mask_run(const b200a_mask_desc* desc, const b200a_mask_spec* masks, const float* in, float* out,
+                   const float* fill_ptr, void* workspace, size_t workspace_bytes, b200a_stream stream);
+/*
+ * The gradient: grad_in = grad_out with every masked element 0 (desc->in_stride describes grad_out, which may have
+ * zero strides; desc->out_stride describes grad_in, which may be null when grad_fill is not).  grad_fill, when not
+ * null, receives the sum of grad_out over the masked elements: per-CTA partial sums in a fixed order, then a one-CTA
+ * fold in a fixed order, in double.  Statuses as b200a_mask_run.
+ */
+int b200a_mask_backward(const b200a_mask_desc* desc, const b200a_mask_spec* masks, const float* grad_out,
+                        float* grad_in, float* grad_fill, void* workspace, size_t workspace_bytes,
+                        b200a_stream stream);
+
 /* ---- polyphase sinc resampler ------------------------------------------------------------- */
 /* Workspace bytes for b200a_resample_prepare (per-phase tap supports + compacted taps). */
 size_t b200a_resample_workspace_bytes(int32_t new_r, int32_t taps);
